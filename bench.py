@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- POIs/sec of the FFT-CC -> IC-GN hot path (BASELINE.json metric) on N B200s.
+"""bench.py -- POIs/sec of the FFT-CC -> IC-GN hot path (BASELINE.json metric) on N H100s.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--config B|C|D|A|E|F] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--config B|C|D|A|E|F] [--impl ours|reference] [--dump-outputs DIR]
   N>1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step = one pass of the hot path (FFT-CC initial guess + IC-GN to convergence, prepare() included)
@@ -24,9 +24,12 @@ PCIe link).
            other ranks idle
   cold_start: a fresh process's ocb_create() and first calls (rank 0, N=1 only)
   roofline: dominant kernel (IC-GN) algorithmic bytes / its CUDA-event time vs MEASURED_PEAKS hbm_gbs; `traffic` and
-           `binding_resources_ncu` (issue-slot / FMA / shared-memory pipe utilisation) come from the committed ncu capture
+           `binding_resources_ncu` (issue-slot / FMA / shared-memory pipe utilisation) come from an ncu capture summarised in
+           profiles/traffic.json, when there is one (null otherwise)
   cpu_baseline: the oracle port of the reference (oracle/, g++ -O3 -fopenmp, nproc-1 threads like
            the reference examples) timed on this box's host cores on the same workload
+  --dump-outputs DIR: rank 0's POI records after the last timed device-resident step, DIR/pois.npy (float32); the inputs
+           are seeded, so two builds run with the same arguments can be compared record for record
 
 --impl reference times the reference's own CPU implementation of the path (here: the oracle port,
 because the reference cannot be compiled without Eigen/FFTW/OpenCV -- DESIGN.md) on the same config.
@@ -69,7 +72,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def make_workload(cfg_name, rank, world, device=None):
@@ -389,6 +392,22 @@ def bind_to_gpu_numa_node(index):
         return "not bound (%s)" % str(e)[:80]
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, pois):
+    """--dump-outputs: the POI records the last timed step returned (float32 [n, 25] 2D / [n, 31] 3D, OpenCorr's POI2D / POI3D
+    layout) as out_dir/pois.npy.  A queue larger than 64 MiB is cut to a fixed, seeded sample of rows, whose indices go to
+    out_dir/poi_index.npy (float64), so that two builds can be compared record for record."""
+    os.makedirs(out_dir, exist_ok=True)
+    if pois.nbytes > DUMP_LIMIT_BYTES:
+        keep = DUMP_LIMIT_BYTES // pois[0].nbytes
+        idx = np.sort(np.random.default_rng(0).choice(len(pois), keep, replace=False))
+        pois = pois[idx]
+        np.save(os.path.join(out_dir, "poi_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "pois.npy"), np.ascontiguousarray(pois, dtype=np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -432,7 +451,7 @@ def run_ours(args):
         eng.set_images_2d_dev(d_ref.data_ptr(), d_tar.data_ptr(), ref.shape[1], ref.shape[0])
     else:
         eng.set_images_3d_dev(d_ref.data_ptr(), d_tar.data_ptr(), ref.shape[2], ref.shape[1], ref.shape[0])
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # 256 MiB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # 256 MiB > the 50 MB L2
 
     def step_resident(ev=None):
         d_q.copy_(d_q0)
@@ -489,6 +508,8 @@ def run_ours(args):
 
     # iteration histogram / sanity of the last step
     res = d_q.cpu().numpy()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res)
     zc, ic = (16, 17) if kind == "2d" else (18, 19)
     good = res[:, zc] >= 0
     hist = np.bincount(res[good, ic].astype(np.int64), minlength=int(cfg["stop"]) + 1).tolist()
@@ -728,6 +749,7 @@ def main():
     ap.add_argument("--cpu-sample", type=int, default=0, help="POIs per step for --impl reference (0 = default)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the rank-0 extras (e2e_shim, capi_multi, cold_start)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write rank 0's POI records of the last timed step to DIR/pois.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

@@ -1,5 +1,5 @@
 // dic_fftcc_icgn1_demo.cpp -- path-independent 2D DIC (FFT-CC initial guess + IC-GN, first-order
-// shape function) on the B200 engine through the OpenCorr-compatible C++ shim.
+// shape function) on the H100 engine through the OpenCorr-compatible C++ shim.
 // Usage: dic_fftcc_icgn1_demo <ref.bmp> <tar.bmp> <out.csv> [radius=16] [grid_step=2]
 #include <chrono>
 #include <iostream>

@@ -1,6 +1,6 @@
 /*
  * opencorr.h -- API-compatible C++ shim for the FFT-CC -> IC-GN path of OpenCorr, running on the
- * B200 engine behind include/opencorr_b200.h.  Header-only; link with -lopencorr_b200.
+ * H100 engine behind include/opencorr_b200.h.  Header-only; link with -lopencorr_b200.
  *
  * It re-declares (same names, same signatures, same public members, same POI record layout) the
  * part of the reference's `namespace opencorr` that examples/test_2d_dic_fftcc_icgn1.cpp and

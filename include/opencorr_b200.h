@@ -1,5 +1,5 @@
 /*
- * opencorr_b200.h -- C ABI of the B200-native FFT-CC -> IC-GN correlation engine.
+ * opencorr_b200.h -- C ABI of the H100-native (sm_90a) FFT-CC -> IC-GN correlation engine.
  *
  * This is the drop-in boundary for ONE hot path of vincentjzy/OpenCorr: the per-POI
  * FFT-CC integer-pixel initial guess followed by inverse-compositional Gauss-Newton

@@ -1,4 +1,4 @@
-"""opencorr_b200 -- B200-native (sm_100a) FFT-CC -> IC-GN correlation engine behind OpenCorr's API.
+"""opencorr_b200 -- H100-native (sm_90a) FFT-CC -> IC-GN correlation engine behind OpenCorr's API.
 
 Only the hot path of vincentjzy/OpenCorr is implemented: FFTCC2D/FFTCC3D and
 ICGN2D1/ICGN2D2/ICGN3D1.  The compute lives in opencorr_b200/csrc (CUDA) behind the C ABI of

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI in include/opencorr_b200.h (libopencorr_b200.so).
 
-The library is hand-written CUDA for sm_100a; there is no CPU path.  Loading works without a
+The library is hand-written CUDA for sm_90a; there is no CPU path.  Loading works without a
 GPU (so the symbol table can be checked), but ocb_create() fails loudly.
 """
 import ctypes

@@ -58,7 +58,7 @@ def _check_queue(q, floats):
 class Engine:
     """One GPU context (ocb_ctx), or a GROUP context over several devices: device = -1 / "all" (every visible device) or a
     list of device indices -- host-queue calls then shard the queue over the devices inside the C ABI (one process, G
-    devices; include/opencorr_b200.h ocb_create_multi).  Raises OpenCorrB200Error when no B200-class GPU is usable."""
+    devices; include/opencorr_b200.h ocb_create_multi).  Raises OpenCorrB200Error when no H100-class (sm_90) GPU is usable."""
 
     def __init__(self, device=0):
         self._lib = _capi.load()

@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library in-tree: opencorr_b200/lib/libopencorr_b200.so.
+"""Build the sm_90a shared library in-tree: opencorr_b200/lib/libopencorr_b200.so.
 
 nvcc cross-compiles without a GPU.  The library is a plain C-ABI .so (static cudart, no torch).
 """
@@ -10,8 +10,8 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_DIR = os.path.join(_HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libopencorr_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-              "-shared", "-Xcompiler", "-fPIC"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
+NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC"]
 
 
 def _nvcc():
@@ -42,11 +42,11 @@ def _compile(nvcc, flags, src, obj):
 
 
 def build(force=False, verbose=False, variant=None, variant_flags=(), variant_sources=()):
-    """Compile every CUDA source for sm_100a into one shared library (objects in parallel, then one link).  Objects are kept
+    """Compile every CUDA source for sm_90a into one shared library (objects in parallel, then one link).  Objects are kept
     under lib/obj/ so that only stale sources are recompiled.
 
     variant: build lib/variants/<variant>.so instead (A/B experiments, selected at run time with OCB_LIB_PATH): the
-    sources named in variant_sources are compiled with variant_flags added (e.g. -DICGN2D_PAIRS=0), the rest is linked
+    sources named in variant_sources are compiled with variant_flags added (e.g. -DICGN2D_PAIRS=1), the rest is linked
     from the regular objects."""
     if variant is None and not force and not is_stale():
         return LIB_PATH
@@ -82,7 +82,7 @@ def build(force=False, verbose=False, variant=None, variant_flags=(), variant_so
     if variant is not None:
         os.makedirs(os.path.join(LIB_DIR, "variants"), exist_ok=True)
         out = os.path.join(LIB_DIR, "variants", variant + ".so")
-    subprocess.check_call(nvcc + ["-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-Xcompiler", "-fPIC", "-o", out] + objs)
+    subprocess.check_call(nvcc + GENCODE + ["-shared", "-Xcompiler", "-fPIC", "-o", out] + objs)
     return out
 
 

@@ -1,4 +1,4 @@
-// epipolar.cu -- the candidate sweep of EpipolarSearch as ONE batch (SURVEY.md section 8(f) N4), for sm_100a.
+// epipolar.cu -- the candidate sweep of EpipolarSearch as ONE batch (SURVEY.md section 8(f) N4), for sm_90a.
 //
 // Replaces EpipolarSearch::compute(POI2D*) (reference src/oc_epipolar_search.cpp:133-195), which for every POI of
 // the primary view spawns ~2*radius/step candidate POIs along its epipolar line in the secondary view, runs

@@ -48,45 +48,59 @@ __device__ __forceinline__ void mul_tw32(float xr, float xi, int k, float& yr, f
 	}
 }
 
+// One radix-2 stage with butterflies `HALF` apart.  HALF is a template argument so that every loop below has a
+// compile-time trip count and is unrolled completely (re/im then stay in registers instead of local memory).
+template <bool INV, int HALF>
+__device__ __forceinline__ void fft32_dif_stage(float* re, float* im) {
+#pragma unroll
+	for (int base = 0; base < 32; base += 2 * HALF) {
+#pragma unroll
+		for (int k = 0; k < HALF; k++) {
+			const int i = base + k, j = i + HALF;
+			const float ar = re[i], ai = im[i], br = re[j], bi = im[j];
+			re[i] = ar + br;
+			im[i] = ai + bi;
+			mul_tw32<INV>(ar - br, ai - bi, k * (16 / HALF), re[j], im[j]);
+		}
+	}
+}
+
+template <bool INV, int HALF>
+__device__ __forceinline__ void fft32_dit_stage(float* re, float* im) {
+#pragma unroll
+	for (int base = 0; base < 32; base += 2 * HALF) {
+#pragma unroll
+		for (int k = 0; k < HALF; k++) {
+			const int i = base + k, j = i + HALF;
+			float tr, ti;
+			mul_tw32<INV>(re[j], im[j], k * (16 / HALF), tr, ti);
+			const float ar = re[i], ai = im[i];
+			re[i] = ar + tr;
+			im[i] = ai + ti;
+			re[j] = ar - tr;
+			im[j] = ai - ti;
+		}
+	}
+}
+
 // radix-2 decimation in frequency: natural order in, bit-reversed order out
 template <bool INV>
 __device__ __forceinline__ void fft32_dif(float* re, float* im) {
-#pragma unroll
-	for (int half = 16; half >= 1; half >>= 1) {
-#pragma unroll
-		for (int base = 0; base < 32; base += 2 * half) {
-#pragma unroll
-			for (int k = 0; k < half; k++) {
-				const int i = base + k, j = i + half;
-				const float ar = re[i], ai = im[i], br = re[j], bi = im[j];
-				re[i] = ar + br;
-				im[i] = ai + bi;
-				mul_tw32<INV>(ar - br, ai - bi, k * (16 / half), re[j], im[j]);
-			}
-		}
-	}
+	fft32_dif_stage<INV, 16>(re, im);
+	fft32_dif_stage<INV, 8>(re, im);
+	fft32_dif_stage<INV, 4>(re, im);
+	fft32_dif_stage<INV, 2>(re, im);
+	fft32_dif_stage<INV, 1>(re, im);
 }
 
 // radix-2 decimation in time: bit-reversed order in, natural order out
 template <bool INV>
 __device__ __forceinline__ void fft32_dit(float* re, float* im) {
-#pragma unroll
-	for (int half = 1; half <= 16; half <<= 1) {
-#pragma unroll
-		for (int base = 0; base < 32; base += 2 * half) {
-#pragma unroll
-			for (int k = 0; k < half; k++) {
-				const int i = base + k, j = i + half;
-				float tr, ti;
-				mul_tw32<INV>(re[j], im[j], k * (16 / half), tr, ti);
-				const float ar = re[i], ai = im[i];
-				re[i] = ar + tr;
-				im[i] = ai + ti;
-				re[j] = ar - tr;
-				im[j] = ai - ti;
-			}
-		}
-	}
+	fft32_dit_stage<INV, 1>(re, im);
+	fft32_dit_stage<INV, 2>(re, im);
+	fft32_dit_stage<INV, 4>(re, im);
+	fft32_dit_stage<INV, 8>(re, im);
+	fft32_dit_stage<INV, 16>(re, im);
 }
 
 __device__ __forceinline__ void cross32(float zr, float zi, float nr, float ni, float& cr, float& ci) {

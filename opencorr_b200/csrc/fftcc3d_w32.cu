@@ -12,7 +12,8 @@
 //            C = conj(A) B; DIT inverse FFT along kz; back to S.
 //   phase C: warp per z-slice: DIT inverse along kx, transpose, DIT inverse along ky, running
 //            first-maximum argmax (linear index (z*32 + y)*32 + x).
-// The scratch volume (256 KB per CTA, 2 CTAs per SM -> 76 MB) stays L2-resident.
+// The scratch volume is 256 KB per CTA; with FFTCC3D_W32_CTAS_PER_SM CTAs on each of the H100's 132 SMs that is 66 MB (2, the
+// default) or 33 MB (1) against the 50 MB L2 -- see DESIGN.md section 5 for the measured choice.
 // Phase A's slice loads go through TMA when the POI and its guess sit on whole voxels and the volume pitch allows it: one
 // cp.async.bulk.tensor.3d box of 36 x 32 x 1 floats per window and slice (x origin rounded down to 16 bytes), straight into the
 // warp's two transpose tiles, completion on a per-warp mbarrier; otherwise the lanes gather their columns (the reference's
@@ -27,6 +28,9 @@
 namespace ocb {
 
 constexpr int F3_WARPS = 8;
+#ifndef FFTCC3D_W32_CTAS_PER_SM
+#define FFTCC3D_W32_CTAS_PER_SM 2
+#endif
 constexpr int F3_PITCH = 33;
 constexpr int F3_BOX_W = 36;              // TMA box: 32 columns + up to 3 of alignment slack
 constexpr int F3_TILE = 32 * F3_BOX_W;    // floats per tile: a TMA box (36 x 32) or a padded transpose tile (32 x 33)
@@ -271,7 +275,7 @@ __global__ void __launch_bounds__(F3_WARPS * 32, 2) fftcc3d_w32_kernel(Image3D i
 	}
 }
 
-int fftcc3d_w32_grid(int sm_count) { return sm_count * 2; }
+int fftcc3d_w32_grid(int sm_count) { return sm_count * FFTCC3D_W32_CTAS_PER_SM; }
 
 int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err) {
 	if ((long long)grid > (long long)n) grid = (int)n;

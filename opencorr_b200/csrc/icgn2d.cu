@@ -1,15 +1,14 @@
 // icgn2d.cu -- inverse-compositional Gauss-Newton subset registration, 2D, first-order (6
-// parameters) and second-order (12 parameters) shape functions, for sm_100a.
+// parameters) and second-order (12 parameters) shape functions, for sm_90a.
 //
 // Replaces ICGN2D1::compute(POI2D*) (reference src/oc_icgn.cpp:144-341) and
 // ICGN2D2::compute(POI2D*) (src/oc_icgn.cpp:685-898), including what ICGN2D*::prepare() feeds
 // them (Gradient2D4, src/oc_gradient.cpp:37-79; BicubicBspline, src/oc_cubic_bspline.cpp:84-181).
 //
-// Round-2 structure in one paragraph: the setup pass and the sampling loop take TWO subset rows per lane and step in packed
-// f32x2 arithmetic (ICGN2D_PAIRS), and in the Tensor-Memory variant (template flag TM: wide-enough subsets, queues that fill the
-// GPU) a lane's per-sample constants live in its own TMEM lane instead of shared memory, which lifts the resident warps per SM
-// from 11 to 16 at r = 16.  The reference's `any sample < 0` rejection is re-decided in the reference's own arithmetic when the
-// smallest sample is borderline (icgn2d_exact_negative).  What follows describes the common skeleton.
+// Structure in one paragraph: the setup pass and the sampling loop take one subset row per lane and step (two as float2
+// pairs with ICGN2D_PAIRS=1), and a lane's per-sample constants live in shared memory.  The reference's `any sample < 0` rejection is
+// re-decided in the reference's own arithmetic when the smallest sample is borderline (icgn2d_exact_negative).  What follows
+// describes the common skeleton.
 //
 // Mapping: ONE WARP PER POI, persistent warps pulling POIs from an atomic counter, no CTA barrier.
 // Lanes run along x: lane c owns column c of the subset for every row (columns >= 32 are a short
@@ -37,23 +36,24 @@
 #include "ocb_tma.cuh"
 #include "ocb_f32x2.cuh"
 #include "ocb_tile2d.cuh"
-#include "ocb_tmem.cuh"
 
 namespace ocb {
 
 #ifndef ICGN2D_PAIRS
-// 1: the fast sampling loop takes TWO subset rows per lane and step and does their arithmetic in packed f32x2 pairs
-// (FFMA2 / FMUL2 / FADD2, ocb_f32x2.cuh) -- position, bicubic weights, taps and all sums of rows r and r + 1 go through ONE
-// instruction per pair, and the two 4x4 pixel blocks, which overlap in three rows, are fetched as one 4x5 block (20 LDS
-// instead of 32).  The two rows are independent, so unlike packing WITHIN one sample (tried in round 1: 10 % slower)
-// no dependency chain gets longer.  0: one row per step, scalar arithmetic (the round-1 loop), kept for A/B runs.
-#define ICGN2D_PAIRS 1
+// 1: the fast sampling loop takes TWO subset rows per lane and step and does their arithmetic as float2 pairs
+// (ocb_f32x2.cuh) -- position, bicubic weights, taps and all sums of rows r and r + 1 go through ONE
+// call per pair, and the two 4x4 pixel blocks, which overlap in three rows, are fetched as one 4x5 block (20 LDS
+// instead of 32).  It was written for packed fp32 instructions, which sm_90 lacks (each pair is two scalar operations
+// here); on the H100 it is no faster for the 6-parameter kernels and slower for the 12-parameter ones (DESIGN.md
+// section 5), so it is built only on request (-DICGN2D_PAIRS=1, A/B runs).
+// 0: one row per step, scalar arithmetic (the default).
+#define ICGN2D_PAIRS 0
 #endif
 #ifndef ICGN2D_PAIR_UNROLL
 #define ICGN2D_PAIR_UNROLL 2 // row pairs in flight per lane
 #endif
 #ifndef ICGN2D_MINB
-#define ICGN2D_MINB 16 // resident one-warp CTAs the 6-parameter kernels' register budget is sized for (16 -> 128 registers; measured best of 11/16/20)
+#define ICGN2D_MINB 16 // resident one-warp CTAs the 6-parameter kernels' register budget is sized for (16 -> 128 registers)
 #endif
 #ifndef ICGN2D_UNROLL
 #define ICGN2D_UNROLL 3
@@ -61,11 +61,11 @@ namespace ocb {
 constexpr int ICGN2D_ROW_UNROLL = ICGN2D_UNROLL; // rows of the fast sampling loop in flight per lane
 constexpr int ICGN2D_PAIR_UNROLL_N = ICGN2D_PAIR_UNROLL;
 #ifndef ICGN2D_SETUP_UNROLL
-#define ICGN2D_SETUP_UNROLL 3 // row pairs of the setup pass in flight per lane (1 / 2 / 3: 0.651 / 0.647 / 0.641 ms on config B)
+#define ICGN2D_SETUP_UNROLL 3 // row pairs of the setup pass in flight per lane
 #endif
 constexpr int ICGN2D_SETUP_UNROLL_N = ICGN2D_SETUP_UNROLL;
 constexpr int ICGN2D_TILE_MARGIN = 1; // slack (pixels) around subset+support in the target tile
-// TMA tile loads need the innermost coordinate 16-byte aligned (x multiple of 4 floats; measured: an
+// TMA tile loads need the innermost coordinate 16-byte aligned (x multiple of 4 floats; seen: an
 // unaligned x raises 'illegal instruction'), so tile origins are rounded down to a multiple of 4 and
 // the boxes are 3 columns wider.
 
@@ -82,14 +82,6 @@ __host__ __device__ inline int icgn2d_tile_floats(int rx, int ry) {
 // wpp > 1 (warps per POI): a reduction area follows -- wpp x 96 floats of setup partials, 2 x wpp x 32 floats of
 // per-iteration partials (double-buffered by iteration parity)
 constexpr int ICGN2D_RED_SETUP = 96, ICGN2D_RED_ITER = 32;
-// TM variant (below): four independent warps per CTA; the {R, gx, gy} constants of the 32 row-mapped columns live in Tensor Memory
-// (3 columns per subset row in the warp's quarter of the 128 TMEM lanes), only the tile and the tail columns' constants in smem
-constexpr int ICGN2D_TM_WARPS = 4, ICGN2D_TM_COLS = 128;
-__host__ __device__ inline int icgn2d_tm_slab_floats(int rx, int ry) {
-	const int rem = (2 * rx + 1) - 32;
-	return 32 + icgn2d_tile_floats(rx, ry) + round_up32(3 * (rem > 0 ? rem : 0) * (2 * ry + 1));
-}
-__host__ inline bool icgn2d_tm_supported(int rx, int ry) { return 2 * rx + 1 >= 32 && 3 * (2 * ry + 1) <= ICGN2D_TM_COLS; }
 __host__ __device__ inline int icgn2d_slab_floats(int rx, int ry, bool lm, int wpp) {
 	const int n = (2 * rx + 1) * (2 * ry + 1);
 	return 32 + icgn2d_tile_floats(rx, ry) + round_up32(3 * n) + (lm ? 96 : 0) + (wpp > 1 ? wpp * (ICGN2D_RED_SETUP + 2 * ICGN2D_RED_ITER) : 0);
@@ -297,13 +289,8 @@ __device__ __noinline__ bool icgn2d_exact_negative(const float* Aw, float pcx, f
 // of 11), which is what the latency-bound row loops need.
 // (the second launch bound keeps the register file from limiting residency below what the slab allows: 16 one-warp CTAs for the
 //  6-parameter kernels of any radius, 12 for the r = 16 specialisation, whose 20 KB slab admits 11)
-// TM: Tensor-Memory variant (WPP == 1, not LM, subset at least 32 columns wide, at most 42 rows).  A CTA is four warps, each
-// registering its own POIs exactly like a one-warp CTA; what changes is where a lane keeps the constants of its subset column:
-// in its own TMEM lane (tcgen05.st in the setup pass, tcgen05.ld in every iteration) instead of 13 of the 20 KB of shared
-// memory per warp.  Shared memory then holds 16 warps per SM instead of 11, and the constants of a row pair come back as the
-// register pairs the packed loop wants.  TMEM: 128 columns per CTA, 4 CTAs per SM = all 512 columns.
-template <int NP, int RC, bool LM, int WPP, bool TM = false>
-__global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP == 6 ? 4 : 1) : (NP == 6 ? (RC == 16 ? 12 : ICGN2D_MINB) / WPP : 7)) icgn2d_kernel(Image2D img, float* __restrict__ pois, int n_poi, int rx_arg, int ry_arg,
+template <int NP, int RC, bool LM, int WPP>
+__global__ void __launch_bounds__(32 * WPP, NP == 6 ? (RC == 16 ? 12 : ICGN2D_MINB) / WPP : 7) icgn2d_kernel(Image2D img, float* __restrict__ pois, int n_poi, int rx_arg, int ry_arg,
 	float conv_criterion, float stop_condition, int* __restrict__ work_counter, const __grid_constant__ CUtensorMap tm_ref,
 	const __grid_constant__ CUtensorMap tm_tar, int use_tma, const float* __restrict__ center_offsets, float lm_lambda, float lm_alpha,
 	float lm_beta) {
@@ -315,10 +302,8 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 	constexpr int NM = (D2 + 1) * (D2 + 2) / 2; // monomials x^P y^Q with P+Q <= 2*DEG: 6 or 15
 	const int rx = RC ? RC : rx_arg, ry = RC ? RC : ry_arg;
 	const int lane = threadIdx.x & 31;
-	static_assert(!TM || (WPP == 1 && !LM), "the Tensor-Memory variant is one warp per POI, plain IC-GN");
 	const int sub = WPP > 1 ? (int)(threadIdx.x >> 5) : 0; // this warp's share of the POI
-	const int warp_in_cta = (int)(threadIdx.x >> 5);
-	const bool poi_leader = TM ? lane == 0 : threadIdx.x == 0; // the thread that speaks for the POI (TMA issue, single stores)
+	const bool poi_leader = threadIdx.x == 0; // the thread that speaks for the POI (TMA issue, single stores)
 	const int sw = 2 * rx + 1, sh = 2 * ry + 1, N = sw * sh;
 	const int rows_per = (sh + WPP - 1) / WPP;
 	const int r_lo = sub * rows_per, r_hi = (r_lo + rows_per) < sh ? (r_lo + rows_per) : sh; // rows [r_lo, r_hi) belong to this warp
@@ -327,11 +312,11 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 	const int ntail = rem * sh;
 	const int RW = icgn2d_ref_w(rx), RH = icgn2d_ref_h(ry);
 	const int TW = icgn2d_tar_w(rx), TH = icgn2d_tar_h(ry);
-	float* slab = TM ? smem + warp_in_cta * icgn2d_tm_slab_floats(rx, ry) : smem;
+	float* slab = smem;
 	uint64_t* bar = (uint64_t*)slab;
 	int* s_poi = (int*)(slab + 8);              // WPP > 1: the POI index fetched by thread 0
 	float* T = slab + 32;
-	float* sC = T + icgn2d_tile_floats(rx, ry); // per-sample constants, interleaved {R, gx, gy} (12-byte lane stride: conflict-free); TM: tail columns only
+	float* sC = T + icgn2d_tile_floats(rx, ry); // per-sample constants, interleaved {R, gx, gy} (12-byte lane stride: conflict-free)
 	float* sH = sC + round_up32(3 * N);         // LM only: the undamped Hessian, packed lower triangle
 	float* sRedS = sH + (LM ? 96 : 0);          // WPP > 1: setup partials [WPP][ICGN2D_RED_SETUP]
 	float* sRedI = sRedS + WPP * ICGN2D_RED_SETUP; // WPP > 1: iteration partials [2][WPP][ICGN2D_RED_ITER]
@@ -344,26 +329,6 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 		if (poi_leader) mbar_init(bar, 1);
 		gsync();
 	}
-	// TM: the CTA's Tensor-Memory columns; a lane's constants of subset rows (2p, 2p+1) sit in columns 6p .. 6p+5 of its TMEM lane
-	// as {R_a, R_b, gx_a, gx_b, gy_a, gy_b}, those of a last single row in 6p .. 6p+2
-	uint32_t tm_base = 0, s_tmem_base_value = 0;
-	if constexpr (TM) {
-		__shared__ uint32_t s_tmem_base;
-		if (warp_in_cta == 0) tmem_alloc<ICGN2D_TM_COLS>(&s_tmem_base);
-		tmem_fence_before_sync();
-		__syncthreads();
-		tmem_fence_after_sync();
-		s_tmem_base_value = s_tmem_base;
-		tm_base = tmem_warp_base(s_tmem_base_value, warp_in_cta);
-	}
-	// the constants of tail column c >= 32 at row r (smem in both variants)
-	auto tail_consts = [&](int r, int c) -> float* { return TM ? sC + 3 * (r * rem + (c - 32)) : sC + 3 * (r * sw + c); };
-	// TM: single-row access to a lane's constants (column of R; gx and gy follow at +stride, +2 stride)
-	auto tm_row = [&](int r, int& stride) -> uint32_t {
-		const bool single = (sh & 1) && r == sh - 1;
-		stride = single ? 1 : 2;
-		return tm_base + (single ? 3 * r : 6 * (r >> 1) + (r & 1));
-	};
 	const float* __restrict__ ref = img.ref;
 	const float* __restrict__ tar = img.tar;
 	const int w = img.w, h = img.h;
@@ -493,10 +458,7 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 					if (!gx_ok) gx2 = make_float2(0.f, 0.f);
 					if (!(yg >= 2 && yg < h - 2)) gy2.x = 0.f;
 					if (!(yg + 1 >= 2 && yg + 1 < h - 2)) gy2.y = 0.f;
-					if constexpr (TM) {
-						tmem_st4(tm_base + 3 * r, v2, v3, gx2.x, gx2.y);
-						tmem_st2(tm_base + 3 * r + 4, gy2.x, gy2.y);
-					} else {
+					{
 						float* pc = sC + 3 * (r * sw + lane);
 						pc[0] = v2; pc[1] = gx2.x; pc[2] = gy2.x;
 						pc[3 * sw] = v3; pc[3 * sw + 1] = gx2.y; pc[3 * sw + 2] = gy2.y;
@@ -548,13 +510,7 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 					float gx = 0.f, gy = 0.f;
 					if (gx_ok) gx = grad4(q[-2], q[-1], q[1], q[2]);
 					if (gy_ok) gy = grad4(q[-2 * RW], q[-RW], q[RW], q[2 * RW]);
-					if constexpr (TM) { // (every lane is on in this variant: the stores are warp-convergent)
-						int st;
-						const uint32_t ta = tm_row(r, st);
-						tmem_st1(ta, q[0]);
-						tmem_st1(ta + st, gx);
-						tmem_st1(ta + 2 * st, gy);
-					} else {
+					{
 						float* pc = sC + 3 * (r * sw + lane);
 						pc[0] = q[0]; // raw R
 						pc[1] = gx;
@@ -619,7 +575,7 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 			float gx = 0.f, gy = 0.f;
 			if (xg >= 2 && xg < w - 2) gx = grad4(q[-2], q[-1], q[1], q[2]);
 			if (yg >= 2 && yg < h - 2) gy = grad4(q[-2 * RW], q[-RW], q[RW], q[2 * RW]);
-			float* pc = tail_consts(r, c);
+			float* pc = sC + 3 * (r * sw + c);
 			pc[0] = q[0];
 			pc[1] = gx;
 			pc[2] = gy;
@@ -730,7 +686,6 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 		}
 		float lm_cur = 0.f, znssd0 = 4.f; // src/oc_iclm.cpp:234-235
 
-		if constexpr (TM) tmem_wait_st(); // the setup pass's constants are in Tensor Memory before the first iteration reads them
 		// ---------------- stage the target tile over the reference tile ----------------
 		// (WPP > 1: the barrier of the setup reduction already ordered every warp's last read of the reference tile)
 		if constexpr (WPP == 1) __syncwarp();
@@ -848,14 +803,8 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 					constexpr float BE[4] = { 0.f, 1.f, 0.f, 0.f };
 					float2 yl2 = make_float2(yl, yl + 1.f);
 					const int npair = (r_hi - r_lo) >> 1;
-#pragma unroll (TM ? 1 : ICGN2D_PAIR_UNROLL_N) // (16 resident warps need less unrolling than 11: measured 0.647 vs 0.653 ms on config B)
+#pragma unroll ICGN2D_PAIR_UNROLL_N
 					for (int pr = 0; pr < npair; pr++) {
-						float2 R2c, gx2c, gy2c; // the two rows' constants
-						if constexpr (TM) { // requested now, needed after the taps
-							const uint32_t ta = tm_base + 3 * (r_lo + 2 * pr);
-							tmem_ld4(ta, R2c.x, R2c.y, gx2c.x, gx2c.y);
-							tmem_ld2(ta + 4, gy2c.x, gy2c.y);
-						}
 						float2 X2, Y2;
 						if constexpr (NP == 6) {
 							X2 = fadd2(pcx2, ffma2(xs1p, yl2, xs0p));
@@ -896,9 +845,7 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 						// breaks that (a few lanes per POI), its sample is evaluated on its own
 						if (xfb != xfa || yfb != yfa + 1.f) t2.y = bicubic_sample(T, TW, tx0, ty0, tar, w, X2.y, Y2.y, true);
 						tmin = fminf(tmin, fminf(t2.x, t2.y));
-						if constexpr (TM) tmem_wait_ld();
-						else { R2c = make_float2(pc[0], pc[3 * sw]); gx2c = make_float2(pc[1], pc[3 * sw + 1]); gy2c = make_float2(pc[2], pc[3 * sw + 2]); }
-						const float2 R2 = R2c;
+						const float2 R2 = make_float2(pc[0], pc[3 * sw]), gx2c = make_float2(pc[1], pc[3 * sw + 1]), gy2c = make_float2(pc[2], pc[3 * sw + 2]);
 						float2 dd = fsub2(t2, R2);
 						if (!lane_on) dd = make_float2(0.f, 0.f);
 						d1p = fadd2(d1p, dd);
@@ -950,17 +897,7 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 						t = fmaf(row, wy[nn], t);
 					}
 					tmin = fminf(tmin, t);
-					float R, gxc, gyc;
-					if constexpr (TM) {
-						int st;
-						const uint32_t ta = tm_row(r, st);
-						R = tmem_ld1(ta);
-						gxc = tmem_ld1(ta + st);
-						gyc = tmem_ld1(ta + 2 * st);
-						tmem_wait_ld();
-					} else {
-						R = pc[0]; gxc = pc[1]; gyc = pc[2];
-					}
+					const float R = pc[0], gxc = pc[1], gyc = pc[2];
 					const float d = lane_on ? t - R : 0.f;
 					d1 += d;
 					d2 = fmaf(d, d, d2);
@@ -989,15 +926,6 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 						X = pcx + fmaf(fmaf(ax2, yl, ax1), yl, ax0);
 						Y = pcy + fmaf(fmaf(ay2, yl, ay1), yl, ay0);
 					}
-					float Rt = 0.f, gxt = 0.f, gyt = 0.f;
-					if constexpr (TM) { // warp-convergent: before the per-lane branches
-						int st;
-						const uint32_t ta = tm_row(r, st);
-						Rt = tmem_ld1(ta);
-						gxt = tmem_ld1(ta + st);
-						gyt = tmem_ld1(ta + 2 * st);
-						tmem_wait_ld();
-					}
 					if (lane_on) {
 						const bool fast = (X >= xlo) && (X < xhi) && (Y >= ylo) && (Y < yhi);
 						const bool ok = fast || ((X >= 1.f) && (Y >= 1.f) && (X < xmax) && (Y < ymax)); // NaN fails
@@ -1006,11 +934,8 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 						} else {
 							const float t = ok ? bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, fast) : -1.f; // BicubicBspline::compute returns -1 outside
 							tmin = fminf(tmin, t);
-							if constexpr (!TM) {
-								const float* pc = sC + 3 * (r * sw + lane);
-								Rt = pc[0]; gxt = pc[1]; gyt = pc[2];
-							}
-							const float R = Rt;
+							const float* pc = sC + 3 * (r * sw + lane);
+							const float R = pc[0], gxt = pc[1], gyt = pc[2];
 							const float d = t - R;
 							d1 += d;
 							d2 = fmaf(d, d, d2);
@@ -1059,7 +984,7 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 				} else {
 					const float t = ok ? bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, fast) : -1.f;
 					tmin = fminf(tmin, t);
-					const float* pc = tail_consts(r, c);
+					const float* pc = sC + 3 * (r * sw + c);
 					const float R = pc[0];
 					const float d = t - R;
 					d1 += d;
@@ -1191,7 +1116,7 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 		// Every lane holds the same final state; the record goes out as ONE coalesced store, lane k writing float k (fields the
 		// reference leaves alone keep the value read at the start) -- the queue may live in page-locked host memory, where
 		// separate 4-byte stores would each cross PCIe on their own.
-		if (TM || threadIdx.x < 32) {
+		if (threadIdx.x < 32) {
 			float u, v;
 			float out = rec;
 			auto put = [&](int field, float value) { if (lane == field) out = value; };
@@ -1228,18 +1153,13 @@ __global__ void __launch_bounds__(TM ? 32 * ICGN2D_TM_WARPS : 32 * WPP, TM ? (NP
 		// The queue head resets itself: the last worker to leave zeroes it (and the departure count 8 ints further on), so a
 		// launch needs no memset in front of it (2-3 us of an otherwise empty stream per launch).  The host zeroes both once.
 		if (lane == 0) {
-			const int workers = (int)gridDim.x * (TM ? ICGN2D_TM_WARPS : 1);
+			const int workers = (int)gridDim.x;
 			__threadfence();
 			if (atomicAdd(work_counter + 8, 1) == workers - 1) {
 				work_counter[0] = 0;
 				work_counter[8] = 0;
 			}
 		}
-	}
-	if constexpr (TM) { // every warp has drained the queue: release the CTA's Tensor-Memory columns
-		tmem_fence_before_sync();
-		__syncthreads();
-		if (warp_in_cta == 0) tmem_dealloc<ICGN2D_TM_COLS>(s_tmem_base_value);
 	}
 }
 
@@ -1261,10 +1181,9 @@ size_t icgn2d_slab_bytes(int rx, int ry) { return (size_t)icgn2d_slab_floats(rx,
 int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
 	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err) {
 	const bool lm = lm_damping != nullptr;
-	// Warps per POI.  Measured on B200 (tools/ab_icgn2d.sh): with the GPU full, one warp per POI wins (config B 0.853 vs
-	// 0.906 ms, C 2.22 vs 2.43 ms, E 8.38 vs 8.87 ms) -- the second warp doubles the resident warps but also the per-POI
-	// fixed work and adds a barrier per pass; with fewer POIs than resident slots, two warps per POI shorten the tail
-	// (config A, 200 POIs: 24.6 vs 32.5 us).  So: 2 only when the queue cannot fill the machine.
+	// Warps per POI (tools/ab_icgn2d.sh compares the two): with the GPU full, one warp per POI wins -- the second warp
+	// doubles the resident warps but also the per-POI fixed work and adds a barrier per pass; with fewer POIs than resident
+	// slots, two warps per POI shorten the tail.  So: 2 only when the queue cannot fill the machine.
 	auto slots = [&](int wpp_) {
 		const size_t b = (size_t)icgn2d_slab_floats(rx, ry, lm, wpp_) * sizeof(float);
 		if (b > smem_optin) return 0;
@@ -1278,14 +1197,6 @@ int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, i
 	}
 	size_t smem = (size_t)icgn2d_slab_floats(rx, ry, lm, wpp) * sizeof(float);
 	if (smem > smem_optin) return -1;
-	// Tensor-Memory variant: when the queue fills the machine, the subset is >= 32 columns wide and <= 42 rows high (3 TMEM columns
-	// per row, 128 per CTA).  OCB_ICGN2D_TMEM=0 switches it off (A/B runs).
-	const char* tm_env = getenv("OCB_ICGN2D_TMEM");
-	// (and four such CTAs must fit the SM's shared memory, or the point of the variant -- 16 resident warps -- is lost)
-	const size_t tm_cta_smem = (size_t)ICGN2D_TM_WARPS * icgn2d_tm_slab_floats(rx, ry) * sizeof(float);
-	const bool use_tm = !lm && np == 6 && wpp == 1 && icgn2d_tm_supported(rx, ry) && !(tm_env && atoi(tm_env) == 0)
-		&& (long long)n >= (long long)sm_count * ICGN2D_TM_WARPS * 4 && ICGN2D_PAIRS && tm_cta_smem <= smem_optin
-		&& 4 * (tm_cta_smem + 1024) <= (size_t)(228 * 1024);
 	int blocks_per_sm = slots(wpp);
 	if (blocks_per_sm < 1) blocks_per_sm = 1;
 	if (const char* cap = getenv("OCB_ICGN2D_MAX_WARPS")) { // tuning knob: cap the resident warps per SM
@@ -1299,14 +1210,7 @@ int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, i
 	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[2] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry) };
 	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
 	Icgn2dKernel kern = wpp == 2 ? icgn2d_pick<2>(np, rx, ry, lm) : icgn2d_pick<1>(np, rx, ry, lm);
-	int threads = wpp * 32;
-	if (use_tm) {
-		// (6-parameter kernels only: the 12-parameter ones need ~250 registers, which already limits them to 8 warps per SM)
-		kern = (rx == 16 && ry == 16) ? icgn2d_kernel<6, 16, false, 1, true> : icgn2d_kernel<6, 0, false, 1, true>;
-		smem = tm_cta_smem;
-		threads = ICGN2D_TM_WARPS * 32;
-		blocks_per_sm = 512 / ICGN2D_TM_COLS; // Tensor Memory: 512 columns per SM
-	}
+	const int threads = wpp * 32;
 	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (*err != cudaSuccess) return -2;
 	if (wpp != 1) {
@@ -1315,9 +1219,8 @@ int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, i
 	} else {
 		d_counter += 32; // the one-warp-per-POI kernels reset their queue head themselves: a set of heads nobody else touches
 	}
-	long long resident = (long long)sm_count * blocks_per_sm;
-	if (use_tm && (long long)n < resident * ICGN2D_TM_WARPS) resident = ((long long)n + ICGN2D_TM_WARPS - 1) / ICGN2D_TM_WARPS;
-	int grid = (int)((long long)n < resident ? (long long)n : resident); // persistent: one wave, one POI per CTA (TM: per warp) at a time
+	const long long resident = (long long)sm_count * blocks_per_sm;
+	int grid = (int)((long long)n < resident ? (long long)n : resident); // persistent: one wave, one POI per CTA at a time
 	if (grid < 1) grid = 1;
 	kern<<<grid, threads, smem, stream>>>(img, d_pois, (int)n, rx, ry, conv, stop, d_counter, tm_ref, tm_tar, use_tma, d_center_offsets,
 		lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);

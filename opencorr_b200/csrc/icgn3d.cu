@@ -1,5 +1,5 @@
 // icgn3d.cu -- DVC: ICGN3D1 (first-order shape function, 12 parameters) and the device-side
-// ICGN3D1::prepare() products, for sm_100a.
+// ICGN3D1::prepare() products, for sm_90a.
 //
 // Replaces ICGN3D1::compute(POI3D*) (reference src/oc_icgn.cpp:1270-1490), Gradient3D4
 // (src/oc_gradient.cpp:143-231) and TricubicBspline::prepare/compute
@@ -7,7 +7,7 @@
 //
 // Round-2 structure in one paragraph: the setup pass runs with lanes along x and accumulates FACTORED Hessian sums
 // (ICGN3D_FACTORED_SETUP); when a whole z-slab of samples lies inside the staged tile (one warp-uniform corner test) every lane
-// takes TWO y-adjacent samples per step, their 4x4x4 blocks fetched as one 4x5x4 block and evaluated in packed f32x2
+// takes TWO y-adjacent samples per step, their 4x4x4 blocks fetched as one 4x5x4 block and evaluated as float2
 // arithmetic (ICGN3D_PAIRS); the `any sample < 0` rejection is re-decided in the reference's own arithmetic when the smallest
 // sample is borderline (icgn3d_exact_negative).  What follows describes the common skeleton.
 //
@@ -217,8 +217,8 @@ __device__ __noinline__ bool icgn3d_exact_negative(const float* A, float px, flo
 // 1: when a whole z-slab of samples has its support inside the staged tile (the normal case: one warp-uniform corner test
 // per slab replaces the per-sample range tests), every lane takes TWO y-adjacent samples per step.  Their 4x4x4 blocks
 // overlap in three of four block rows, so the pair is evaluated from ONE 4x5x4 block (80 LDS instead of 128 -- the kernel
-// was bound by the shared-memory pipe at 64 LDS per sample), and the arithmetic of the two samples runs in packed f32x2
-// pairs (FFMA2), rows (j, j+1) in lanes {.x, .y}: 104 instead of 168 issue slots for the taps, the same operations in the
+// was bound by the shared-memory pipe at 64 LDS per sample), and the arithmetic of the two samples runs as float2
+// pairs (ocb_f32x2.cuh), rows (j, j+1) in lanes {.x, .y}: the same operations in the
 // same order as the one-sample path (the results are bit-identical).  0: one sample per step (round-1 loop), for A/B runs.
 #define ICGN3D_PAIRS 1
 #endif

@@ -1,6 +1,6 @@
 // ocb_api.cu -- host side of the C ABI declared in include/opencorr_b200.h.
 // Owns the per-GPU context (device images, DVC tables, FFT twiddles/scratch, POI staging buffer)
-// and forwards to the sm_100a kernels.  No CPU compute path exists here by design.
+// and forwards to the sm_90a kernels.  No CPU compute path exists here by design.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdarg.h>
@@ -534,8 +534,8 @@ ocb_ctx* ocb_create(int device) {
 		delete ctx;
 		return nullptr;
 	}
-	if (prop.major < 10) {
-		set_error(nullptr, OCB_ERR_CUDA, "device %d is sm_%d%d; this library ships sm_100a code only", device, prop.major, prop.minor);
+	if (prop.major != 9 || prop.minor != 0) { // sm_90a code runs on compute capability 9.0 only
+		set_error(nullptr, OCB_ERR_CUDA, "device %d is sm_%d%d; this library ships sm_90a code only", device, prop.major, prop.minor);
 		cudaStreamDestroy(ctx->own_stream);
 		delete ctx;
 		return nullptr;

@@ -1,4 +1,4 @@
-// ocb_common.cuh -- shared definitions for the sm_100a kernels and the C-ABI host layer.
+// ocb_common.cuh -- shared definitions for the sm_90a kernels and the C-ABI host layer.
 #pragma once
 
 #include <cuda_runtime.h>

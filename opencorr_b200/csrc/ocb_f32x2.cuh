@@ -1,40 +1,21 @@
-// ocb_f32x2.cuh -- packed fp32 pairs on sm_100a: fma/mul/add.rn.f32x2 (SASS FFMA2 / FMUL2 / FADD2).
-// One instruction issues two IEEE round-to-nearest fp32 operations (bit-identical to the scalar ones), so
-// arithmetic-heavy inner loops spend about half the issue slots on math; a scalar operand broadcast to both
-// halves is an operand modifier (R.F32), not an extra move.  Blackwell only: these do not exist on sm_90.
+// ocb_f32x2.cuh -- fp32 pairs: two independent IEEE round-to-nearest operations per call.  sm_90 has no packed fp32
+// instruction, so each pair is two scalar FFMA / FMUL / FADD; the __f*_rn intrinsics keep every operation rounded on its
+// own (no contraction of a multiply into a following add), which is what the callers' arithmetic order relies on.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace ocb {
 
-typedef unsigned long long ocb_u64;
-
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-	float2 d;
-	asm("fma.rn.f32x2 %0, %1, %2, %3;"
-		: "=l"(reinterpret_cast<ocb_u64&>(d))
-		: "l"(reinterpret_cast<ocb_u64&>(a)), "l"(reinterpret_cast<ocb_u64&>(b)), "l"(reinterpret_cast<ocb_u64&>(c)));
-	return d;
+	return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-	float2 d;
-	asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<ocb_u64&>(d)) : "l"(reinterpret_cast<ocb_u64&>(a)), "l"(reinterpret_cast<ocb_u64&>(b)));
-	return d;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-	float2 d;
-	asm("add.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<ocb_u64&>(d)) : "l"(reinterpret_cast<ocb_u64&>(a)), "l"(reinterpret_cast<ocb_u64&>(b)));
-	return d;
-}
-__device__ __forceinline__ float2 fsub2(float2 a, float2 b) {
-	float2 d;
-	asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<ocb_u64&>(d)) : "l"(reinterpret_cast<ocb_u64&>(a)), "l"(reinterpret_cast<ocb_u64&>(b)));
-	return d;
-}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fsub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 bcast2(float a) { return make_float2(a, a); }
 
 // Bicubic weights of the reference's BC matrix (ocb_common.cuh bicubic_weights) as two pairs {w0, w1}, {w2, w3};
-// the same Horner steps, two weights per instruction.
+// the same Horner steps, two weights per call.
 __device__ __forceinline__ void bicubic_weights2(float t, float2& w01, float2& w23) {
 	const float s = 1.0f / 336.0f;
 	const float2 tt = bcast2(t);

@@ -1,4 +1,4 @@
-// ocb_kernels.h -- host-visible launch interfaces of the sm_100a kernels (internal to the library).
+// ocb_kernels.h -- host-visible launch interfaces of the sm_90a kernels (internal to the library).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

@@ -1,7 +1,7 @@
 // ocb_tma.cuh -- TMA (cp.async.bulk.tensor) + mbarrier primitives and the host-side tensor-map helper.
-// Measured on B200 (tools/tma_probe*.cu): the innermost tile coordinate must be 16-byte aligned
-// (x multiple of 4 floats) or the load raises "illegal instruction"; negative / past-the-end
-// coordinates are fine and read as zero.
+// Callers keep the innermost tile coordinate 16-byte aligned (x multiple of 4 floats; an unaligned
+// x was seen to raise "illegal instruction"); negative / past-the-end coordinates are fine and read
+// as zero.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

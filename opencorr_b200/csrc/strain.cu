@@ -1,4 +1,4 @@
-// strain.cu -- Strain post-processing of a POI queue (SURVEY.md section 8(f) N4) for sm_100a.
+// strain.cu -- Strain post-processing of a POI queue (SURVEY.md section 8(f) N4) for sm_90a.
 //
 // Replaces Strain::prepare + Strain::compute(std::vector<POI2D>&) / (std::vector<POI3D>&) of the
 // reference (src/oc_strain.cpp:100-111,150-156,158-250,373-487): for every POI with ZNCC >= threshold,
@@ -9,7 +9,7 @@
 // colPivHouseholderQr in the reference); the plane's slopes are the displacement gradients, from
 // which the Cauchy or Green strains follow.
 //
-// B200 mapping: no tree.  The POIs are binned into a uniform grid (cell edge >= radius) by one
+// GPU mapping: no tree.  The POIs are binned into a uniform grid (cell edge >= radius) by one
 // stable radix sort of (cell id, POI index); a warp per POI then scans the 3 (2D) / 9 (3D) runs of
 // x-adjacent cells that can hold neighbours -- contiguous in the sorted order, found by binary
 // search -- with coalesced 16-byte loads, and accumulates the normal equations in FP64 (12 / 22

@@ -133,6 +133,6 @@ CONFIGS = {
     "D": dict(kind="3d", size=(256, 256, 256), grid=(40, 40, 40, 40, 25, 20, 4, 7, 8), r=16, order=1, conv=1e-3, stop=20),
     "E": dict(kind="2d", size=(4096, 4096), grid=(128, 128, 1000, 500, 3, 7), r=16, order=1, conv=1e-3, stop=10),
     # not a BASELINE.json config: the geometry of the reference's own DVC example (examples/test_dvc_fftcc_icgn1.cpp:
-    # 61^3 subvolumes, stop 20) on a synthetic volume, for the record in profiles/
+    # 61^3 subvolumes, stop 20) on a synthetic volume (bench.py --config F)
     "F": dict(kind="3d", size=(288, 288, 288), grid=(40, 40, 40, 12, 12, 12, 19, 19, 19), r=30, order=1, conv=1e-3, stop=20),
 }

@@ -8,6 +8,7 @@ Outputs
   oht_cfrp_0.bmp, oht_cfrp_4.bmp    the 2D example pair (280x900, 8-bit), verbatim
   oht_cfrp_4_fftcc_icgn1_r16.npz    every 23rd row of the shipped result table + deformation table, plus the three rows whose
                                     FFT-CC guess is an exact tie between two correlation bins (fftcc_tie_rows / fftcc_tie_table)
+  oht_cfrp_4_fftcc_icgn1_r16_full.npz  all 30 000 rows of that table: x, y, u, v, u0, v0, ZNCC, iteration (compact types)
   oht_cfrp_4_fftcc_iclm1_r16.npz    the same rows of the shipped ICLM2D1 table
   oht_cfrp_4_sift_icgn2_gpu_r16.npz every 23rd row of examples/2d_dic/oht_cfrp_4_sift_icgn2(gpu)_r16.csv (the reference's GPU ICGN2D2,
                                     SIFT-seeded): x,y,u,v,u0,v0,ZNCC,iteration,convergence.  u0, v0 are the seeds; the affine part
@@ -164,6 +165,16 @@ def make_epipolar_fixture():
                         fundamental=fm, columns=np.array("x,y,r1r2 ZNCC,r2_x,r2_y".split(",")), table=blk[:, :5])
 
 
+def make_full_table_fixture(tab):
+    """All 30 000 rows of the shipped oht_cfrp_4_fftcc_icgn1_r16.csv in the columns the full-table test reads, in compact types:
+    x, y, u0, v0 and the iteration count are integers; u, v (8 printed decimals, |u|, |v| < 20 px) and ZNCC keep float32, whose
+    rounding (< 1e-6 px, < 6e-8) sits far below the test's tolerances (5e-5 px, 2e-6)."""
+    assert np.all(tab[:, [0, 1, 4, 5, 7]] == np.round(tab[:, [0, 1, 4, 5, 7]]))
+    np.savez_compressed(os.path.join(OUT, "oht_cfrp_4_fftcc_icgn1_r16_full.npz"),
+                        xy=tab[:, 0:2].astype(np.int16), uv=tab[:, 2:4].astype(np.float32), uv0=tab[:, 4:6].astype(np.int16),
+                        zncc=tab[:, 6].astype(np.float32), iteration=tab[:, 7].astype(np.int8))
+
+
 def main():
     for name in ("oht_cfrp_0.bmp", "oht_cfrp_4.bmp"):
         shutil.copyfile(os.path.join(REF, "2d_dic", name), os.path.join(OUT, name))
@@ -178,6 +189,7 @@ def main():
                         columns=np.array("x,y,u,v,u0,v0,ZNCC,iteration,convergence".split(",")),
                         table=tab[sel, :9], deformation_columns=np.array("x,y,u,ux,uy,v,vx,vy".split(",")),
                         deformation=dtab[sel, :8], rows=sel, fftcc_tie_rows=ties, fftcc_tie_table=tab[ties, :9])
+    make_full_table_fixture(tab)
 
     # ICLM2D1 table shipped by the reference (examples/2d_dic/oht_cfrp_4_fftcc_iclm1_r16.csv, same POIs)
     itab = np.genfromtxt(os.path.join(REF, "2d_dic", "oht_cfrp_4_fftcc_iclm1_r16.csv"), delimiter=",", skip_header=1)

@@ -578,9 +578,9 @@ def test_two_operators_with_different_pairs_interleaved(engine):
     assert np.array_equal(qb, want_b)
 
 
-def test_large_deformation_gradient_tensor_memory_variant(engine):
-    """The 12 % stretch of test_large_deformation_gradient_falls_back_to_global_reads on a queue of 3 136 POIs: the
-    Tensor-Memory variant of the kernel, whose row-by-row path fetches a lane's constants from TMEM one row at a time."""
+def test_large_deformation_gradient_long_queue(engine):
+    """The 12 % stretch of test_large_deformation_gradient_falls_back_to_global_reads on a queue of 3 136 POIs, long enough
+    to fill every SM with one-warp-per-POI CTAs, whose row-by-row path reads a lane's constants one row at a time."""
     ref, _ = synth.speckle_pair_2d(704, 704)
     yy, xx = np.mgrid[0:704, 0:704].astype(np.float32)
     o_ref = Oracle2D(ref, ref)
@@ -599,5 +599,5 @@ def test_large_deformation_gradient_tensor_memory_variant(engine):
     engine.icgn2d1(q_gpu, 16, 16, 0.001, 10)
     Oracle2D(ref, tar).icgn2d1(q_cpu, 16, 16, 0.001, 10)
     assert (q_cpu[:, 16] > 0.9).all()
-    stats = util.compare_2d(q_gpu, q_cpu, "stretch, TM variant", max_iter_mismatch_frac=0.05)
+    stats = util.compare_2d(q_gpu, q_cpu, "stretch, long queue", max_iter_mismatch_frac=0.05)
     assert stats["n_compared"] > 0.9 * len(q)

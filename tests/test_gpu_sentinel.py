@@ -87,8 +87,8 @@ def test_negative_interpolated_sample_rule_3d(engine):
     assert seen_rejected > 300 and seen_kept > 50
 
 
-def test_negative_interpolated_sample_rule_tensor_memory_variant(engine):
-    """The same rule on a queue long enough (4 900 POIs >= 16 warps per SM) for the Tensor-Memory variant of the ICGN2D1 kernel."""
+def test_negative_interpolated_sample_rule_long_queue(engine):
+    """The same rule on a queue long enough (4 900 POIs) to fill every SM with one-warp-per-POI CTAs of the ICGN2D1 kernel."""
     ref, tar = synth.speckle_pair_2d(704, 704)
     holes = _discs((704, 704), 60, 4, 14, 3)
     ref, tar = np.where(holes, 0, ref).astype(np.float32), np.where(holes, 0, tar).astype(np.float32)

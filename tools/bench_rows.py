@@ -1,6 +1,6 @@
 """Per-row timings for SURVEY section 8(f) rows N1/N2/N4 on bench config B (2048^2, 50 000 POIs, 33x33):
 device-resident CUDA-event time of each operator through the C ABI's _dev entry points, next to the CPU oracle
-(nproc-1 threads) on a bounded sample.  Writes one JSON line per row; `python tools/bench_rows.py > profiles/...`.
+(nproc-1 threads) on a bounded sample.  Writes one JSON line per row; `python tools/bench_rows.py > rows.jsonl`.
 Not the headline benchmark (that is bench.py)."""
 import json
 import os

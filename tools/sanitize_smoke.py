@@ -13,7 +13,7 @@ for r in (16,7):
     else: xyz2=xyz
     q=ob.make_poi3d(xyz2); e.set_images_3d(r3,t3); e.fftcc3d(q,r,r,r); e.icgn3d_prepare(); e.icgn3d1(q,r,r,r,0.001,20); print('3d r',r,q[:,18])
 e.close(); print('done')
-# round 2: a queue long enough for the Tensor-Memory variant of ICGN2D1 (>= 16 warps per SM) and the chunked host-queue path,
+# round 2: a queue long enough to fill every SM with one-warp-per-POI ICGN2D1 CTAs and the chunked host-queue path,
 # once with a pageable and once with a page-locked (zero-copy) queue; a group context of every visible device
 import ctypes
 from opencorr_b200 import _capi
@@ -25,7 +25,7 @@ for pin in (0,1):
     if pin: lib.ocb_host_register(ctypes.c_void_p(q.ctypes.data), q.nbytes)
     e.set_images_2d(ref,tar); e.fftcc2d(q,16,16); e.icgn2d_prepare(); e.icgn2d1(q,16,16,0.001,10)
     if pin: lib.ocb_host_unregister(ctypes.c_void_p(q.ctypes.data))
-    print('tmem path, pinned' if pin else 'tmem path, pageable', len(q), (q[:,16]>0.9).sum())
+    print('long queue, pinned' if pin else 'long queue, pageable', len(q), (q[:,16]>0.9).sum())
 e.close()
 g=ob.Engine(list(range(lib.ocb_device_count()))); q=ob.make_poi2d(xy); g.set_images_2d(ref,tar); g.fftcc2d(q,16,16); g.icgn2d_prepare(); g.icgn2d1(q,16,16,0.001,10); print('group', g.member_count, (q[:,16]>0.9).sum()); g.close()
 print('done round 2')
