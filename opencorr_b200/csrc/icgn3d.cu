@@ -30,8 +30,6 @@
 
 namespace ocb {
 
-constexpr int ICGN3D_MAX_WARPS = 16; // CTAs run 8 warps (two CTAs per SM) or, when only one slab-carrying CTA fits, 16
-
 // ---- ICGN3D1::prepareRef: Gradient3D4::getGradientX/Y/Z, src/oc_gradient.cpp:143-231 ----------
 // Output is packed {ref, gx, gy, gz} per voxel so that IC-GN fetches a sample's constants with one 16-byte load.
 __global__ void gradient3d_kernel(const float* __restrict__ f, float4* __restrict__ rg, int dx, int dy, int dz) {
@@ -82,24 +80,8 @@ void prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int
 	prefilter3d_kernel<<<sm_count * 8, 256, 0, s>>>(in, out, dx, dy, dz, axis);
 }
 
-// ---- ICGN3D1::compute ---------------------------------------------------------------------------
-constexpr int NP3 = 12;
-constexpr int NH3 = NP3 * (NP3 + 1) / 2; // 78
-constexpr int NSETUP = NH3 + 2 * NP3 + 2; // Hessian + S + SR + r1 + r2 = 104
-constexpr int NITER = 3 + NP3;            // d1, d2, rd, SD[12]
-constexpr int ICGN3D_TILE_MARGIN = 1;
-
-struct Icgn3dShared {
-	float part[ICGN3D_MAX_WARPS][NSETUP]; // per-warp partial sums
-	float tot[NSETUP];
-	float L[NH3];   // packed Cholesky factor (diag = 1/L_ii)
-	float S[NP3], SF[NP3];
-	float A[12];    // running warp rows: [1+ux uy uz u | vx 1+vy vz v | wx wy 1+wz w]
-	float f2, rbar, c0;
-	float dp_norm, zncc;
-	int keep_going;
-	int poi;
-};
+// ---- ICGN3D1::compute (NP3, NSETUP, Icgn3dShared, tile extents and launch plan: ocb_kernels.h) ---------------------------
+constexpr int NITER = 3 + NP3; // d1, d2, rd, SD[12]
 
 // floor(x / d) for 0 <= x < 2^21, d >= 1 (inv = 1.0f / d); see fftcc.cu
 __device__ __forceinline__ int fdiv3(int x, float inv) { return __float2int_rz(((float)x + 0.5f) * inv); }
@@ -231,10 +213,6 @@ __device__ __forceinline__ void bspline_basis_fast2(float2 t, float2* b) {
 	b[1] = ffma2(t2, ffma2(bcast2(0.5f), t, bcast2(-1.f)), bcast2(2.f / 3.f));
 	b[2] = fsub2(fsub2(fsub2(bcast2(1.f), b[0]), b[1]), b[3]);
 }
-
-__host__ __device__ inline int icgn3d_tile_x(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * ICGN3D_TILE_MARGIN + 3); }
-__host__ __device__ inline int icgn3d_tile_y(int ry) { return 2 * ry + 1 + 3 + 2 * ICGN3D_TILE_MARGIN; }
-__host__ __device__ inline int icgn3d_tile_z(int slab_k) { return slab_k + 3 + 2 * ICGN3D_TILE_MARGIN; }
 
 // RC > 0: radius known at compile time (rx == ry == rz == RC): tile pitches become immediates.
 // THREADS: 256 (two CTAs per SM) or 512 (large radii: the slab leaves room for one CTA only, which then brings 16 warps)
@@ -740,37 +718,24 @@ __global__ void __launch_bounds__(THREADS, 512 / THREADS) icgn3d1_kernel(Image3D
 // Returns 0, -1 when even a one-layer slab does not fit in shared memory, -2 on a CUDA error.
 int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop, int sm_count, size_t smem_optin,
 	int* d_counter, cudaStream_t stream, cudaError_t* err) {
-	const int sz = 2 * rz + 1;
-	const size_t layer = (size_t)icgn3d_tile_x(rx) * icgn3d_tile_y(ry) * sizeof(float);
-	const size_t fixed = 128 + sizeof(Icgn3dShared) + 1024; // barrier pad + static smem + per-CTA reservation
-	const int halo = 3 + 2 * ICGN3D_TILE_MARGIN;
-	// prefer two CTAs per SM (one loads while the other computes) when that leaves slabs of >= 6 layers
-	int ctas = 2;
-	long long k = (long long)(((228 * 1024) / 2 - fixed) / layer) - halo;
-	if (k < 6 && k < sz) {
-		ctas = 1;
-		size_t budget = smem_optin < (size_t)(227 * 1024) ? smem_optin : (size_t)(227 * 1024);
-		k = (long long)((budget - 128 - sizeof(Icgn3dShared)) / layer) - halo;
-	}
-	if (k < 1) return -1;
-	if (k > sz) k = sz;
-	const int nslab = (int)((sz + k - 1) / k);
-	const int slab_k = (sz + nslab - 1) / nslab; // even out the slabs
-	const size_t smem = 128 + layer * icgn3d_tile_z(slab_k);
+	Icgn3dPlan plan;
+	if (!icgn3d1_plan(rx, ry, rz, smem_optin, &plan)) return -1;
+	const int slab_k = plan.slab_k;
+	const size_t smem = plan.smem;
 	CUtensorMap tm;
 	memset(&tm, 0, sizeof(tm));
 	const int dims[3] = { img.dx, img.dy, img.dz };
 	const int box[3] = { icgn3d_tile_x(rx), icgn3d_tile_y(ry), icgn3d_tile_z(slab_k) };
 	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm, img.coef, 3, dims, box);
 	void (*kern)(Image3D, float*, int, int, int, int, float, float, int, int*, const CUtensorMap, int);
-	const int threads = ctas == 1 ? 512 : 256;
-	if (ctas == 1) kern = (rx == 30 && ry == 30 && rz == 30) ? icgn3d1_kernel<30, 512> : icgn3d1_kernel<0, 512>; // 61^3: the reference's own DVC example
-	else kern = (rx == 16 && ry == 16 && rz == 16) ? icgn3d1_kernel<16, 256> : icgn3d1_kernel<0, 256>;
+	const int threads = plan.threads;
+	if (plan.threads == 512) kern = plan.rc == 30 ? icgn3d1_kernel<30, 512> : icgn3d1_kernel<0, 512>;
+	else kern = plan.rc == 16 ? icgn3d1_kernel<16, 256> : icgn3d1_kernel<0, 256>;
 	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (*err != cudaSuccess) return -2;
 	*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
 	if (*err != cudaSuccess) return -2;
-	long long grid = (long long)sm_count * ctas;
+	long long grid = (long long)sm_count * plan.ctas_per_sm;
 	if (grid > (long long)n) grid = (long long)n;
 	if (grid < 1) grid = 1;
 	kern<<<(int)grid, threads, smem, stream>>>(img, d_pois, (int)n, rx, ry, rz, conv, stop, slab_k, d_counter, tm, use_tma);

@@ -71,6 +71,68 @@ int fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, 
 int fftcc3d_w32_grid(int sm_count);
 int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err);
 // icgn3d.cu
+constexpr int ICGN3D_MAX_WARPS = 16; // CTAs run 8 warps (two CTAs per SM) or, when only one slab-carrying CTA fits, 16
+constexpr int NP3 = 12;
+constexpr int NH3 = NP3 * (NP3 + 1) / 2;  // 78
+constexpr int NSETUP = NH3 + 2 * NP3 + 2; // Hessian + S + SR + r1 + r2 = 104
+constexpr int ICGN3D_TILE_MARGIN = 1;
+
+// static shared memory of icgn3d1_kernel
+struct Icgn3dShared {
+	float part[ICGN3D_MAX_WARPS][NSETUP]; // per-warp partial sums
+	float tot[NSETUP];
+	float L[NH3];   // packed Cholesky factor (diag = 1/L_ii)
+	float S[NP3], SF[NP3];
+	float A[12];    // running warp rows: [1+ux uy uz u | vx 1+vy vz v | wx wy 1+wz w]
+	float f2, rbar, c0;
+	float dp_norm, zncc;
+	int keep_going;
+	int poi;
+};
+
+// extents of the staged B-spline coefficient tile: x padded to a multiple of 4 floats (16-byte TMA rows)
+__host__ __device__ inline int icgn3d_tile_x(int rx) { return (2 * rx + 1 + 3 + 2 * ICGN3D_TILE_MARGIN + 3 + 3) & ~3; }
+__host__ __device__ inline int icgn3d_tile_y(int ry) { return 2 * ry + 1 + 3 + 2 * ICGN3D_TILE_MARGIN; }
+__host__ __device__ inline int icgn3d_tile_z(int slab_k) { return slab_k + 3 + 2 * ICGN3D_TILE_MARGIN; }
+
+// Launch geometry of icgn3d1_kernel for a subvolume of radii (rx, ry, rz): the (2rz+1) layers are processed in nslab z-slabs of
+// slab_k layers (the last one may be thinner), each staged as one tile of icgn3d_tile_z(slab_k) layers in dynamic shared memory.
+struct Icgn3dPlan {
+	int ctas_per_sm; // 2 (256 threads each) or 1 (512 threads)
+	int threads;
+	int rc;          // radius baked into the kernel (16 or 30), 0 for the generic kernel
+	int slab_k;
+	int nslab;       // slabs per iteration: ceil((2rz+1) / slab_k)
+	size_t smem;     // dynamic shared memory per CTA
+};
+
+// false when even a one-layer slab does not fit in shared memory (smem_optin: the device's opt-in limit per block)
+inline bool icgn3d1_plan(int rx, int ry, int rz, size_t smem_optin, Icgn3dPlan* p) {
+	const int sz = 2 * rz + 1;
+	const size_t layer = (size_t)icgn3d_tile_x(rx) * icgn3d_tile_y(ry) * sizeof(float);
+	const size_t fixed = 128 + sizeof(Icgn3dShared) + 1024; // barrier pad + static smem + per-CTA reservation
+	const int halo = 3 + 2 * ICGN3D_TILE_MARGIN;
+	// prefer two CTAs per SM (one loads while the other computes) when that leaves slabs of >= 6 layers
+	int ctas = 2;
+	long long k = (long long)(((228 * 1024) / 2 - fixed) / layer) - halo;
+	if (k < 6 && k < sz) {
+		ctas = 1;
+		const size_t budget = smem_optin < (size_t)(227 * 1024) ? smem_optin : (size_t)(227 * 1024);
+		k = (long long)((budget - 128 - sizeof(Icgn3dShared)) / layer) - halo;
+	}
+	if (k < 1) return false;
+	if (k > sz) k = sz;
+	p->ctas_per_sm = ctas;
+	p->threads = ctas == 1 ? 512 : 256;
+	const int nslab = (int)((sz + k - 1) / k);
+	p->slab_k = (sz + nslab - 1) / nslab; // even out the slabs
+	p->nslab = (sz + p->slab_k - 1) / p->slab_k;
+	p->smem = 128 + layer * icgn3d_tile_z(p->slab_k);
+	if (ctas == 1) p->rc = (rx == 30 && ry == 30 && rz == 30) ? 30 : 0; // 61^3: the reference's own DVC example
+	else p->rc = (rx == 16 && ry == 16 && rz == 16) ? 16 : 0;
+	return true;
+}
+
 void gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s);
 void prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s);
 int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop, int sm_count, size_t smem_optin,
