@@ -195,6 +195,32 @@ int ocb_strain2ds_dev(ocb_ctx* ctx, void* d_poi2ds, size_t n, float radius, int 
 int ocb_strain2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation);
 int ocb_strain3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation);
 
+/* ---- Stereo reconstruction: Calibration::prepare / undistort (src/oc_calibration.cpp:161-264) and
+ *      Stereovision::reconstruct (src/oc_stereovision.cpp:70-133) ----------------------------------------------------------
+ * intrinsics: the 13 floats of CameraIntrinsics (src/oc_calibration.h:25-35), fx fy fs cx cy k1 k2 k3 k4 k5 k6 p1 p2.
+ * projection: the camera's 3x4 projection matrix K [R | t], row-major (Calibration::updateProjectionMatrix, :69-77).
+ * ocb_calib = one camera's distortion map (map_x, map_y: float32 [height][width] in device memory), built by ocb_calib_prepare
+ * with the fixed-point loop of :180-218 (at most `iteration` rounds, stop when both deviations are <= convergence; the
+ * reference's defaults are 0.001 and 40).  The handle belongs to the context it was made with; on a GROUP context the maps live
+ * on the first member and the calls below run there (the point sets are small; see DESIGN.md section 6).
+ * Points are n (x, y) float pairs.  As the reference takes Point2D&, every point is clamped IN PLACE to [0, W-2] x [0, H-2]
+ * before the bilinear lookup (:224-239).  The intrinsics of the lookup are passed with each call ("current at call time"). */
+typedef struct ocb_calib ocb_calib;
+int ocb_calib_prepare(ocb_ctx* ctx, const float* intrinsics, int height, int width, float convergence, int iteration, ocb_calib** out);
+void ocb_calib_destroy(ocb_calib* calib);
+/* Copy the maps to host buffers of height*width floats each (row-major); either pointer may be NULL. */
+int ocb_calib_get_map(ocb_ctx* ctx, const ocb_calib* calib, float* map_x, float* map_y);
+/* Calibration::undistort for n host points: pts (n x 2) clamped in place, out (n x 2) = sensor coordinates.  A point with a
+ * NaN coordinate (undefined in the reference) is left as it is and gives NaN.  Blocking. */
+int ocb_calib_undistort(ocb_ctx* ctx, const ocb_calib* calib, const float* intrinsics, float* pts, float* out, size_t n);
+/* Stereovision::reconstruct(queue, queue, queue) as one batch: pts3d (n x 3) = world coordinates.  A NaN coordinate in either view
+ * gives (0, 0, 0) and leaves both points untouched; every other pair is clamped in place.  The 4x3 system of :87-112 is formed
+ * in float32 and solved as least squares in FP64.  Host buffers (blocking) / device buffers (enqueue only, single-device context). */
+int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, float* pts1, float* pts2, float* pts3d, size_t n);
+int ocb_stereo_reconstruct_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n);
+
 /* ---- inspection (parity tests of the prepare() products) ----------------------------------- */
 /* Copy the device tables built by ocb_icgn3d_prepare() to host buffers of dim_x*dim_y*dim_z
  * floats each; any pointer may be NULL. */

@@ -74,6 +74,12 @@ SIGNATURES = {
     "ocb_nr2d1": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_nr2d1_dev": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_get_tables_3d": (_i, [_vp, _vp, _vp, _vp, _vp]),
+    "ocb_calib_prepare": (_i, [_vp, _vp, _i, _i, _f, _i, ctypes.POINTER(_vp)]),
+    "ocb_calib_destroy": (None, [_vp]),
+    "ocb_calib_get_map": (_i, [_vp, _vp, _vp, _vp]),
+    "ocb_calib_undistort": (_i, [_vp, _vp, _vp, _vp, _vp, _sz]),
+    "ocb_stereo_reconstruct": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz]),
+    "ocb_stereo_reconstruct_dev": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz]),
 }
 
 _lib = None

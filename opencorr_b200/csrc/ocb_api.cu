@@ -166,6 +166,19 @@ struct ocb_ctx {
 	size_t d_cand_bytes = 0;
 	void* d_strain_ws = nullptr; // Strain: sort keys / compact neighbour arrays / cub scratch
 	size_t d_strain_ws_bytes = 0;
+	float* d_stereo = nullptr; // stereo reconstruction / undistortion: staged points
+	size_t d_stereo_bytes = 0;
+};
+
+// One camera's distortion map (Calibration::prepare).  `owner` is the context the caller made it with (a group or a single
+// device); `exec` is the single-device context that holds the maps and runs every call on them.
+struct ocb_calib {
+	const ocb_ctx* owner = nullptr;
+	ocb_ctx* exec = nullptr;
+	int device = 0;
+	int height = 0, width = 0;
+	float* map_x = nullptr;
+	float* map_y = nullptr;
 };
 
 static int set_error(ocb_ctx* ctx, int code, const char* fmt, ...) {
@@ -661,6 +674,7 @@ void ocb_destroy(ocb_ctx* ctx) {
 	cudaFree(ctx->d_off);
 	cudaFree(ctx->d_strain_ws);
 	cudaFree(ctx->d_cand);
+	cudaFree(ctx->d_stereo);
 	for (int i = 0; i < 4; i++)
 		if (ctx->pipe[i]) cudaStreamDestroy(ctx->pipe[i]);
 	if (ctx->pipe_ready) cudaEventDestroy(ctx->pipe_ready);
@@ -1369,6 +1383,181 @@ int ocb_get_tables_3d(ocb_ctx* ctx, float* gx, float* gy, float* gz, float* coef
 	if (coefficient) OCB_CUDA(ctx, cudaMemcpyAsync(coefficient, ctx->coef3, elems * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
 	OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return OCB_OK;
+}
+
+// ---- Stereo reconstruction: Calibration::prepare / undistort, Stereovision::reconstruct --------------------------------------
+// A failure on the executing member of a group is reported on the group as well.
+static int relay_error(ocb_ctx* ctx, const ocb_ctx* exec, int rc) {
+	if (rc != OCB_OK && ctx != exec) {
+		ctx->last_error = exec->last_error;
+		g_last_error = ctx->last_error;
+	}
+	return rc;
+}
+
+static int calib_check(ocb_ctx* ctx, const ocb_calib* c, const char* what) {
+	if (!c) return set_error(ctx, OCB_ERR_ARG, "%s: null calibration handle", what);
+	if (c->owner != ctx) return set_error(ctx, OCB_ERR_ARG, "%s: calibration handle belongs to another context", what);
+	return OCB_OK;
+}
+
+static int ensure_stereo_buffer(ocb_ctx* x, size_t bytes) {
+	if (bytes > x->d_stereo_bytes) {
+		if (x->d_stereo) cudaFree(x->d_stereo);
+		x->d_stereo = nullptr;
+		x->d_stereo_bytes = 0;
+		OCB_CUDA(x, cudaMalloc(&x->d_stereo, bytes));
+		x->d_stereo_bytes = bytes;
+	}
+	return OCB_OK;
+}
+
+static void free_calib(ocb_calib* c) {
+	if (!c) return;
+	if (c->map_x || c->map_y) {
+		cudaSetDevice(c->device);
+		cudaFree(c->map_x);
+		cudaFree(c->map_y);
+	}
+	delete c;
+}
+
+static int calib_build(ocb_ctx* x, ocb_calib* c, const float* intrinsics, float convergence, int iteration) {
+	if (ensure_device(x)) return OCB_ERR_CUDA;
+	const size_t bytes = (size_t)c->height * c->width * sizeof(float);
+	OCB_CUDA(x, cudaMalloc(&c->map_x, bytes));
+	OCB_CUDA(x, cudaMalloc(&c->map_y, bytes));
+	ocb::calib_map_launch(intrinsics, c->height, c->width, convergence, iteration, c->map_x, c->map_y, x->stream);
+	OCB_CUDA(x, cudaGetLastError());
+	x->launches++;
+	return OCB_OK;
+}
+
+int ocb_calib_prepare(ocb_ctx* ctx, const float* intrinsics, int height, int width, float convergence, int iteration, ocb_calib** out) {
+	if (out) *out = nullptr;
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	if (!intrinsics || !out) return set_error(ctx, OCB_ERR_ARG, "calib_prepare: bad arguments");
+	if (height < 2 || width < 2) return set_error(ctx, OCB_ERR_ARG, "calib_prepare: image size %d x %d is below 2 x 2", width, height);
+	ocb_ctx* x = is_group(ctx) ? ctx->members[0] : ctx;
+	ocb_calib* c = new ocb_calib;
+	c->owner = ctx;
+	c->exec = x;
+	c->device = x->device;
+	c->height = height;
+	c->width = width;
+	const int rc = calib_build(x, c, intrinsics, convergence, iteration);
+	if (rc != OCB_OK) {
+		free_calib(c);
+		return relay_error(ctx, x, rc);
+	}
+	*out = c;
+	return OCB_OK;
+}
+
+void ocb_calib_destroy(ocb_calib* calib) { free_calib(calib); }
+
+int ocb_calib_get_map(ocb_ctx* ctx, const ocb_calib* calib, float* map_x, float* map_y) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	int rc = calib_check(ctx, calib, "calib_get_map");
+	if (rc) return rc;
+	ocb_ctx* x = calib->exec;
+	const size_t bytes = (size_t)calib->height * calib->width * sizeof(float);
+	rc = [&]() -> int {
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		if (map_x) OCB_CUDA(x, cudaMemcpyAsync(map_x, calib->map_x, bytes, cudaMemcpyDeviceToHost, x->stream));
+		if (map_y) OCB_CUDA(x, cudaMemcpyAsync(map_y, calib->map_y, bytes, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+int ocb_calib_undistort(ocb_ctx* ctx, const ocb_calib* calib, const float* intrinsics, float* pts, float* out, size_t n) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	int rc = calib_check(ctx, calib, "calib_undistort");
+	if (rc) return rc;
+	if (!intrinsics || ((!pts || !out) && n)) return set_error(ctx, OCB_ERR_ARG, "calib_undistort: bad arguments");
+	if (n == 0) return OCB_OK;
+	ocb_ctx* x = calib->exec;
+	rc = [&]() -> int {
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t bytes = n * 2 * sizeof(float);
+		int r = ensure_stereo_buffer(x, 2 * bytes);
+		if (r) return r;
+		float* d_pts = x->d_stereo;
+		float* d_out = x->d_stereo + 2 * n;
+		OCB_CUDA(x, cudaMemcpyAsync(d_pts, pts, bytes, cudaMemcpyHostToDevice, x->stream));
+		ocb::calib_undistort_launch(calib->map_x, calib->map_y, calib->height, calib->width, intrinsics, d_pts, d_out, n, x->stream);
+		OCB_CUDA(x, cudaGetLastError());
+		x->launches++;
+		OCB_CUDA(x, cudaMemcpyAsync(pts, d_pts, bytes, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+static int stereo_check(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, const float* pts1, const float* pts2, const float* pts3d, size_t n) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	int rc = calib_check(ctx, calib1, "stereo_reconstruct");
+	if (!rc) rc = calib_check(ctx, calib2, "stereo_reconstruct");
+	if (rc) return rc;
+	if (!intrinsics1 || !projection1 || !intrinsics2 || !projection2 || ((!pts1 || !pts2 || !pts3d) && n))
+		return set_error(ctx, OCB_ERR_ARG, "stereo_reconstruct: bad arguments");
+	return OCB_OK;
+}
+
+static void stereo_cams(const ocb_calib* c1, const float* i1, const float* p1, const ocb_calib* c2, const float* i2, const float* p2,
+	ocb::StereoCam* s1, ocb::StereoCam* s2) {
+	*s1 = ocb::StereoCam{ c1->map_x, c1->map_y, c1->height, c1->width, i1, p1 };
+	*s2 = ocb::StereoCam{ c2->map_x, c2->map_y, c2->height, c2->width, i2, p2 };
+}
+
+int ocb_stereo_reconstruct_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n) {
+	OCB_NO_GROUP(ctx, "stereo_reconstruct_dev");
+	int rc = stereo_check(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, d_pts1, d_pts2, d_pts3d, n);
+	if (rc) return rc;
+	if (n == 0) return OCB_OK;
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	ocb::StereoCam s1, s2;
+	stereo_cams(calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2);
+	ocb::stereo_reconstruct_launch(s1, s2, d_pts1, d_pts2, d_pts3d, n, ctx->stream);
+	OCB_CUDA(ctx, cudaGetLastError());
+	ctx->launches++;
+	return OCB_OK;
+}
+
+int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, float* pts1, float* pts2, float* pts3d, size_t n) {
+	int rc = stereo_check(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, pts1, pts2, pts3d, n);
+	if (rc) return rc;
+	if (n == 0) return OCB_OK;
+	ocb_ctx* x = calib1->exec;
+	rc = [&]() -> int {
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t b2 = n * 2 * sizeof(float), b3 = n * 3 * sizeof(float);
+		int r = ensure_stereo_buffer(x, 2 * b2 + b3);
+		if (r) return r;
+		float* d1 = x->d_stereo;
+		float* d2 = d1 + 2 * n;
+		float* d3 = d2 + 2 * n;
+		OCB_CUDA(x, cudaMemcpyAsync(d1, pts1, b2, cudaMemcpyHostToDevice, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(d2, pts2, b2, cudaMemcpyHostToDevice, x->stream));
+		ocb::StereoCam s1, s2;
+		stereo_cams(calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2);
+		ocb::stereo_reconstruct_launch(s1, s2, d1, d2, d3, n, x->stream);
+		OCB_CUDA(x, cudaGetLastError());
+		x->launches++;
+		OCB_CUDA(x, cudaMemcpyAsync(pts1, d1, b2, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(pts2, d2, b2, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(pts3d, d3, b3, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
 }
 
 } // extern "C"

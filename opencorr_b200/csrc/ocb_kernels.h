@@ -133,6 +133,21 @@ inline bool icgn3d1_plan(int rx, int ry, int rz, size_t smem_optin, Icgn3dPlan* 
 	return true;
 }
 
+// stereo.cu (intrinsics: the 13 floats of CameraIntrinsics, fx fy fs cx cy k1..k6 p1 p2; maps row-major [height][width])
+struct StereoCam {
+	const float* map_x;
+	const float* map_y;
+	int height, width;
+	const float* intrinsics; // host pointer, 13 floats
+	const float* projection; // host pointer, 3x4 row-major
+};
+void calib_map_launch(const float* intrinsics, int height, int width, float convergence, int iteration, float* d_map_x, float* d_map_y,
+	cudaStream_t stream);
+void calib_undistort_launch(const float* d_map_x, const float* d_map_y, int height, int width, const float* intrinsics, float* d_pts, float* d_out,
+	size_t n, cudaStream_t stream);
+void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
+	cudaStream_t stream);
+
 void gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s);
 void prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s);
 int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop, int sm_count, size_t smem_optin,
