@@ -103,6 +103,20 @@ struct ocb_worker {
 	}
 };
 
+// Grow-only device buffer of a context (see grow).  Released when the context is deleted, after ocb_destroy has made its
+// device current.
+struct DevBuf {
+	void* p = nullptr;
+	size_t bytes = 0;
+	DevBuf() = default;
+	DevBuf(const DevBuf&) = delete;
+	DevBuf& operator=(const DevBuf&) = delete;
+	~DevBuf() {
+		if (p) cudaFree(p);
+	}
+	template <class T> T* as() const { return (T*)p; }
+};
+
 struct ocb_ctx {
 	// GROUP context: non-empty `members` (single-device contexts owned by the group); none of the per-device fields below
 	// is used.  Host-buffer entry points shard their POI queue over the members; *_dev entry points are refused.
@@ -121,38 +135,29 @@ struct ocb_ctx {
 	long long launches = 0;
 
 	// 2D images
-	float* own_ref2 = nullptr;
-	float* own_tar2 = nullptr;
-	size_t own2_elems = 0;
+	DevBuf own2[2]; // {ref, tar} uploaded from the host
 	ocb::Image2D img2{ nullptr, nullptr, 0, 0 };
 	bool prepared2 = false;
 	bool prepared_nr2 = false;
 
 	// 3D images + tables
-	float* own_ref3 = nullptr;
-	float* own_tar3 = nullptr;
-	size_t own3_elems = 0;
-	float4* rg3 = nullptr;   // packed {ref, gx, gy, gz}
-	float* coef3 = nullptr;  // tricubic B-spline coefficients
-	float* tmp3 = nullptr;
-	size_t tab3_elems = 0;
+	DevBuf own3[2]; // {ref, tar} uploaded from the host
+	DevBuf rg3;     // float4: packed {ref, gx, gy, gz}
+	DevBuf coef3;   // tricubic B-spline coefficients
+	DevBuf tmp3;
 	ocb::Image3D img3{ nullptr, nullptr, nullptr, nullptr, 0, 0, 0 };
 	bool prepared3 = false;
 
 	// FFT
 	std::map<int, float2*> twiddles;
-	float2* fft_scratch = nullptr;
-	size_t fft_scratch_elems = 0;
+	DevBuf fft_scratch; // float2
 
 	int* d_counter = nullptr; // work-queue heads of the persistent kernels
 
 	// POI staging
-	float* d_poi = nullptr;
-	size_t d_poi_bytes = 0;
-	unsigned char* d_u8 = nullptr; // staging for 8-bit image uploads
-	size_t d_u8_bytes = 0;
-	float* d_off = nullptr; // centre offsets (2 floats per POI)
-	size_t d_off_bytes = 0;
+	DevBuf d_poi;
+	DevBuf d_u8;  // staging for 8-bit image uploads
+	DevBuf d_off; // centre offsets (2 floats per POI)
 	// host-queue calls on large 2D queues are split into chunks whose H2D copy, kernel and D2H copy run on separate
 	// streams, so the PCIe transfers of one chunk overlap the kernel of another
 	cudaStream_t pipe[4] = { nullptr, nullptr, nullptr, nullptr };
@@ -162,12 +167,9 @@ struct ocb_ctx {
 	cudaEvent_t band_done[4] = { nullptr, nullptr, nullptr, nullptr };
 	int band_end[4] = { 0, 0, 0, 0 }; // first row NOT covered once band_done[b] has fired
 	bool bands_fresh = false;         // nothing has been enqueued on `stream` since the banded upload
-	float* d_cand = nullptr; // EpipolarSearch candidate queue
-	size_t d_cand_bytes = 0;
-	void* d_strain_ws = nullptr; // Strain: sort keys / compact neighbour arrays / cub scratch
-	size_t d_strain_ws_bytes = 0;
-	float* d_stereo = nullptr; // stereo reconstruction / undistortion: staged points
-	size_t d_stereo_bytes = 0;
+	DevBuf d_cand;      // EpipolarSearch candidate queue
+	DevBuf d_strain_ws; // Strain: sort keys / compact neighbour arrays / cub scratch
+	DevBuf d_stereo;    // stereo reconstruction / undistortion: staged points
 };
 
 // One camera's distortion map (Calibration::prepare).  `owner` is the context the caller made it with (a group or a single
@@ -203,6 +205,22 @@ static int ensure_device(ocb_ctx* ctx) {
 	return OCB_OK;
 }
 
+// Make b hold at least `bytes` (on ctx's device, which must be current).  It only grows, and its contents are not kept across
+// a growth.  Work already enqueued on ctx->stream may still use the old allocation, so the stream is drained before it is
+// released.  If the allocation fails, b is left empty and the next call tries again.
+static int grow(ocb_ctx* ctx, DevBuf& b, size_t bytes) {
+	if (bytes <= b.bytes) return OCB_OK;
+	if (b.p) {
+		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		cudaFree(b.p);
+		b.p = nullptr;
+		b.bytes = 0;
+	}
+	OCB_CUDA(ctx, cudaMalloc(&b.p, bytes));
+	b.bytes = bytes;
+	return OCB_OK;
+}
+
 static int get_twiddles(ocb_ctx* ctx, int n, const float2** out) {
 	auto it = ctx->twiddles.find(n);
 	if (it != ctx->twiddles.end()) {
@@ -222,28 +240,6 @@ static int get_twiddles(ocb_ctx* ctx, int n, const float2** out) {
 	return OCB_OK;
 }
 
-static int stage_pois(ocb_ctx* ctx, const void* host, size_t bytes) {
-	if (bytes > ctx->d_poi_bytes) {
-		if (ctx->d_poi) cudaFree(ctx->d_poi);
-		ctx->d_poi = nullptr;
-		ctx->d_poi_bytes = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->d_poi, bytes));
-		ctx->d_poi_bytes = bytes;
-	}
-	OCB_CUDA(ctx, cudaMemcpyAsync(ctx->d_poi, host, bytes, cudaMemcpyHostToDevice, ctx->stream));
-	return OCB_OK;
-}
-
-static int unstage_pois(ocb_ctx* ctx, void* host, size_t bytes) {
-	OCB_CUDA(ctx, cudaMemcpyAsync(host, ctx->d_poi, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-	OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	return OCB_OK;
-}
-
-// Host-queue driver for the per-POI independent 2D operators: stage -> dev_call(d_queue, n, first) -> unstage.
-// Queues of >= OCB_PIPE_MIN records are processed in 4 chunks on 4 internal streams (each chunk: H2D, kernel, D2H), which
-// hides most of the POI traffic behind the kernels; results do not depend on the split (the POIs are independent).
-// dev_call launches on ctx->stream with ctx->d_counter, both of which are redirected per chunk.
 static const size_t OCB_PIPE_MIN = 16384;
 // Device-visible address of a host queue that is page-locked (cudaHostAlloc / cudaHostRegister / ocb_host_alloc), else NULL.
 static float* mapped_queue(const void* host) {
@@ -257,33 +253,55 @@ static float* mapped_queue(const void* host) {
 }
 
 static const int OCB_BANDS = 4;
-// fftcc_radius_y > 0: the call is FFT-CC right after a banded image upload -- a chunk only waits for the bands its windows touch
+
+// How a host-queue entry point moves its records:
+//   entry point                                         pipeline  in_place                    band_ry
+//   fftcc2d                                             yes       if the w32 kernel runs      ry
+//   icgn2d1/2, icgn2d_ex (each radius group), iclm2d    yes       yes                         0
+//   nr2d1                                               yes       no                          0
+//   fftcc3d, icgn3d1, epipolar_search2d, strain         no        no                          0
+struct QueuePolicy {
+	// Queues of >= OCB_PIPE_MIN records are processed in 4 chunks on 4 internal streams (each chunk: H2D, kernel, D2H), which
+	// hides most of the POI traffic behind the kernels.  Only for operators whose POIs are independent, so that results do not
+	// depend on the split.
+	bool pipeline;
+	// A page-locked queue is not copied at all: the kernels read each record and write its results straight through PCIe, which
+	// also keeps the copy engines free for the image upload.  Only for kernels that store a record with one coalesced write.
+	bool in_place;
+	// > 0: the call is FFT-CC with this y radius.  Right after a banded image upload, a chunk only waits for the bands its
+	// windows touch.
+	int band_ry;
+};
+static const QueuePolicy STAGED = { false, false, 0 }, PIPELINED = { true, false, 0 }, PIPELINED_IN_PLACE = { true, true, 0 };
+
+// Host-queue driver: checks the arguments, runs dev_call(d_queue, count, first) over the n records of rec_floats floats in
+// `host` as `policy` says, and returns once the results are back in `host`.  dev_call launches on ctx->stream with
+// ctx->d_counter, both of which are redirected per chunk of a pipelined queue.  `what` names the entry point in errors.
 template <class F>
-static int run_host_queue_2d(ocb_ctx* ctx, void* host, size_t n, F dev_call, bool allow_mapped = false, int fftcc_radius_y = 0) {
-	const size_t rec = OCB_POI2D_FLOATS * sizeof(float);
+static int run_host_queue(ocb_ctx* ctx, const char* what, void* host, size_t n, size_t rec_floats, F dev_call, QueuePolicy policy) {
+	if (!ctx || (!host && n)) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
+	if (n == 0) return OCB_OK;
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	const size_t rec = rec_floats * sizeof(float);
 	int rc;
-	const bool banded = fftcc_radius_y > 0 && ctx->bands_fresh && ctx->stream == ctx->own_stream;
+	const bool banded = policy.band_ry > 0 && ctx->bands_fresh && ctx->stream == ctx->own_stream;
 	ctx->bands_fresh = false;
-	// A page-locked queue is not copied at all: the kernels read each 100-byte record and write its results straight through
-	// PCIe (one coalesced load, one coalesced store per POI), which also keeps the copy engines free for the image upload.
-	float* const mapped = allow_mapped ? mapped_queue(host) : nullptr; // (only kernels that store a record with one coalesced write)
+	float* const mapped = policy.in_place ? mapped_queue(host) : nullptr;
 	if (mapped && !(banded && n >= OCB_PIPE_MIN)) {
 		if ((rc = dev_call(mapped, n, (size_t)0))) return rc;
 		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 		return OCB_OK;
 	}
-	if (n < OCB_PIPE_MIN || getenv("OCB_NO_PIPELINE")) {
-		if ((rc = stage_pois(ctx, host, n * rec))) return rc;
-		if ((rc = dev_call((float*)ctx->d_poi, n, (size_t)0))) return rc;
-		return unstage_pois(ctx, host, n * rec);
+	if (!policy.pipeline || n < OCB_PIPE_MIN || getenv("OCB_NO_PIPELINE")) {
+		if ((rc = grow(ctx, ctx->d_poi, n * rec))) return rc;
+		float* const d = ctx->d_poi.as<float>();
+		OCB_CUDA(ctx, cudaMemcpyAsync(d, host, n * rec, cudaMemcpyHostToDevice, ctx->stream));
+		if ((rc = dev_call(d, n, (size_t)0))) return rc;
+		OCB_CUDA(ctx, cudaMemcpyAsync(host, d, n * rec, cudaMemcpyDeviceToHost, ctx->stream));
+		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		return OCB_OK;
 	}
-	if (!mapped && n * rec > ctx->d_poi_bytes) {
-		if (ctx->d_poi) cudaFree(ctx->d_poi);
-		ctx->d_poi = nullptr;
-		ctx->d_poi_bytes = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->d_poi, n * rec));
-		ctx->d_poi_bytes = n * rec;
-	}
+	if (!mapped && (rc = grow(ctx, ctx->d_poi, n * rec))) return rc;
 	const int K = 4;
 	if (!ctx->pipe_ready) {
 		OCB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->pipe_ready, cudaEventDisableTiming));
@@ -298,7 +316,7 @@ static int run_host_queue_2d(ocb_ctx* ctx, void* host, size_t n, F dev_call, boo
 		const size_t a = n * (size_t)c / K, b = n * (size_t)(c + 1) / K;
 		if (b == a) continue;
 		char* h = (char*)host + a * rec;
-		float* d = mapped ? mapped + a * OCB_POI2D_FLOATS : ctx->d_poi + a * OCB_POI2D_FLOATS;
+		float* d = (mapped ? mapped : ctx->d_poi.as<float>()) + a * rec_floats;
 		cudaEvent_t gate = ctx->pipe_ready;
 		if (banded) { // last image row this chunk's windows read: max over its POIs of max(y, y + v0) + r (src/oc_fftcc.cpp:204-219)
 			float ymax = -1e30f;
@@ -311,7 +329,7 @@ static int run_host_queue_2d(ocb_ctx* ctx, void* host, size_t n, F dev_call, boo
 				ymax = top > ymax ? top : ymax;
 			}
 			if (finite) {
-				const int need = (int)ymax + fftcc_radius_y + 1;
+				const int need = (int)ymax + policy.band_ry + 1;
 				for (int k = 0; k < OCB_BANDS; k++)
 					if (ctx->band_end[k] >= need || k == OCB_BANDS - 1) { gate = ctx->band_done[k]; break; }
 			}
@@ -377,6 +395,14 @@ static int group_run(ocb_ctx* g, int used, F f) {
 template <class F>
 static int group_each(ocb_ctx* g, F f) {
 	return group_run(g, (int)g->members.size(), [f](ocb_ctx* m, int) { return f(m); });
+}
+// A prepare that only sets a flag runs on every member from the calling thread: no need to wake the members' threads.
+static int prepare_members(ocb_ctx* g, int (*prepare)(ocb_ctx*)) {
+	for (ocb_ctx* m : g->members) {
+		const int rc = prepare(m);
+		if (rc) { g->last_error = m->last_error; return rc; }
+	}
+	return OCB_OK;
 }
 // Contiguous block split of a host queue of n records of rec_bytes: member i gets records [n i / G, n (i+1) / G) and
 // copies them in and out of the caller's array itself (its own PCIe link, straight into the caller's slice).  Queues
@@ -444,30 +470,12 @@ static ocb_ctx* create_group(const int* devices, int n) {
 	return g;
 }
 
-// Image buffers of a single-device context (grow-only)
-static int ensure_buffers_2d(ocb_ctx* ctx, size_t elems) {
-	if (elems > ctx->own2_elems) {
-		cudaFree(ctx->own_ref2);
-		cudaFree(ctx->own_tar2);
-		ctx->own_ref2 = ctx->own_tar2 = nullptr;
-		ctx->own2_elems = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_ref2, elems * sizeof(float)));
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_tar2, elems * sizeof(float)));
-		ctx->own2_elems = elems;
-	}
-	return OCB_OK;
-}
-static int ensure_buffers_3d(ocb_ctx* ctx, size_t elems) {
-	if (elems > ctx->own3_elems) {
-		cudaFree(ctx->own_ref3);
-		cudaFree(ctx->own_tar3);
-		ctx->own_ref3 = ctx->own_tar3 = nullptr;
-		ctx->own3_elems = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_ref3, elems * sizeof(float)));
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_tar3, elems * sizeof(float)));
-		ctx->own3_elems = elems;
-	}
-	return OCB_OK;
+// Image pair buffers of a single-device context (dim 2 or 3), each grown to `elems` floats
+static DevBuf* own_pair(ocb_ctx* ctx, int dim) { return dim == 2 ? ctx->own2 : ctx->own3; }
+static int ensure_pair(ocb_ctx* ctx, int dim, size_t elems) {
+	DevBuf* pair = own_pair(ctx, dim);
+	const int rc = grow(ctx, pair[0], elems * sizeof(float));
+	return rc ? rc : grow(ctx, pair[1], elems * sizeof(float));
 }
 
 // GROUP upload of an image pair (elems floats each) into every member's buffers: member m copies ONLY slice m of both images
@@ -479,7 +487,7 @@ static int group_distribute_pair(ocb_ctx* g, const float* ref, const float* tar,
 	int rc = OCB_OK;
 	for (ocb_ctx* m : g->members) { // buffers first: a peer may push into them as soon as the exchange starts
 		if (ensure_device(m)) return OCB_ERR_CUDA;
-		rc = dim == 2 ? ensure_buffers_2d(m, elems) : ensure_buffers_3d(m, elems);
+		rc = ensure_pair(m, dim, elems);
 		if (rc == OCB_OK && cudaEventRecord(m->ev_idle, m->stream) != cudaSuccess) rc = set_error(m, OCB_ERR_CUDA, "cudaEventRecord failed");
 		if (rc) {
 			g->last_error = m->last_error;
@@ -491,15 +499,16 @@ static int group_distribute_pair(ocb_ctx* g, const float* ref, const float* tar,
 		if (ensure_device(m)) return (int)OCB_ERR_CUDA;
 		const size_t a = (elems * (size_t)i / (size_t)G) / gran * gran, b = i + 1 == G ? elems : (elems * (size_t)(i + 1) / (size_t)G) / gran * gran;
 		const size_t len = (b - a) * sizeof(float);
-		float* mine[2] = { dim == 2 ? m->own_ref2 : m->own_ref3, dim == 2 ? m->own_tar2 : m->own_tar3 };
+		const DevBuf* mine = own_pair(m, dim);
 		const float* src[2] = { ref, tar };
 		if (len) {
-			for (int k = 0; k < 2; k++) OCB_CUDA(m, cudaMemcpyAsync(mine[k] + a, src[k] + a, len, cudaMemcpyHostToDevice, m->stream));
+			for (int k = 0; k < 2; k++) OCB_CUDA(m, cudaMemcpyAsync(mine[k].as<float>() + a, src[k] + a, len, cudaMemcpyHostToDevice, m->stream));
 			for (int jj = 1; jj < G; jj++) { // start with the next neighbour so that the pushes of all members spread over the peers
 				ocb_ctx* peer = g->members[(i + jj) % G];
 				OCB_CUDA(m, cudaStreamWaitEvent(m->stream, peer->ev_idle, 0)); // the peer is done with its old images
-				float* theirs[2] = { dim == 2 ? peer->own_ref2 : peer->own_ref3, dim == 2 ? peer->own_tar2 : peer->own_tar3 };
-				for (int k = 0; k < 2; k++) OCB_CUDA(m, cudaMemcpyPeerAsync(theirs[k] + a, peer->device, mine[k] + a, m->device, len, m->stream));
+				const DevBuf* theirs = own_pair(peer, dim);
+				for (int k = 0; k < 2; k++)
+					OCB_CUDA(m, cudaMemcpyPeerAsync(theirs[k].as<float>() + a, peer->device, mine[k].as<float>() + a, m->device, len, m->stream));
 			}
 		}
 		OCB_CUDA(m, cudaEventRecord(m->ev_pushed, m->stream));
@@ -661,29 +670,15 @@ void ocb_destroy(ocb_ctx* ctx) {
 	}
 	cudaSetDevice(ctx->device);
 	cudaDeviceSynchronize();
-	cudaFree(ctx->own_ref2);
-	cudaFree(ctx->own_tar2);
-	cudaFree(ctx->own_ref3);
-	cudaFree(ctx->own_tar3);
-	cudaFree(ctx->rg3);
-	cudaFree(ctx->coef3);
-	cudaFree(ctx->tmp3);
 	for (auto& kv : ctx->twiddles) cudaFree(kv.second);
-	cudaFree(ctx->fft_scratch);
-	cudaFree(ctx->d_poi);
-	cudaFree(ctx->d_off);
-	cudaFree(ctx->d_strain_ws);
-	cudaFree(ctx->d_cand);
-	cudaFree(ctx->d_stereo);
 	for (int i = 0; i < 4; i++)
 		if (ctx->pipe[i]) cudaStreamDestroy(ctx->pipe[i]);
 	if (ctx->pipe_ready) cudaEventDestroy(ctx->pipe_ready);
 	for (int i = 0; i < 4; i++)
 		if (ctx->band_done[i]) cudaEventDestroy(ctx->band_done[i]);
-	cudaFree(ctx->d_u8);
 	cudaFree(ctx->d_counter);
 	cudaStreamDestroy(ctx->own_stream);
-	delete ctx;
+	delete ctx; // frees the DevBuf members on this device
 }
 
 const char* ocb_last_error(const ocb_ctx* ctx) { return ctx ? ctx->last_error.c_str() : g_last_error.c_str(); }
@@ -734,7 +729,7 @@ int ocb_set_images_2d(ocb_ctx* ctx, const float* ref, const float* tar, int widt
 			int rc = group_distribute_pair(ctx, ref, tar, (size_t)width * height, 2);
 			if (rc) return rc;
 			for (ocb_ctx* m : ctx->members)
-				if ((rc = ocb_set_images_2d_dev(m, m->own_ref2, m->own_tar2, width, height))) return rc;
+				if ((rc = ocb_set_images_2d_dev(m, m->own2[0].as<float>(), m->own2[1].as<float>(), width, height))) return rc;
 			return OCB_OK;
 		}
 		return group_each(ctx, [=](ocb_ctx* m) { return ocb_set_images_2d(m, ref, tar, width, height, col_major); });
@@ -743,9 +738,11 @@ int ocb_set_images_2d(ocb_ctx* ctx, const float* ref, const float* tar, int widt
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
 	const size_t elems = (size_t)width * height;
 	{
-		const int rcb = ensure_buffers_2d(ctx, elems);
+		const int rcb = ensure_pair(ctx, 2, elems);
 		if (rcb) return rcb;
 	}
+	float* const own_ref = ctx->own2[0].as<float>();
+	float* const own_tar = ctx->own2[1].as<float>();
 	bool banded = false;
 	if (!col_major) {
 		if (ctx->stream == ctx->own_stream && elems >= ((size_t)1 << 20) && !getenv("OCB_NO_PIPELINE")) {
@@ -753,51 +750,49 @@ int ocb_set_images_2d(ocb_ctx* ctx, const float* ref, const float* tar, int widt
 				if (!ctx->band_done[b]) OCB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->band_done[b], cudaEventDisableTiming));
 				const size_t r0 = (size_t)height * b / OCB_BANDS, r1 = (size_t)height * (b + 1) / OCB_BANDS;
 				const size_t off = r0 * (size_t)width, len = (r1 - r0) * (size_t)width * sizeof(float);
-				OCB_CUDA(ctx, cudaMemcpyAsync(ctx->own_ref2 + off, ref + off, len, cudaMemcpyHostToDevice, ctx->stream));
-				OCB_CUDA(ctx, cudaMemcpyAsync(ctx->own_tar2 + off, tar + off, len, cudaMemcpyHostToDevice, ctx->stream));
+				OCB_CUDA(ctx, cudaMemcpyAsync(own_ref + off, ref + off, len, cudaMemcpyHostToDevice, ctx->stream));
+				OCB_CUDA(ctx, cudaMemcpyAsync(own_tar + off, tar + off, len, cudaMemcpyHostToDevice, ctx->stream));
 				OCB_CUDA(ctx, cudaEventRecord(ctx->band_done[b], ctx->stream));
 				ctx->band_end[b] = (int)r1;
 			}
 			banded = true;
 		} else {
-			OCB_CUDA(ctx, cudaMemcpyAsync(ctx->own_ref2, ref, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-			OCB_CUDA(ctx, cudaMemcpyAsync(ctx->own_tar2, tar, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+			OCB_CUDA(ctx, cudaMemcpyAsync(own_ref, ref, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+			OCB_CUDA(ctx, cudaMemcpyAsync(own_tar, tar, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 		}
 	} else {
-		float* tmp = nullptr;
-		OCB_CUDA(ctx, cudaMalloc(&tmp, elems * sizeof(float)));
+		DevBuf tmp; // freed on every way out of this block
+		const int rct = grow(ctx, tmp, elems * sizeof(float));
+		if (rct) return rct;
 		dim3 grid((width + 31) / 32, (height + 31) / 32), block(32, 8);
 		const float* src[2] = { ref, tar };
-		float* dst[2] = { ctx->own_ref2, ctx->own_tar2 };
+		float* dst[2] = { own_ref, own_tar };
 		for (int i = 0; i < 2; i++) {
-			OCB_CUDA(ctx, cudaMemcpyAsync(tmp, src[i], elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-			ocb::transpose_kernel<<<grid, block, 0, ctx->stream>>>(tmp, dst[i], width, height);
+			OCB_CUDA(ctx, cudaMemcpyAsync(tmp.p, src[i], elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+			ocb::transpose_kernel<<<grid, block, 0, ctx->stream>>>(tmp.as<float>(), dst[i], width, height);
 			ctx->launches++;
 		}
 		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		cudaFree(tmp);
 	}
-	const int rc_dev = ocb_set_images_2d_dev(ctx, ctx->own_ref2, ctx->own_tar2, width, height);
+	const int rc_dev = ocb_set_images_2d_dev(ctx, own_ref, own_tar, width, height);
 	ctx->bands_fresh = banded && rc_dev == OCB_OK;
 	return rc_dev;
 }
 
-// upload `elems` bytes twice (ref, tar) and widen into the context-owned float buffers dst_ref/dst_tar
-static int upload_u8_pair(ocb_ctx* ctx, const unsigned char* ref, const unsigned char* tar, size_t elems, float* dst_ref, float* dst_tar) {
+// upload `elems` bytes twice (ref, tar) and widen into the context-owned float pair of dimension `dim`
+static int upload_u8_pair(ocb_ctx* ctx, const unsigned char* ref, const unsigned char* tar, size_t elems, int dim) {
+	int rc = ensure_pair(ctx, dim, elems);
+	if (rc) return rc;
 	// the widening kernel reads uchar4: the second image starts at a 16-byte aligned offset whatever the pixel count
 	const size_t tar_off = (elems + 15) & ~(size_t)15;
-	if (tar_off + elems > ctx->d_u8_bytes) {
-		cudaFree(ctx->d_u8);
-		ctx->d_u8 = nullptr;
-		ctx->d_u8_bytes = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->d_u8, tar_off + elems));
-		ctx->d_u8_bytes = tar_off + elems;
-	}
-	OCB_CUDA(ctx, cudaMemcpyAsync(ctx->d_u8, ref, elems, cudaMemcpyHostToDevice, ctx->stream));
-	OCB_CUDA(ctx, cudaMemcpyAsync(ctx->d_u8 + tar_off, tar, elems, cudaMemcpyHostToDevice, ctx->stream));
+	if ((rc = grow(ctx, ctx->d_u8, tar_off + elems))) return rc;
+	unsigned char* const d_u8 = ctx->d_u8.as<unsigned char>();
+	const DevBuf* dst = own_pair(ctx, dim);
+	OCB_CUDA(ctx, cudaMemcpyAsync(d_u8, ref, elems, cudaMemcpyHostToDevice, ctx->stream));
+	OCB_CUDA(ctx, cudaMemcpyAsync(d_u8 + tar_off, tar, elems, cudaMemcpyHostToDevice, ctx->stream));
 	const int grid = ctx->sm_count * 8;
-	ocb::widen_u8_kernel<<<grid, 256, 0, ctx->stream>>>(ctx->d_u8, dst_ref, elems);
-	ocb::widen_u8_kernel<<<grid, 256, 0, ctx->stream>>>(ctx->d_u8 + tar_off, dst_tar, elems);
+	ocb::widen_u8_kernel<<<grid, 256, 0, ctx->stream>>>(d_u8, dst[0].as<float>(), elems);
+	ocb::widen_u8_kernel<<<grid, 256, 0, ctx->stream>>>(d_u8 + tar_off, dst[1].as<float>(), elems);
 	ctx->launches += 2;
 	OCB_CUDA(ctx, cudaGetLastError());
 	return OCB_OK;
@@ -807,19 +802,9 @@ int ocb_set_images_2d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned 
 	if (is_group(ctx)) return group_each(ctx, [=](ocb_ctx* m) { return ocb_set_images_2d_u8(m, ref, tar, width, height); });
 	if (!ctx || !ref || !tar || width < 5 || height < 5) return set_error(ctx, OCB_ERR_ARG, "set_images_2d_u8: bad arguments");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	const size_t elems = (size_t)width * height;
-	if (elems > ctx->own2_elems) {
-		cudaFree(ctx->own_ref2);
-		cudaFree(ctx->own_tar2);
-		ctx->own_ref2 = ctx->own_tar2 = nullptr;
-		ctx->own2_elems = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_ref2, elems * sizeof(float)));
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_tar2, elems * sizeof(float)));
-		ctx->own2_elems = elems;
-	}
-	int rc = upload_u8_pair(ctx, ref, tar, elems, ctx->own_ref2, ctx->own_tar2);
+	int rc = upload_u8_pair(ctx, ref, tar, (size_t)width * height, 2);
 	if (rc) return rc;
-	return ocb_set_images_2d_dev(ctx, ctx->own_ref2, ctx->own_tar2, width, height);
+	return ocb_set_images_2d_dev(ctx, ctx->own2[0].as<float>(), ctx->own2[1].as<float>(), width, height);
 }
 
 int ocb_set_images_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned char* tar, int dim_x, int dim_y, int dim_z) {
@@ -827,19 +812,9 @@ int ocb_set_images_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned 
 	if (!ctx || !ref || !tar || dim_x < 15 || dim_y < 15 || dim_z < 15)
 		return set_error(ctx, OCB_ERR_ARG, "set_images_3d_u8: bad arguments (each dimension must be >= 15)");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	const size_t elems = (size_t)dim_x * dim_y * dim_z;
-	if (elems > ctx->own3_elems) {
-		cudaFree(ctx->own_ref3);
-		cudaFree(ctx->own_tar3);
-		ctx->own_ref3 = ctx->own_tar3 = nullptr;
-		ctx->own3_elems = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_ref3, elems * sizeof(float)));
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_tar3, elems * sizeof(float)));
-		ctx->own3_elems = elems;
-	}
-	int rc = upload_u8_pair(ctx, ref, tar, elems, ctx->own_ref3, ctx->own_tar3);
+	int rc = upload_u8_pair(ctx, ref, tar, (size_t)dim_x * dim_y * dim_z, 3);
 	if (rc) return rc;
-	return ocb_set_images_3d_dev(ctx, ctx->own_ref3, ctx->own_tar3, dim_x, dim_y, dim_z);
+	return ocb_set_images_3d_dev(ctx, ctx->own3[0].as<float>(), ctx->own3[1].as<float>(), dim_x, dim_y, dim_z);
 }
 
 int ocb_set_images_3d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tar, int dim_x, int dim_y, int dim_z) {
@@ -857,7 +832,7 @@ int ocb_set_images_3d(ocb_ctx* ctx, const float* ref, const float* tar, int dim_
 			int rc = group_distribute_pair(ctx, ref, tar, (size_t)dim_x * dim_y * dim_z, 3);
 			if (rc) return rc;
 			for (ocb_ctx* m : ctx->members)
-				if ((rc = ocb_set_images_3d_dev(m, m->own_ref3, m->own_tar3, dim_x, dim_y, dim_z))) return rc;
+				if ((rc = ocb_set_images_3d_dev(m, m->own3[0].as<float>(), m->own3[1].as<float>(), dim_x, dim_y, dim_z))) return rc;
 			return OCB_OK;
 		}
 		return group_each(ctx, [=](ocb_ctx* m) { return ocb_set_images_3d(m, ref, tar, dim_x, dim_y, dim_z); });
@@ -866,21 +841,31 @@ int ocb_set_images_3d(ocb_ctx* ctx, const float* ref, const float* tar, int dim_
 		return set_error(ctx, OCB_ERR_ARG, "set_images_3d: bad arguments (each dimension must be >= 15)");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
 	const size_t elems = (size_t)dim_x * dim_y * dim_z;
-	if (elems > ctx->own3_elems) {
-		cudaFree(ctx->own_ref3);
-		cudaFree(ctx->own_tar3);
-		ctx->own_ref3 = ctx->own_tar3 = nullptr;
-		ctx->own3_elems = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_ref3, elems * sizeof(float)));
-		OCB_CUDA(ctx, cudaMalloc(&ctx->own_tar3, elems * sizeof(float)));
-		ctx->own3_elems = elems;
-	}
-	OCB_CUDA(ctx, cudaMemcpyAsync(ctx->own_ref3, ref, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-	OCB_CUDA(ctx, cudaMemcpyAsync(ctx->own_tar3, tar, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-	return ocb_set_images_3d_dev(ctx, ctx->own_ref3, ctx->own_tar3, dim_x, dim_y, dim_z);
+	const int rc = ensure_pair(ctx, 3, elems);
+	if (rc) return rc;
+	float* const own_ref = ctx->own3[0].as<float>();
+	float* const own_tar = ctx->own3[1].as<float>();
+	OCB_CUDA(ctx, cudaMemcpyAsync(own_ref, ref, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+	OCB_CUDA(ctx, cudaMemcpyAsync(own_tar, tar, elems * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+	return ocb_set_images_3d_dev(ctx, own_ref, own_tar, dim_x, dim_y, dim_z);
 }
 
 // ---- FFT-CC ----------------------------------------------------------------------------------
+// Which FFT-CC kernel runs: W32 is the register-FFT kernel specialised for the 32-point window (r = 16 on every axis), REG the
+// register FFT codelets for square / cubic windows of N = 2^a 3^b 5^c <= 64 points, GENERIC the shared-memory kernel for any
+// window whose prime factors are <= 31.  OCB_FFTCC2D_GENERIC / OCB_FFTCC3D_GENERIC select GENERIC for every window.
+enum class FftPath { W32, REG, GENERIC };
+static FftPath fftcc2d_path(int rx, int ry) {
+	if (getenv("OCB_FFTCC2D_GENERIC")) return FftPath::GENERIC;
+	if (rx == 16 && ry == 16) return FftPath::W32;
+	return rx == ry && ocb::fftcc2d_reg_supported(rx) ? FftPath::REG : FftPath::GENERIC;
+}
+static FftPath fftcc3d_path(int rx, int ry, int rz) {
+	if (getenv("OCB_FFTCC3D_GENERIC")) return FftPath::GENERIC;
+	if (rx == 16 && ry == 16 && rz == 16) return FftPath::W32;
+	return rx == ry && ry == rz && ocb::fftcc3d_reg_supported(rx) ? FftPath::REG : FftPath::GENERIC;
+}
+
 int ocb_fftcc2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry) {
 	OCB_NO_GROUP(ctx, "fftcc2d_dev");
 	if (!ctx || (!d_poi2d && n) || rx < 1 || ry < 1) return set_error(ctx, OCB_ERR_ARG, "fftcc2d: bad arguments");
@@ -888,43 +873,35 @@ int ocb_fftcc2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry) {
 	if (n == 0) return OCB_OK;
 	if (n > 0x7fffffffull) return set_error(ctx, OCB_ERR_ARG, "fftcc2d: too many POIs in one call");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	if (rx == 16 && ry == 16 && !getenv("OCB_FFTCC2D_GENERIC")) { // specialised register-FFT kernel for the 32x32 window
-		cudaError_t err32;
-		if (ocb::fftcc2d_w32_launch(ctx->img2, (float*)d_poi2d, n, ctx->sm_count, ctx->stream, &err32))
-			return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(err32));
-		ctx->launches++;
-		return OCB_OK;
-	}
-	if (rx == ry && ocb::fftcc2d_reg_supported(rx) && !getenv("OCB_FFTCC2D_GENERIC")) { // thread-per-row register FFTs, N = 2^a 3^b 5^c <= 64
-		cudaError_t errr;
-		if (ocb::fftcc2d_reg_launch(ctx->img2, (float*)d_poi2d, n, rx, ctx->sm_count, ctx->stream, &errr))
-			return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(errr));
-		ctx->launches++;
-		return OCB_OK;
-	}
-	ocb::FftAxis ax, ay;
-	if (!ocb::fft_plan_axis(2 * rx, &ax) || !ocb::fft_plan_axis(2 * ry, &ay))
-		return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: window size %dx%d has a prime factor > 31", 2 * rx, 2 * ry);
-	if (ocb::fftcc2d_smem_bytes(rx, ry) > ctx->smem_optin)
-		return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: %dx%d window needs %zu B of shared memory (> %zu)", 2 * rx, 2 * ry,
-			ocb::fftcc2d_smem_bytes(rx, ry), ctx->smem_optin);
-	const float2 *twx, *twy;
-	int rc;
-	if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy))) return rc;
+	float* const q = (float*)d_poi2d;
 	cudaError_t err;
-	if (ocb::fftcc2d_launch(ctx->img2, (float*)d_poi2d, n, rx, ry, ax, ay, twx, twy, ctx->sm_count, ctx->stream, &err))
-		return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(err));
+	int failed;
+	const FftPath path = fftcc2d_path(rx, ry);
+	if (path == FftPath::W32) {
+		failed = ocb::fftcc2d_w32_launch(ctx->img2, q, n, ctx->sm_count, ctx->stream, &err);
+	} else if (path == FftPath::REG) { // one thread per row
+		failed = ocb::fftcc2d_reg_launch(ctx->img2, q, n, rx, ctx->sm_count, ctx->stream, &err);
+	} else {
+		ocb::FftAxis ax, ay;
+		if (!ocb::fft_plan_axis(2 * rx, &ax) || !ocb::fft_plan_axis(2 * ry, &ay))
+			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: window size %dx%d has a prime factor > 31", 2 * rx, 2 * ry);
+		if (ocb::fftcc2d_smem_bytes(rx, ry) > ctx->smem_optin)
+			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: %dx%d window needs %zu B of shared memory (> %zu)", 2 * rx, 2 * ry,
+				ocb::fftcc2d_smem_bytes(rx, ry), ctx->smem_optin);
+		const float2 *twx, *twy;
+		int rc;
+		if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy))) return rc;
+		failed = ocb::fftcc2d_launch(ctx->img2, q, n, rx, ry, ax, ay, twx, twy, ctx->sm_count, ctx->stream, &err);
+	}
+	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(err));
 	ctx->launches++;
 	return OCB_OK;
 }
 
 int ocb_fftcc2d(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry) {
 	if (is_group(ctx) && poi2d) return group_shard(ctx, poi2d, n, OCB_POI2D_FLOATS * sizeof(float), OCB_GROUP_MIN_2D, [=](ocb_ctx* m, void* q, size_t c, size_t) { return ocb_fftcc2d(m, q, c, rx, ry); });
-	if (!ctx || (!poi2d && n)) return set_error(ctx, OCB_ERR_ARG, "fftcc2d: bad arguments");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	return run_host_queue_2d(ctx, poi2d, n, [&](float* d, size_t m, size_t) { return ocb_fftcc2d_dev(ctx, d, m, rx, ry); },
-		rx == 16 && ry == 16 && !getenv("OCB_FFTCC2D_GENERIC"), ry > 0 ? ry : 0);
+	const QueuePolicy policy = { true, fftcc2d_path(rx, ry) == FftPath::W32, ry > 0 ? ry : 0 };
+	return run_host_queue(ctx, "fftcc2d", poi2d, n, OCB_POI2D_FLOATS, [&](float* d, size_t m, size_t) { return ocb_fftcc2d_dev(ctx, d, m, rx, ry); }, policy);
 }
 
 int ocb_fftcc3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int rz) {
@@ -935,90 +912,52 @@ int ocb_fftcc3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int r
 	if (n > 0x7fffffffull) return set_error(ctx, OCB_ERR_ARG, "fftcc3d: too many POIs in one call");
 	if ((size_t)8 * rx * ry * rz > 0x7fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window too large");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	if (rx == 16 && ry == 16 && rz == 16 && !getenv("OCB_FFTCC3D_GENERIC")) { // specialised register-FFT kernel for the 32^3 window
-		int grid32 = ocb::fftcc3d_w32_grid(ctx->sm_count);
-		if ((size_t)grid32 > n) grid32 = (int)n;
-		const size_t need32 = (size_t)grid32 * 32768;
-		if (need32 > ctx->fft_scratch_elems) {
-			OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-			cudaFree(ctx->fft_scratch);
-			ctx->fft_scratch = nullptr;
-			ctx->fft_scratch_elems = 0;
-			OCB_CUDA(ctx, cudaMalloc(&ctx->fft_scratch, need32 * sizeof(float2)));
-			ctx->fft_scratch_elems = need32;
-		}
-		cudaError_t err32;
-		if (ocb::fftcc3d_w32_launch(ctx->img3, (float*)d_poi3d, n, ctx->fft_scratch, grid32, ctx->stream, &err32))
-			return set_error(ctx, OCB_ERR_CUDA, "fftcc3d launch failed: %s", cudaGetErrorString(err32));
-		ctx->launches++;
-		return OCB_OK;
-	}
-	if (rx == ry && ry == rz && ocb::fftcc3d_reg_supported(rx) && !getenv("OCB_FFTCC3D_GENERIC")) { // register FFT codelets, N = 2^a 3^b 5^c <= 64
-		int gridr = ocb::fftcc3d_reg_grid(rx, ctx->sm_count);
-		if ((size_t)gridr > n) gridr = (int)n;
-		const size_t needr = (size_t)gridr * 2 * 8 * rx * ry * rz; // two scratch volumes of (2r)^3 complex per CTA
-		if (needr > ctx->fft_scratch_elems) {
-			OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-			cudaFree(ctx->fft_scratch);
-			ctx->fft_scratch = nullptr;
-			ctx->fft_scratch_elems = 0;
-			OCB_CUDA(ctx, cudaMalloc(&ctx->fft_scratch, needr * sizeof(float2)));
-			ctx->fft_scratch_elems = needr;
-		}
-		cudaError_t errr;
-		if (ocb::fftcc3d_reg_launch(ctx->img3, (float*)d_poi3d, n, rx, ctx->fft_scratch, gridr, ctx->stream, &errr))
-			return set_error(ctx, OCB_ERR_CUDA, "fftcc3d launch failed: %s", cudaGetErrorString(errr));
-		ctx->launches++;
-		return OCB_OK;
-	}
+	const FftPath path = fftcc3d_path(rx, ry, rz);
 	ocb::FftAxis ax, ay, az;
-	if (!ocb::fft_plan_axis(2 * rx, &ax) || !ocb::fft_plan_axis(2 * ry, &ay) || !ocb::fft_plan_axis(2 * rz, &az))
-		return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window size has a prime factor > 31");
-	if (ocb::fftcc3d_smem_bytes(rx, ry, rz) > ctx->smem_optin)
-		return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window needs %zu B of shared memory (> %zu)", ocb::fftcc3d_smem_bytes(rx, ry, rz),
-			ctx->smem_optin);
-	const float2 *twx, *twy, *twz;
-	int rc;
-	if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy)) || (rc = get_twiddles(ctx, 2 * rz, &twz))) return rc;
-	int grid = ocb::fftcc3d_grid(rx, ry, rz, ctx->sm_count);
-	if ((size_t)grid > n) grid = (int)n;
-	const size_t need = (size_t)grid * 8 * rx * ry * rz;
-	if (need > ctx->fft_scratch_elems) {
-		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		cudaFree(ctx->fft_scratch);
-		ctx->fft_scratch = nullptr;
-		ctx->fft_scratch_elems = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->fft_scratch, need * sizeof(float2)));
-		ctx->fft_scratch_elems = need;
+	const float2 *twx = nullptr, *twy = nullptr, *twz = nullptr;
+	int grid, rc;
+	size_t cta_scratch; // float2 scratch elements per CTA
+	if (path == FftPath::W32) {
+		grid = ocb::fftcc3d_w32_grid(ctx->sm_count);
+		cta_scratch = 32768;
+	} else if (path == FftPath::REG) {
+		grid = ocb::fftcc3d_reg_grid(rx, ctx->sm_count);
+		cta_scratch = (size_t)2 * 8 * rx * ry * rz; // two scratch volumes of (2r)^3 complex
+	} else {
+		if (!ocb::fft_plan_axis(2 * rx, &ax) || !ocb::fft_plan_axis(2 * ry, &ay) || !ocb::fft_plan_axis(2 * rz, &az))
+			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window size has a prime factor > 31");
+		if (ocb::fftcc3d_smem_bytes(rx, ry, rz) > ctx->smem_optin)
+			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window needs %zu B of shared memory (> %zu)", ocb::fftcc3d_smem_bytes(rx, ry, rz),
+				ctx->smem_optin);
+		if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy)) || (rc = get_twiddles(ctx, 2 * rz, &twz))) return rc;
+		grid = ocb::fftcc3d_grid(rx, ry, rz, ctx->sm_count);
+		cta_scratch = (size_t)8 * rx * ry * rz;
 	}
+	if ((size_t)grid > n) grid = (int)n;
+	if ((rc = grow(ctx, ctx->fft_scratch, (size_t)grid * cta_scratch * sizeof(float2)))) return rc;
+	float* const q = (float*)d_poi3d;
+	float2* const scratch = ctx->fft_scratch.as<float2>();
 	cudaError_t err;
-	if (ocb::fftcc3d_launch(ctx->img3, (float*)d_poi3d, n, rx, ry, rz, ax, ay, az, twx, twy, twz, ctx->fft_scratch, grid, ctx->stream, &err))
-		return set_error(ctx, OCB_ERR_CUDA, "fftcc3d launch failed: %s", cudaGetErrorString(err));
+	int failed;
+	if (path == FftPath::W32)
+		failed = ocb::fftcc3d_w32_launch(ctx->img3, q, n, scratch, grid, ctx->stream, &err);
+	else if (path == FftPath::REG)
+		failed = ocb::fftcc3d_reg_launch(ctx->img3, q, n, rx, scratch, grid, ctx->stream, &err);
+	else
+		failed = ocb::fftcc3d_launch(ctx->img3, q, n, rx, ry, rz, ax, ay, az, twx, twy, twz, scratch, grid, ctx->stream, &err);
+	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc3d launch failed: %s", cudaGetErrorString(err));
 	ctx->launches++;
 	return OCB_OK;
 }
 
 int ocb_fftcc3d(ocb_ctx* ctx, void* poi3d, size_t n, int rx, int ry, int rz) {
 	if (is_group(ctx) && poi3d) return group_shard(ctx, poi3d, n, OCB_POI3D_FLOATS * sizeof(float), OCB_GROUP_MIN_3D, [=](ocb_ctx* m, void* q, size_t c, size_t) { return ocb_fftcc3d(m, q, c, rx, ry, rz); });
-	if (!ctx || (!poi3d && n)) return set_error(ctx, OCB_ERR_ARG, "fftcc3d: bad arguments");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	int rc;
-	const size_t bytes = n * OCB_POI3D_FLOATS * sizeof(float);
-	if ((rc = stage_pois(ctx, poi3d, bytes))) return rc;
-	if ((rc = ocb_fftcc3d_dev(ctx, ctx->d_poi, n, rx, ry, rz))) return rc;
-	return unstage_pois(ctx, poi3d, bytes);
+	return run_host_queue(ctx, "fftcc3d", poi3d, n, OCB_POI3D_FLOATS, [&](float* d, size_t m, size_t) { return ocb_fftcc3d_dev(ctx, d, m, rx, ry, rz); }, STAGED);
 }
 
 // ---- IC-GN -----------------------------------------------------------------------------------
 int ocb_icgn2d_prepare(ocb_ctx* ctx) {
-	if (is_group(ctx)) { // flag only: no need to wake the members' threads
-		for (ocb_ctx* m : ctx->members) {
-			const int rc = ocb_icgn2d_prepare(m);
-			if (rc) { ctx->last_error = m->last_error; return rc; }
-		}
-		return OCB_OK;
-	}
+	if (is_group(ctx)) return prepare_members(ctx, ocb_icgn2d_prepare);
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
 	if (!ctx->img2.ref) return set_error(ctx, OCB_ERR_STATE, "icgn2d_prepare: images not set");
 	ctx->prepared2 = true; // gradients and bicubic weights are recomputed on chip per POI
@@ -1048,10 +987,8 @@ int ocb_icgn2d2_dev(ocb_ctx* ctx, void* d, size_t n, int rx, int ry, float conv,
 
 static int icgn2d_host(ocb_ctx* ctx, int np, void* poi2d, size_t n, int rx, int ry, float conv, float stop) {
 	if (is_group(ctx) && poi2d) return group_shard(ctx, poi2d, n, OCB_POI2D_FLOATS * sizeof(float), OCB_GROUP_MIN_2D, [=](ocb_ctx* m, void* q, size_t c, size_t) { return icgn2d_host(m, np, q, c, rx, ry, conv, stop); });
-	if (!ctx || (!poi2d && n)) return set_error(ctx, OCB_ERR_ARG, "icgn2d: bad arguments");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	return run_host_queue_2d(ctx, poi2d, n, [&](float* d, size_t m, size_t) { return icgn2d_dev(ctx, np, d, m, rx, ry, conv, stop); }, true);
+	return run_host_queue(ctx, "icgn2d", poi2d, n, OCB_POI2D_FLOATS, [&](float* d, size_t m, size_t) { return icgn2d_dev(ctx, np, d, m, rx, ry, conv, stop); },
+		PIPELINED_IN_PLACE);
 }
 int ocb_icgn2d1(ocb_ctx* ctx, void* p, size_t n, int rx, int ry, float conv, float stop) { return icgn2d_host(ctx, 6, p, n, rx, ry, conv, stop); }
 int ocb_icgn2d2(ocb_ctx* ctx, void* p, size_t n, int rx, int ry, float conv, float stop) { return icgn2d_host(ctx, 12, p, n, rx, ry, conv, stop); }
@@ -1066,18 +1003,14 @@ static int icgn2d_host_group(ocb_ctx* ctx, int np, float* poi2d, size_t n, int r
 	const float* d_off = nullptr;
 	if (offsets) {
 		const size_t ob = n * 2 * sizeof(float);
-		if (ob > ctx->d_off_bytes) {
-			cudaFree(ctx->d_off);
-			ctx->d_off = nullptr;
-			ctx->d_off_bytes = 0;
-			OCB_CUDA(ctx, cudaMalloc(&ctx->d_off, ob));
-			ctx->d_off_bytes = ob;
-		}
-		OCB_CUDA(ctx, cudaMemcpyAsync(ctx->d_off, offsets, ob, cudaMemcpyHostToDevice, ctx->stream));
-		d_off = ctx->d_off;
+		const int rc = grow(ctx, ctx->d_off, ob);
+		if (rc) return rc;
+		OCB_CUDA(ctx, cudaMemcpyAsync(ctx->d_off.p, offsets, ob, cudaMemcpyHostToDevice, ctx->stream));
+		d_off = ctx->d_off.as<float>();
 	}
-	return run_host_queue_2d(ctx, poi2d, n,
-		[&](float* d, size_t m, size_t first) { return icgn2d_dev(ctx, np, d, m, rx, ry, conv, stop, d_off ? d_off + 2 * first : nullptr); }, true);
+	return run_host_queue(ctx, "icgn2d_ex", poi2d, n, OCB_POI2D_FLOATS,
+		[&](float* d, size_t m, size_t first) { return icgn2d_dev(ctx, np, d, m, rx, ry, conv, stop, d_off ? d_off + 2 * first : nullptr); },
+		PIPELINED_IN_PLACE);
 }
 
 int ocb_icgn2d_ex(ocb_ctx* ctx, int order, void* poi2d, size_t n, int rx, int ry, float conv, float stop, const float* center_offsets,
@@ -1139,23 +1072,14 @@ int ocb_iclm2d(ocb_ctx* ctx, int order, void* poi2d, size_t n, int rx, int ry, f
 	if (is_group(ctx) && poi2d)
 		return group_shard(ctx, poi2d, n, OCB_POI2D_FLOATS * sizeof(float), OCB_GROUP_MIN_2D,
 			[=](ocb_ctx* m, void* q, size_t c, size_t) { return ocb_iclm2d(m, order, q, c, rx, ry, conv, stop, lambda, alpha, beta); });
-	if (!ctx || (!poi2d && n)) return set_error(ctx, OCB_ERR_ARG, "iclm2d: bad arguments");
 	if (order != 1 && order != 2) return set_error(ctx, OCB_ERR_ARG, "iclm2d: order must be 1 or 2");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	return run_host_queue_2d(ctx, poi2d, n,
-		[&](float* d, size_t m, size_t) { return ocb_iclm2d_dev(ctx, order, d, m, rx, ry, conv, stop, lambda, alpha, beta); }, true);
+	return run_host_queue(ctx, "iclm2d", poi2d, n, OCB_POI2D_FLOATS,
+		[&](float* d, size_t m, size_t) { return ocb_iclm2d_dev(ctx, order, d, m, rx, ry, conv, stop, lambda, alpha, beta); }, PIPELINED_IN_PLACE);
 }
 
 // ---- NR2D1 (SURVEY.md section 8(f) N2) ---------------------------------------------------------------
 int ocb_nr2d_prepare(ocb_ctx* ctx) {
-	if (is_group(ctx)) {
-		for (ocb_ctx* m : ctx->members) {
-			const int rc = ocb_nr2d_prepare(m);
-			if (rc) { ctx->last_error = m->last_error; return rc; }
-		}
-		return OCB_OK;
-	}
+	if (is_group(ctx)) return prepare_members(ctx, ocb_nr2d_prepare);
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
 	if (!ctx->img2.ref) return set_error(ctx, OCB_ERR_STATE, "nr2d_prepare: images not set");
 	ctx->prepared_nr2 = true; // target gradients and the three interpolants are evaluated on chip per POI
@@ -1180,10 +1104,8 @@ int ocb_nr2d1_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry, float c
 
 int ocb_nr2d1(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry, float conv, float stop) {
 	if (is_group(ctx) && poi2d) return group_shard(ctx, poi2d, n, OCB_POI2D_FLOATS * sizeof(float), OCB_GROUP_MIN_2D, [=](ocb_ctx* m, void* q, size_t c, size_t) { return ocb_nr2d1(m, q, c, rx, ry, conv, stop); });
-	if (!ctx || (!poi2d && n)) return set_error(ctx, OCB_ERR_ARG, "nr2d1: bad arguments");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	return run_host_queue_2d(ctx, poi2d, n, [&](float* d, size_t m, size_t) { return ocb_nr2d1_dev(ctx, d, m, rx, ry, conv, stop); });
+	return run_host_queue(ctx, "nr2d1", poi2d, n, OCB_POI2D_FLOATS, [&](float* d, size_t m, size_t) { return ocb_nr2d1_dev(ctx, d, m, rx, ry, conv, stop); },
+		PIPELINED);
 }
 
 // ---- EpipolarSearch candidate sweep (SURVEY.md section 8(f) N4) ----------------------------------------
@@ -1203,23 +1125,17 @@ int ocb_epipolar_search2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, const float
 	size_t block = ((size_t)1 << 22) / (size_t)slots;
 	if (block < 1) block = 1;
 	if (block > n) block = n;
-	const size_t need = block * (size_t)slots * OCB_POI2D_FLOATS * sizeof(float);
-	if (need > ctx->d_cand_bytes) {
-		if (ctx->d_cand) cudaFree(ctx->d_cand);
-		ctx->d_cand = nullptr;
-		ctx->d_cand_bytes = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->d_cand, need));
-		ctx->d_cand_bytes = need;
-	}
+	int rc = grow(ctx, ctx->d_cand, block * (size_t)slots * OCB_POI2D_FLOATS * sizeof(float));
+	if (rc) return rc;
+	float* const cand = ctx->d_cand.as<float>();
 	for (size_t p0 = 0; p0 < n; p0 += block) {
 		const size_t nb = n - p0 < block ? n - p0 : block;
 		ocb::epipolar_candidates_launch((const float*)d_poi2d, p0, nb, fundamental, parallax_x, parallax_y, search_radius, search_step, rx, ry, ctx->img2.w,
-			ctx->img2.h, slots, ctx->d_cand, ctx->sm_count, ctx->stream);
+			ctx->img2.h, slots, cand, ctx->sm_count, ctx->stream);
 		OCB_CUDA(ctx, cudaGetLastError());
 		ctx->launches++;
-		int rc = icgn2d_dev(ctx, 6, ctx->d_cand, nb * (size_t)slots, rx, ry, conv, stop);
-		if (rc) return rc;
-		ocb::epipolar_select_launch((float*)d_poi2d, p0, nb, slots, ctx->d_cand, ctx->sm_count, ctx->stream);
+		if ((rc = icgn2d_dev(ctx, 6, cand, nb * (size_t)slots, rx, ry, conv, stop))) return rc;
+		ocb::epipolar_select_launch((float*)d_poi2d, p0, nb, slots, cand, ctx->sm_count, ctx->stream);
 		OCB_CUDA(ctx, cudaGetLastError());
 		ctx->launches++;
 	}
@@ -1232,14 +1148,9 @@ int ocb_epipolar_search2d(ocb_ctx* ctx, void* poi2d, size_t n, const float* fund
 		return group_shard(ctx, poi2d, n, OCB_POI2D_FLOATS * sizeof(float), 256, [=](ocb_ctx* m, void* q, size_t c, size_t) {
 			return ocb_epipolar_search2d(m, q, c, fundamental, parallax_x, parallax_y, search_radius, search_step, rx, ry, conv, stop);
 		});
-	if (!ctx || (!poi2d && n)) return set_error(ctx, OCB_ERR_ARG, "epipolar_search2d: bad arguments");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	int rc;
-	const size_t bytes = n * OCB_POI2D_FLOATS * sizeof(float);
-	if ((rc = stage_pois(ctx, poi2d, bytes))) return rc;
-	if ((rc = ocb_epipolar_search2d_dev(ctx, ctx->d_poi, n, fundamental, parallax_x, parallax_y, search_radius, search_step, rx, ry, conv, stop))) return rc;
-	return unstage_pois(ctx, poi2d, bytes);
+	return run_host_queue(ctx, "epipolar_search2d", poi2d, n, OCB_POI2D_FLOATS, [&](float* d, size_t m, size_t) {
+		return ocb_epipolar_search2d_dev(ctx, d, m, fundamental, parallax_x, parallax_y, search_radius, search_step, rx, ry, conv, stop);
+	}, STAGED);
 }
 
 // ---- Strain (SURVEY.md section 8(f) N4) ---------------------------------------------------------------
@@ -1250,16 +1161,10 @@ static int strain_dev(ocb_ctx* ctx, int dim, void* d_poi, size_t n, float radius
 	if (n == 0) return OCB_OK;
 	if (n > 0x7fffffffull) return set_error(ctx, OCB_ERR_ARG, "strain: too many POIs in one call");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	const size_t need = ocb::strain_workspace_bytes(n);
-	if (need > ctx->d_strain_ws_bytes) {
-		if (ctx->d_strain_ws) cudaFree(ctx->d_strain_ws);
-		ctx->d_strain_ws = nullptr;
-		ctx->d_strain_ws_bytes = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->d_strain_ws, need));
-		ctx->d_strain_ws_bytes = need;
-	}
+	int rc = grow(ctx, ctx->d_strain_ws, ocb::strain_workspace_bytes(n));
+	if (rc) return rc;
 	cudaError_t err = cudaSuccess;
-	int rc = ocb::strain_launch(dim, (float*)d_poi, n, radius, min_neighbors, zncc_threshold, approximation, only, ctx->d_strain_ws, ctx->sm_count, ctx->stream,
+	rc = ocb::strain_launch(dim, (float*)d_poi, n, radius, min_neighbors, zncc_threshold, approximation, only, ctx->d_strain_ws.p, ctx->sm_count, ctx->stream,
 		&err, &ctx->launches);
 	if (rc) return set_error(ctx, OCB_ERR_CUDA, "strain launch failed: %s", cudaGetErrorString(err));
 	return OCB_OK;
@@ -1272,14 +1177,10 @@ static int strain_host(ocb_ctx* ctx, int dim, void* poi, size_t n, float radius,
 		if (rc) ctx->last_error = ctx->members[0]->last_error;
 		return rc;
 	}
-	if (!ctx || (!poi && n)) return set_error(ctx, OCB_ERR_ARG, "strain: bad arguments");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	int rc;
-	const size_t bytes = n * (dim == 2 ? OCB_POI2D_FLOATS : (dim == 3 ? OCB_POI3D_FLOATS : OCB_POI2DS_FLOATS)) * sizeof(float);
-	if ((rc = stage_pois(ctx, poi, bytes))) return rc;
-	if ((rc = strain_dev(ctx, dim, ctx->d_poi, n, radius, min_neighbors, zncc_threshold, approximation, only))) return rc;
-	return unstage_pois(ctx, poi, bytes);
+	const size_t rec_floats = dim == 2 ? OCB_POI2D_FLOATS : (dim == 3 ? OCB_POI3D_FLOATS : OCB_POI2DS_FLOATS);
+	return run_host_queue(ctx, "strain", poi, n, rec_floats, [&](float* d, size_t m, size_t) {
+		return strain_dev(ctx, dim, d, m, radius, min_neighbors, zncc_threshold, approximation, only);
+	}, STAGED);
 }
 
 int ocb_strain2d(ocb_ctx* ctx, void* poi2d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
@@ -1314,27 +1215,22 @@ int ocb_icgn3d_prepare(ocb_ctx* ctx) {
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
 	const int dx = ctx->img3.dx, dy = ctx->img3.dy, dz = ctx->img3.dz;
 	const size_t elems = (size_t)dx * dy * dz;
-	if (elems > ctx->tab3_elems) {
-		cudaFree(ctx->rg3);
-		cudaFree(ctx->coef3);
-		cudaFree(ctx->tmp3);
-		ctx->rg3 = nullptr;
-		ctx->coef3 = ctx->tmp3 = nullptr;
-		ctx->tab3_elems = 0;
-		OCB_CUDA(ctx, cudaMalloc(&ctx->rg3, elems * sizeof(float4)));
-		OCB_CUDA(ctx, cudaMalloc(&ctx->coef3, elems * sizeof(float)));
-		OCB_CUDA(ctx, cudaMalloc(&ctx->tmp3, elems * sizeof(float)));
-		ctx->tab3_elems = elems;
-	}
-	ocb::gradient3d_launch(ctx->img3.ref, ctx->rg3, dx, dy, dz, ctx->sm_count, ctx->stream);
+	int rc;
+	if ((rc = grow(ctx, ctx->rg3, elems * sizeof(float4))) || (rc = grow(ctx, ctx->coef3, elems * sizeof(float)))
+		|| (rc = grow(ctx, ctx->tmp3, elems * sizeof(float))))
+		return rc;
+	float4* const rg = ctx->rg3.as<float4>();
+	float* const coef = ctx->coef3.as<float>();
+	float* const tmp = ctx->tmp3.as<float>();
+	ocb::gradient3d_launch(ctx->img3.ref, rg, dx, dy, dz, ctx->sm_count, ctx->stream);
 	// TricubicBspline::prepare: x -> coefficient, y -> conv_buffer, z -> coefficient
-	ocb::prefilter3d_launch(ctx->img3.tar, ctx->coef3, dx, dy, dz, 0, ctx->sm_count, ctx->stream);
-	ocb::prefilter3d_launch(ctx->coef3, ctx->tmp3, dx, dy, dz, 1, ctx->sm_count, ctx->stream);
-	ocb::prefilter3d_launch(ctx->tmp3, ctx->coef3, dx, dy, dz, 2, ctx->sm_count, ctx->stream);
+	ocb::prefilter3d_launch(ctx->img3.tar, coef, dx, dy, dz, 0, ctx->sm_count, ctx->stream);
+	ocb::prefilter3d_launch(coef, tmp, dx, dy, dz, 1, ctx->sm_count, ctx->stream);
+	ocb::prefilter3d_launch(tmp, coef, dx, dy, dz, 2, ctx->sm_count, ctx->stream);
 	ctx->launches += 4;
 	OCB_CUDA(ctx, cudaGetLastError());
-	ctx->img3.rg = ctx->rg3;
-	ctx->img3.coef = ctx->coef3;
+	ctx->img3.rg = rg;
+	ctx->img3.coef = coef;
 	ctx->prepared3 = true;
 	return OCB_OK;
 }
@@ -1359,14 +1255,8 @@ int ocb_icgn3d1_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int r
 
 int ocb_icgn3d1(ocb_ctx* ctx, void* poi3d, size_t n, int rx, int ry, int rz, float conv, float stop) {
 	if (is_group(ctx) && poi3d) return group_shard(ctx, poi3d, n, OCB_POI3D_FLOATS * sizeof(float), OCB_GROUP_MIN_3D, [=](ocb_ctx* m, void* q, size_t c, size_t) { return ocb_icgn3d1(m, q, c, rx, ry, rz, conv, stop); });
-	if (!ctx || (!poi3d && n)) return set_error(ctx, OCB_ERR_ARG, "icgn3d1: bad arguments");
-	if (n == 0) return OCB_OK;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	int rc;
-	const size_t bytes = n * OCB_POI3D_FLOATS * sizeof(float);
-	if ((rc = stage_pois(ctx, poi3d, bytes))) return rc;
-	if ((rc = ocb_icgn3d1_dev(ctx, ctx->d_poi, n, rx, ry, rz, conv, stop))) return rc;
-	return unstage_pois(ctx, poi3d, bytes);
+	return run_host_queue(ctx, "icgn3d1", poi3d, n, OCB_POI3D_FLOATS, [&](float* d, size_t m, size_t) { return ocb_icgn3d1_dev(ctx, d, m, rx, ry, rz, conv, stop); },
+		STAGED);
 }
 
 int ocb_get_tables_3d(ocb_ctx* ctx, float* gx, float* gy, float* gz, float* coefficient) {
@@ -1378,9 +1268,9 @@ int ocb_get_tables_3d(ocb_ctx* ctx, float* gx, float* gy, float* gz, float* coef
 	float* dst[3] = { gx, gy, gz };
 	for (int i = 0; i < 3; i++) // de-interleave component i+1 of the packed {ref, gx, gy, gz} volume (inspection path, not hot)
 		if (dst[i])
-			OCB_CUDA(ctx, cudaMemcpy2DAsync(dst[i], sizeof(float), (const float*)ctx->rg3 + (i + 1), sizeof(float4), sizeof(float), elems,
+			OCB_CUDA(ctx, cudaMemcpy2DAsync(dst[i], sizeof(float), ctx->rg3.as<const float>() + (i + 1), sizeof(float4), sizeof(float), elems,
 				cudaMemcpyDeviceToHost, ctx->stream));
-	if (coefficient) OCB_CUDA(ctx, cudaMemcpyAsync(coefficient, ctx->coef3, elems * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+	if (coefficient) OCB_CUDA(ctx, cudaMemcpyAsync(coefficient, ctx->coef3.p, elems * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
 	OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return OCB_OK;
 }
@@ -1398,17 +1288,6 @@ static int relay_error(ocb_ctx* ctx, const ocb_ctx* exec, int rc) {
 static int calib_check(ocb_ctx* ctx, const ocb_calib* c, const char* what) {
 	if (!c) return set_error(ctx, OCB_ERR_ARG, "%s: null calibration handle", what);
 	if (c->owner != ctx) return set_error(ctx, OCB_ERR_ARG, "%s: calibration handle belongs to another context", what);
-	return OCB_OK;
-}
-
-static int ensure_stereo_buffer(ocb_ctx* x, size_t bytes) {
-	if (bytes > x->d_stereo_bytes) {
-		if (x->d_stereo) cudaFree(x->d_stereo);
-		x->d_stereo = nullptr;
-		x->d_stereo_bytes = 0;
-		OCB_CUDA(x, cudaMalloc(&x->d_stereo, bytes));
-		x->d_stereo_bytes = bytes;
-	}
 	return OCB_OK;
 }
 
@@ -1482,10 +1361,10 @@ int ocb_calib_undistort(ocb_ctx* ctx, const ocb_calib* calib, const float* intri
 	rc = [&]() -> int {
 		if (ensure_device(x)) return OCB_ERR_CUDA;
 		const size_t bytes = n * 2 * sizeof(float);
-		int r = ensure_stereo_buffer(x, 2 * bytes);
+		int r = grow(x, x->d_stereo, 2 * bytes);
 		if (r) return r;
-		float* d_pts = x->d_stereo;
-		float* d_out = x->d_stereo + 2 * n;
+		float* d_pts = x->d_stereo.as<float>();
+		float* d_out = d_pts + 2 * n;
 		OCB_CUDA(x, cudaMemcpyAsync(d_pts, pts, bytes, cudaMemcpyHostToDevice, x->stream));
 		ocb::calib_undistort_launch(calib->map_x, calib->map_y, calib->height, calib->width, intrinsics, d_pts, d_out, n, x->stream);
 		OCB_CUDA(x, cudaGetLastError());
@@ -1539,9 +1418,9 @@ int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* i
 	rc = [&]() -> int {
 		if (ensure_device(x)) return OCB_ERR_CUDA;
 		const size_t b2 = n * 2 * sizeof(float), b3 = n * 3 * sizeof(float);
-		int r = ensure_stereo_buffer(x, 2 * b2 + b3);
+		int r = grow(x, x->d_stereo, 2 * b2 + b3);
 		if (r) return r;
-		float* d1 = x->d_stereo;
+		float* d1 = x->d_stereo.as<float>();
 		float* d2 = d1 + 2 * n;
 		float* d3 = d2 + 2 * n;
 		OCB_CUDA(x, cudaMemcpyAsync(d1, pts1, b2, cudaMemcpyHostToDevice, x->stream));
