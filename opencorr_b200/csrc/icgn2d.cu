@@ -403,19 +403,25 @@ __global__ void __launch_bounds__(32 * WPP, NP == 6 ? (RC == 16 ? 12 : ICGN2D_MI
 		{
 			const int xg = x0 + lane;
 			const bool gx_ok = lane_on && xg >= 2 && xg < w - 2; // gradient maps are zero on a 2-pixel border (src/oc_gradient.cpp:42,46)
+			// the lane's column at rows r - 2 .. r + 2 (the pixel and its gy taps) rolls down in registers: one new pixel per row
+			const float* qn = T + r_lo * RW + lane_c + 2 + ex;
+			float cm2 = qn[0], cm1 = qn[RW], cc = qn[2 * RW], cp1 = qn[3 * RW];
+			qn += 4 * RW;
 			for (int r = r_lo; r < r_hi; r++) {
+				const float cp2 = *qn;
+				qn += RW;
 				const int yg = y0 + r;
 				const bool gy_ok = yg >= 2 && yg < h - 2;
 				const float yl = (float)(r - ry) - oy;
 				if (lane_on) {
 					const float* q = T + (r + 2) * RW + lane + 2 + ex;
-					const float R = q[0] - c0;
+					const float R = cc - c0;
 					float gx = 0.f, gy = 0.f;
 					if (gx_ok) gx = grad4(q[-2], q[-1], q[1], q[2]);
-					if (gy_ok) gy = grad4(q[-2 * RW], q[-RW], q[RW], q[2 * RW]);
+					if (gy_ok) gy = grad4(cm2, cm1, cp1, cp2);
 					{
 						float* pc = sC + 3 * (r * sw + lane);
-						pc[0] = q[0]; // raw R
+						pc[0] = cc; // raw R
 						pc[1] = gx;
 						pc[2] = gy;
 					}
@@ -443,6 +449,10 @@ __global__ void __launch_bounds__(32 * WPP, NP == 6 ? (RC == 16 ? 12 : ICGN2D_MI
 						}
 					}
 				}
+				cm2 = cm1;
+				cm1 = cc;
+				cc = cp1;
+				cp1 = cp2;
 			}
 		}
 		// expand with this lane's x powers: M[pair][mono(P,Q)] = x^P * accH[pair][Q]
@@ -898,10 +908,24 @@ __global__ void __launch_bounds__(32 * WPP, NP == 6 ? (RC == 16 ? 12 : ICGN2D_MI
 #pragma unroll
 					for (int i = 0; i < NPHI; i++) SD[a * NPHI + i] = phi_c(i) * xp[phi_p(i)] * G[a][phi_q(i)];
 			}
-			for (int idx = sub * 32 + lane; idx < ntail; idx += 32 * WPP) {
-				const int r = idx / rem, c = 32 + (idx - r * rem);
-				const float xl = (float)(c - rx) - ox, yl = (float)(r - ry) - oy;
-				float X, Y;
+			// tail columns (>= 32): lanes run over (row, column) pairs
+			auto tail_sums = [&](int r, int c, float xl, float yl, float t) {
+				tmin = fminf(tmin, t);
+				const float* pc = sC + 3 * (r * sw + c);
+				const float R = pc[0];
+				const float d = t - R;
+				d1 += d;
+				d2 = fmaf(d, d, d2);
+				rd = fmaf(R, d, rd);
+				float gd[2] = { pc[1] * d, pc[2] * d };
+#pragma unroll
+				for (int ii = 0; ii < NPHI; ii++) {
+					const float mm = phi_c(ii) * ipow(xl, phi_p(ii)) * ipow(yl, phi_q(ii));
+#pragma unroll
+					for (int a = 0; a < 2; a++) SD[a * NPHI + ii] = fmaf(gd[a], mm, SD[a * NPHI + ii]);
+				}
+			};
+			auto tail_xy = [&](float xl, float yl, float& X, float& Y) {
 				if constexpr (NP == 6) {
 					X = pcx + fmaf(A[0], xl, fmaf(A[1], yl, A[2]));
 					Y = pcy + fmaf(A[3], xl, fmaf(A[4], yl, A[5]));
@@ -910,25 +934,38 @@ __global__ void __launch_bounds__(32 * WPP, NP == 6 ? (RC == 16 ? 12 : ICGN2D_MI
 					X = pcx + fmaf(A[0], m0, fmaf(A[1], m1, fmaf(A[2], m2, fmaf(A[3], xl, fmaf(A[4], yl, A[5])))));
 					Y = pcy + fmaf(A[6], m0, fmaf(A[7], m1, fmaf(A[8], m2, fmaf(A[9], xl, fmaf(A[10], yl, A[11])))));
 				}
-				const bool fast = (X >= xlo) && (X < xhi) && (Y >= ylo) && (Y < yhi);
-				const bool ok = fast || ((X >= 1.f) && (Y >= 1.f) && (X < xmax) && (Y < ymax));
-				if (!ok && !LM) {
-					invalid = true;
-				} else {
-					const float t = whole ? T[wofs + r * TW + c] + 0.f : ok ? bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, fast) : -1.f;
-					tmin = fminf(tmin, t);
-					const float* pc = sC + 3 * (r * sw + c);
-					const float R = pc[0];
-					const float d = t - R;
-					d1 += d;
-					d2 = fmaf(d, d, d2);
-					rd = fmaf(R, d, rd);
-					float gd[2] = { pc[1] * d, pc[2] * d };
-#pragma unroll
-					for (int ii = 0; ii < NPHI; ii++) {
-						const float mm = phi_c(ii) * ipow(xl, phi_p(ii)) * ipow(yl, phi_q(ii));
-#pragma unroll
-						for (int a = 0; a < 2; a++) SD[a * NPHI + ii] = fmaf(gd[a], mm, SD[a * NPHI + ii]);
+			};
+			if (RC == 16 && iter_fast) {
+				// one tail column (rem == 1: the row is the index), and the corner test of iter_fast covers column 2r: every
+				// sample is valid and its support is in the tile, so no per-sample tests and no global-memory fallback
+				static_assert(RC != 16 || 2 * RC + 1 == 33, "the r = 16 tail is one column wide");
+				constexpr int c = 32;
+				const float xl = (float)(c - rx) - ox;
+				for (int r = sub * 32 + lane; r < sh; r += 32 * WPP) {
+					const float yl = (float)(r - ry) - oy;
+					float t;
+					if (whole) {
+						t = T[wofs + r * TW + c] + 0.f;
+					} else {
+						float X, Y;
+						tail_xy(xl, yl, X, Y);
+						t = bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, true);
+					}
+					tail_sums(r, c, xl, yl, t);
+				}
+			} else {
+				for (int idx = sub * 32 + lane; idx < ntail; idx += 32 * WPP) {
+					const int r = idx / rem, c = 32 + (idx - r * rem);
+					const float xl = (float)(c - rx) - ox, yl = (float)(r - ry) - oy;
+					float X, Y;
+					tail_xy(xl, yl, X, Y);
+					const bool fast = (X >= xlo) && (X < xhi) && (Y >= ylo) && (Y < yhi);
+					const bool ok = fast || ((X >= 1.f) && (Y >= 1.f) && (X < xmax) && (Y < ymax));
+					if (!ok && !LM) {
+						invalid = true;
+					} else {
+						const float t = whole ? T[wofs + r * TW + c] + 0.f : ok ? bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, fast) : -1.f;
+						tail_sums(r, c, xl, yl, t);
 					}
 				}
 			}
