@@ -811,6 +811,111 @@ namespace opencorr
 		}
 	};
 
+	// ------------------------------------------------------------------ src/oc_feature.h:46-63, src/oc_sift.h:71-155
+	class Feature3D
+	{
+	protected:
+		Image3D* ref_img = nullptr;
+		Image3D* tar_img = nullptr;
+
+	public:
+		virtual ~Feature3D() = default;
+		inline void setImages(Image3D& ref_img, Image3D& tar_img)
+		{
+			this->ref_img = &ref_img;
+			this->tar_img = &tar_img;
+		}
+		virtual void prepare() = 0;
+		virtual void compute() = 0;
+	};
+
+	struct Sift3dConfig
+	{
+		int n_octave_layers;
+		int n_octave;
+		int min_dimension;
+		float alpha;
+		float beta;
+		float gamma;
+		float sigma_source;
+		float sigma_base;
+		float gradient_threshold;
+		float truncate_threshold;
+	};
+
+	// SIFT3D on the GPU (ocb_sift3d).  The reference's helpers on host float*** layers (gaussianBlur, createGaussianPyramid,
+	// detectExtrema, ...) are not provided: the pyramid lives on the device, one octave at a time.
+	class SIFT3D : public Feature3D
+	{
+	protected:
+		Sift3dConfig sift_config;
+		float matching_ratio;
+		float physical_unit[3];
+
+	public:
+		std::vector<Point3D> ref_matched_kp;
+		std::vector<Point3D> tar_matched_kp;
+
+		SIFT3D()
+		{
+			sift_config.n_octave_layers = 3; // src/oc_sift.cpp:142-158
+			sift_config.n_octave = 0;
+			sift_config.min_dimension = 8;
+			sift_config.alpha = 0.1f;
+			sift_config.beta = 0.9f;
+			sift_config.gamma = 0.4f;
+			sift_config.sigma_source = 1.15f;
+			sift_config.sigma_base = 1.6f;
+			sift_config.gradient_threshold = 0.0000000001f;
+			sift_config.truncate_threshold = 0.2f * 128 / 768;
+			matching_ratio = 0.85f;
+			physical_unit[0] = physical_unit[1] = physical_unit[2] = 1.f;
+			b200::Engine::get().warm();
+		}
+		~SIFT3D() {}
+
+		Sift3dConfig getSiftConfig() const { return sift_config; }
+		float getPhysicalUnit(int dim) const { return (dim >= 0 && dim < 3) ? physical_unit[dim] : 0.f; }
+		float getMatchingRatio() const { return matching_ratio; }
+		void setSiftConfig(Sift3dConfig sift_config) { this->sift_config = sift_config; }
+		void setPhysicalUnit(float unit_x, float unit_y, float unit_z)
+		{
+			physical_unit[0] = unit_x;
+			physical_unit[1] = unit_y;
+			physical_unit[2] = unit_z;
+		}
+		void setMatchingRatio(float matching_ratio) { this->matching_ratio = matching_ratio; }
+		void prepare() {} // the icosahedron (:209-232) is built into the kernels
+		void compute()
+		{
+			b200::Engine& e = b200::Engine::get();
+			std::lock_guard<std::mutex> g(e.lock);
+			e.useImages(ref_img, tar_img, false);
+			const float cfg[OCB_SIFT3D_CONFIG_FLOATS] = { (float)sift_config.n_octave_layers, (float)sift_config.n_octave, (float)sift_config.min_dimension,
+				sift_config.alpha, sift_config.beta, sift_config.gamma, sift_config.sigma_source, sift_config.sigma_base, sift_config.gradient_threshold,
+				sift_config.truncate_threshold };
+			size_t n = 0, counts[2][3];
+			int n_octave = 0;
+			e.check(ocb_sift3d(e.context(), cfg, physical_unit, matching_ratio, &n, &n_octave));
+			sift_config.n_octave = n_octave;
+			for (int i = 0; i < 2; i++) e.check(ocb_sift3d_inspect(e.context(), i, counts[i], nullptr, nullptr, nullptr, nullptr));
+			std::cout << counts[0][2] << " features are extracted from the reference image." << std::endl;
+			std::cout << counts[1][2] << " features are extracted from the target image." << std::endl;
+			clear();
+			std::vector<float> r(3 * n), t(3 * n);
+			e.check(ocb_sift3d_get_matches(e.context(), r.data(), t.data()));
+			for (size_t i = 0; i < n; i++) {
+				ref_matched_kp.push_back(Point3D(r[3 * i], r[3 * i + 1], r[3 * i + 2]));
+				tar_matched_kp.push_back(Point3D(t[3 * i], t[3 * i + 1], t[3 * i + 2]));
+			}
+		}
+		void clear()
+		{
+			std::vector<Point3D>().swap(ref_matched_kp);
+			std::vector<Point3D>().swap(tar_matched_kp);
+		}
+	};
+
 	// ------------------------------------------------------------------ src/oc_icgn.h
 	namespace b200
 	{

@@ -221,6 +221,34 @@ int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* i
 int ocb_stereo_reconstruct_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
 	const float* intrinsics2, const float* projection2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n);
 
+/* ---- SIFT3D: SIFT3D::compute() src/oc_sift.cpp:234-293 on the volumes of ocb_set_images_3d / _u8 / _dev --------------------
+ * Extracts the keypoints of the reference and of the target volume (Gaussian pyramid :676-754 built one octave at a time, DoG
+ * extrema :795-847, orientation :849-1049, descriptors :1051-1249) and matches them (monodirectionalMatch :1251-1418).
+ * config: OCB_SIFT3D_CONFIG_FLOATS floats, the fields of Sift3dConfig (src/oc_sift.h:71-83) in order:
+ *   n_octave_layers, n_octave (ignored: computed, :683-684), min_dimension, alpha, beta, gamma, sigma_source, sigma_base,
+ *   gradient_threshold, truncate_threshold
+ * (the constructor's defaults, :142-152: 3, -, 8, 0.1, 0.9, 0.4, 1.15, 1.6, 1e-10, 0.2 * 128 / 768).
+ * unit_xyz: the physical voxel size (setPhysicalUnit :197-202); matching_ratio: setMatchingRatio (:204-207, default 0.85).
+ * Blocking.  *n_matched = number of matched pairs; *n_octave = the computed octave count (written back to sift_config by the
+ * reference).  Either pointer may be NULL.  Results stay in the context until the next ocb_sift3d call.  Where the reference is
+ * undefined (a mirrored blur index still out of range, reads past the end of its match list) DESIGN.md defines the result.
+ * On a GROUP context the first member runs it.  There is no CPU path. */
+#define OCB_SIFT3D_CONFIG_FLOATS 10
+#define OCB_SIFT3D_KP_FLOATS 18 /* coor_layer xyz, coor_img xyz, octave, layer, scale, R[9] (rows q0, q1, q0 x q1) */
+#define OCB_SIFT3D_DESC_FLOATS 768
+#define OCB_SIFT3D_STAGES 10
+int ocb_sift3d(ocb_ctx* ctx, const float* config, const float* unit_xyz, float matching_ratio, size_t* n_matched, int* n_octave);
+/* The matched pairs: ref_matched_kp / tar_matched_kp (coor_img of each keypoint, :1392-1417), n_matched x 3 floats each. */
+int ocb_sift3d_get_matches(ocb_ctx* ctx, float* ref_xyz, float* tar_xyz);
+/* Inspection of one image's products (image 0 = reference, 1 = target) for parity tests.  counts[3] = { candidates, max_abs
+ * entries, keypoints }; any array may be NULL (call once with NULLs to size them).  candidates: 5 ints each (octave, layer, z, y,
+ * x) in the reference's push order; max_abs: one per DoG layer, octave-major (n_octave x (n_octave_layers + 2)); keypoints:
+ * OCB_SIFT3D_KP_FLOATS each, the kept candidates in order; descriptors: 768 floats each. */
+int ocb_sift3d_inspect(ocb_ctx* ctx, int image, size_t* counts, int* candidates, float* max_abs, float* keypoints, float* descriptors);
+/* Milliseconds of the last ocb_sift3d per stage (CUDA events; the host post-pass on the host clock): ref pyramid, extrema,
+ * orientation, descriptors; tar the same four; matching (distance kernels and the copy of the top-2 table); host post-pass. */
+int ocb_sift3d_stage_times(ocb_ctx* ctx, float* ms);
+
 /* ---- inspection (parity tests of the prepare() products) ----------------------------------- */
 /* Copy the device tables built by ocb_icgn3d_prepare() to host buffers of dim_x*dim_y*dim_z
  * floats each; any pointer may be NULL. */

@@ -80,6 +80,10 @@ SIGNATURES = {
     "ocb_calib_undistort": (_i, [_vp, _vp, _vp, _vp, _vp, _sz]),
     "ocb_stereo_reconstruct": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz]),
     "ocb_stereo_reconstruct_dev": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz]),
+    "ocb_sift3d": (_i, [_vp, _vp, _vp, _f, ctypes.POINTER(_sz), ctypes.POINTER(_i)]),
+    "ocb_sift3d_get_matches": (_i, [_vp, _vp, _vp]),
+    "ocb_sift3d_inspect": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "ocb_sift3d_stage_times": (_i, [_vp, _vp]),
 }
 
 _lib = None

@@ -30,6 +30,17 @@ P3 = dict(x=0, y=1, z=2, u=3, ux=4, uy=5, uz=6, v=7, vx=8, vy=9, vz=10, w=11, wx
           exx=22, eyy=23, ezz=24, exy=25, eyz=26, ezx=27, subset_rx=28, subset_ry=29, subset_rz=30)
 
 
+# ---- SIFT3D (reference src/oc_sift.h:71-155) ----------------------------------------------------
+SIFT3D_CONFIG_FLOATS = 10
+SIFT3D_KP_FLOATS = 18
+# Sift3dConfig in field order, the constructor's defaults (src/oc_sift.cpp:142-152); n_octave is computed by compute()
+SIFT3D_CONFIG_FIELDS = ("n_octave_layers", "n_octave", "min_dimension", "alpha", "beta", "gamma", "sigma_source", "sigma_base",
+                        "gradient_threshold", "truncate_threshold")
+SIFT3D_DEFAULT_CONFIG = np.array([3, 0, 8, 0.1, 0.9, 0.4, 1.15, 1.6, 1e-10, np.float32(0.2) * 128 / 768], np.float32)
+SIFT3D_STAGES = ("ref_pyramid", "ref_extrema", "ref_orientation", "ref_descriptors", "tar_pyramid", "tar_extrema",
+                 "tar_orientation", "tar_descriptors", "matching", "host_post_pass")
+
+
 def make_poi2d(xy):
     """POI2D(Point2D) for every row of xy: location set, everything else cleared (oc_poi.h:112-135)."""
     xy = np.asarray(xy, dtype=np.float32).reshape(-1, 2)
@@ -245,6 +256,44 @@ class Engine:
 
     def icgn3d1_dev(self, d_q, n, rx, ry, rz, conv, stop):
         self._ck(self._lib.ocb_icgn3d1_dev(self._ctx, int(d_q), n, rx, ry, rz, conv, stop))
+
+    # SIFT3D --------------------------------------------------------------------------------------
+    def sift3d(self, config=None, unit=(1.0, 1.0, 1.0), matching_ratio=0.85):
+        """SIFT3D::compute() on the volumes of set_images_3d: returns (ref_matched_kp, tar_matched_kp, n_octave), the
+        matched keypoints as float32 [n, 3] (x, y, z) arrays.  config: the 10 floats of Sift3dConfig in field order
+        (SIFT3D_DEFAULT_CONFIG)."""
+        cfg = np.ascontiguousarray(SIFT3D_DEFAULT_CONFIG if config is None else config, dtype=np.float32).reshape(SIFT3D_CONFIG_FLOATS)
+        u = np.ascontiguousarray(unit, dtype=np.float32).reshape(3)
+        n = ctypes.c_size_t(0)
+        n_oct = ctypes.c_int(0)
+        self._ck(self._lib.ocb_sift3d(self._ctx, _vp(cfg), _vp(u), float(matching_ratio), ctypes.byref(n), ctypes.byref(n_oct)))
+        ref = np.empty((n.value, 3), np.float32)
+        tar = np.empty((n.value, 3), np.float32)
+        self._ck(self._lib.ocb_sift3d_get_matches(self._ctx, _vp(ref), _vp(tar)))
+        return ref, tar, int(n_oct.value)
+
+    def sift3d_inspect(self, image):
+        """Products of the last sift3d() for image 0 (reference) or 1 (target): dict of cand [n, 5] int32 (octave, layer, z,
+        y, x), max_abs [m] float32, kp [k, 18] float32, desc [k, 768] float32."""
+        counts = (ctypes.c_size_t * 3)()
+        self._ck(self._lib.ocb_sift3d_inspect(self._ctx, int(image), counts, None, None, None, None))
+        out = dict(cand=np.empty((counts[0], 5), np.int32), max_abs=np.empty(counts[1], np.float32),
+                   kp=np.empty((counts[2], SIFT3D_KP_FLOATS), np.float32), desc=np.empty((counts[2], 768), np.float32))
+        self._ck(self._lib.ocb_sift3d_inspect(self._ctx, int(image), counts, _vp(out["cand"]), _vp(out["max_abs"]), _vp(out["kp"]),
+                                              _vp(out["desc"])))
+        return out
+
+    def sift3d_inspect_counts(self, image):
+        """Number of keypoints the last sift3d() kept in image 0 (reference) or 1 (target)."""
+        counts = (ctypes.c_size_t * 3)()
+        self._ck(self._lib.ocb_sift3d_inspect(self._ctx, int(image), counts, None, None, None, None))
+        return int(counts[2])
+
+    def sift3d_stage_times(self):
+        """Milliseconds per stage of the last sift3d(), keyed by SIFT3D_STAGES."""
+        ms = np.zeros(len(SIFT3D_STAGES), np.float32)
+        self._ck(self._lib.ocb_sift3d_stage_times(self._ctx, _vp(ms)))
+        return dict(zip(SIFT3D_STAGES, ms.tolist()))
 
 
 _default_engines = {}
@@ -795,3 +844,73 @@ class ICGN3D1(_DVC):
 
     setIteration = set_iteration
     prepareRef = prepareTar = prepare
+
+
+class SIFT3D:
+    """SIFT3D (reference src/oc_sift.h:117-155, src/oc_sift.cpp:140-1418): volumetric keypoints of the reference and target
+    volumes, matched by descriptor distance with a ratio test.  compute() fills ref_matched_kp / tar_matched_kp, float32
+    [n, 3] arrays of (x, y, z) in voxels of the input volumes, and prints the reference's two lines."""
+
+    def __init__(self, engine=None):
+        self.engine = engine if engine is not None else default_engine()
+        self.sift_config = dict(zip(SIFT3D_CONFIG_FIELDS, SIFT3D_DEFAULT_CONFIG.tolist()))
+        for k in ("n_octave_layers", "n_octave", "min_dimension"):
+            self.sift_config[k] = int(self.sift_config[k])
+        self.matching_ratio = float(np.float32(0.85))
+        self.physical_unit = [1.0, 1.0, 1.0]
+        self.ref_img = None
+        self.tar_img = None
+        self._token = None
+        self.ref_matched_kp = np.empty((0, 3), np.float32)
+        self.tar_matched_kp = np.empty((0, 3), np.float32)
+
+    def set_images(self, ref_img, tar_img):
+        self.ref_img, self.tar_img = ref_img, tar_img
+        self.engine.set_images_3d(ref_img, tar_img)
+        self._token = self.engine.image_token
+
+    def get_sift_config(self):
+        return dict(self.sift_config)
+
+    def set_sift_config(self, sift_config):
+        self.sift_config = dict(sift_config)
+
+    def get_physical_unit(self, dim):
+        return self.physical_unit[dim] if dim in (0, 1, 2) else 0.0
+
+    def set_physical_unit(self, unit_x, unit_y, unit_z):
+        self.physical_unit = [float(unit_x), float(unit_y), float(unit_z)]
+
+    def get_matching_ratio(self):
+        return self.matching_ratio
+
+    def set_matching_ratio(self, matching_ratio):
+        self.matching_ratio = float(matching_ratio)
+
+    def prepare(self):
+        """The icosahedron of prepare() is built into the kernels; nothing to do."""
+
+    def clear(self):
+        self.ref_matched_kp = np.empty((0, 3), np.float32)
+        self.tar_matched_kp = np.empty((0, 3), np.float32)
+
+    def compute(self):
+        if self.ref_img is None:
+            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "SIFT3D: set_images() has not been called")
+        if self._token != self.engine.image_token:  # another operator replaced the engine's volumes
+            self.set_images(self.ref_img, self.tar_img)
+        cfg = np.array([self.sift_config[k] for k in SIFT3D_CONFIG_FIELDS], np.float32)
+        self.clear()
+        self.ref_matched_kp, self.tar_matched_kp, n_octave = self.engine.sift3d(cfg, self.physical_unit, self.matching_ratio)
+        self.sift_config["n_octave"] = n_octave
+        counts = [self.engine.sift3d_inspect_counts(i) for i in (0, 1)]
+        print("%d features are extracted from the reference image." % counts[0])
+        print("%d features are extracted from the target image." % counts[1])
+
+    setImages = set_images
+    getSiftConfig = get_sift_config
+    setSiftConfig = set_sift_config
+    getPhysicalUnit = get_physical_unit
+    setPhysicalUnit = set_physical_unit
+    getMatchingRatio = get_matching_ratio
+    setMatchingRatio = set_matching_ratio

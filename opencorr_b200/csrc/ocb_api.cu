@@ -170,6 +170,7 @@ struct ocb_ctx {
 	DevBuf d_cand;      // EpipolarSearch candidate queue
 	DevBuf d_strain_ws; // Strain: sort keys / compact neighbour arrays / cub scratch
 	DevBuf d_stereo;    // stereo reconstruction / undistortion: staged points
+	ocb::Sift3d* sift3d = nullptr; // SIFT3D working buffers and the products of the last ocb_sift3d call
 };
 
 // One camera's distortion map (Calibration::prepare).  `owner` is the context the caller made it with (a group or a single
@@ -677,6 +678,7 @@ void ocb_destroy(ocb_ctx* ctx) {
 	for (int i = 0; i < 4; i++)
 		if (ctx->band_done[i]) cudaEventDestroy(ctx->band_done[i]);
 	cudaFree(ctx->d_counter);
+	ocb::sift3d_destroy(ctx->sift3d);
 	cudaStreamDestroy(ctx->own_stream);
 	delete ctx; // frees the DevBuf members on this device
 }
@@ -1437,6 +1439,62 @@ int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* i
 		return OCB_OK;
 	}();
 	return relay_error(ctx, x, rc);
+}
+
+// ---- SIFT3D: SIFT3D::compute (src/oc_sift.cpp:234-293) --------------------------------------------------------------------
+// On a group context the first member runs it and keeps the results (one pair of volumes; see DESIGN.md section 6).
+static ocb_ctx* sift3d_exec(ocb_ctx* ctx) { return is_group(ctx) ? ctx->members[0] : ctx; }
+
+int ocb_sift3d(ocb_ctx* ctx, const float* config, const float* unit_xyz, float matching_ratio, size_t* n_matched, int* n_octave) {
+	if (!ctx || !config || !unit_xyz) return set_error(ctx, OCB_ERR_ARG, "sift3d: null argument");
+	ocb_ctx* x = sift3d_exec(ctx);
+	const int rc = [&]() -> int {
+		if (!x->img3.ref) return set_error(x, OCB_ERR_STATE, "sift3d: images not set");
+		for (int a = 0; a < 3; a++)
+			if (!(unit_xyz[a] > 0.f) || !std::isfinite(unit_xyz[a])) return set_error(x, OCB_ERR_ARG, "sift3d: physical units must be positive");
+		if (!(config[0] >= 1.f) || !(config[2] >= 1.f)) return set_error(x, OCB_ERR_ARG, "sift3d: n_octave_layers and min_dimension must be >= 1");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		if (!x->sift3d) x->sift3d = ocb::sift3d_create();
+		std::string err;
+		const int r = ocb::sift3d_run(x->sift3d, x->img3.ref, x->img3.tar, x->img3.dx, x->img3.dy, x->img3.dz, config, unit_xyz, matching_ratio, x->sm_count,
+			x->stream, &x->launches, &err);
+		if (r) return set_error(x, r == -2 ? OCB_ERR_ARG : OCB_ERR_CUDA, "%s", err.c_str());
+		if (n_matched) *n_matched = ocb::sift3d_n_matched(x->sift3d);
+		if (n_octave) *n_octave = ocb::sift3d_n_octave(x->sift3d, 1);
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+int ocb_sift3d_get_matches(ocb_ctx* ctx, float* ref_xyz, float* tar_xyz) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* x = sift3d_exec(ctx);
+	if (!x->sift3d) return relay_error(ctx, x, set_error(x, OCB_ERR_STATE, "sift3d_get_matches: ocb_sift3d has not run"));
+	ocb::sift3d_get_matches(x->sift3d, ref_xyz, tar_xyz);
+	return OCB_OK;
+}
+
+int ocb_sift3d_inspect(ocb_ctx* ctx, int image, size_t* counts, int* candidates, float* max_abs, float* keypoints, float* descriptors) {
+	if (!ctx || !counts || (image != 0 && image != 1)) return set_error(ctx, OCB_ERR_ARG, "sift3d_inspect: bad arguments");
+	ocb_ctx* x = sift3d_exec(ctx);
+	const int rc = [&]() -> int {
+		if (!x->sift3d) return set_error(x, OCB_ERR_STATE, "sift3d_inspect: ocb_sift3d has not run");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		std::string err;
+		if (ocb::sift3d_inspect(x->sift3d, image, counts, candidates, max_abs, keypoints, descriptors, x->stream, &err))
+			return set_error(x, OCB_ERR_CUDA, "%s", err.c_str());
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+int ocb_sift3d_stage_times(ocb_ctx* ctx, float* ms) {
+	if (!ctx || !ms) return set_error(ctx, OCB_ERR_ARG, "sift3d_stage_times: bad arguments");
+	ocb_ctx* x = sift3d_exec(ctx);
+	if (!x->sift3d) return relay_error(ctx, x, set_error(x, OCB_ERR_STATE, "sift3d_stage_times: ocb_sift3d has not run"));
+	const float* t = ocb::sift3d_stage_ms(x->sift3d);
+	std::copy(t, t + ocb::SIFT3D_STAGES, ms);
+	return OCB_OK;
 }
 
 } // extern "C"

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 
+#include <string>
+
 #include "ocb_common.cuh"
 
 namespace ocb {
@@ -32,6 +34,18 @@ inline bool fft_plan_axis(int n, FftAxis* ax) {
 	return true;
 }
 
+// sift3d.cu (SIFT3D feature extraction and matching; state kept between ocb_sift3d and the calls that read its results)
+struct Sift3d;
+enum { SIFT3D_STAGES = 10 }; // ref: pyramid, extrema, orientation, descriptors; tar: the same four; matching; host post-pass
+Sift3d* sift3d_create();
+void sift3d_destroy(Sift3d* s);
+int sift3d_run(Sift3d* s, const float* d_ref, const float* d_tar, int nx, int ny, int nz, const float* cfg, const float* unit, float ratio,
+	int sm_count, cudaStream_t stream, long long* launches, std::string* err);
+size_t sift3d_n_matched(const Sift3d* s);
+int sift3d_n_octave(const Sift3d* s, int which);
+const float* sift3d_stage_ms(const Sift3d* s);
+void sift3d_get_matches(const Sift3d* s, float* ref_xyz, float* tar_xyz);
+int sift3d_inspect(const Sift3d* s, int which, size_t* counts, int* cand, float* max_abs, float* kp, float* desc, cudaStream_t stream, std::string* err);
 // icgn2d.cu
 int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
 	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err);
