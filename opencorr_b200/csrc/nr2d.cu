@@ -208,25 +208,18 @@ __global__ void __launch_bounds__(128) nr2d1_kernel(Image2D img, float* __restri
 				bicubic_weights(X - xf, wx);
 				bicubic_weights(Y - yf, wy);
 				const int ix = (int)xf - 1, iy = (int)yf - 1;
-				float t = 0.f, gx = 0.f, gy = 0.f;
+				float t, gx = 0.f, gy = 0.f;
 				if (fast) {
 					const float* q = T + (iy - ty0) * TW + (ix - tx0);
 					const float2* g = G + (iy - gy0) * GW + (ix - gx0);
-#pragma unroll
-					for (int nn = 0; nn < 4; nn++) {
-						const float row = fmaf(q[nn * TW + 3], wx[3], fmaf(q[nn * TW + 2], wx[2], fmaf(q[nn * TW + 1], wx[1], q[nn * TW] * wx[0])));
-						const float2 g0 = g[nn * GW], g1 = g[nn * GW + 1], g2 = g[nn * GW + 2], g3 = g[nn * GW + 3];
-						const float rgx = fmaf(g3.x, wx[3], fmaf(g2.x, wx[2], fmaf(g1.x, wx[1], g0.x * wx[0])));
-						const float rgy = fmaf(g3.y, wx[3], fmaf(g2.y, wx[2], fmaf(g1.y, wx[1], g0.y * wx[0])));
-						t = fmaf(row, wy[nn], t);
-						gx = fmaf(rgx, wy[nn], gx);
-						gy = fmaf(rgy, wy[nn], gy);
-					}
+					t = bicubic_fold(wx, wy, [&](int n, int m) { return q[n * TW + m]; });
+					gx = bicubic_fold(wx, wy, [&](int n, int m) { return g[n * GW + m].x; });
+					gy = bicubic_fold(wx, wy, [&](int n, int m) { return g[n * GW + m].y; });
 				} else {
+					const float* q = tar + (size_t)iy * w + ix;
+					t = bicubic_fold(wx, wy, [&](int n, int m) { return __ldg(q + (size_t)n * w + m); });
 #pragma unroll 1
 					for (int nn = 0; nn < 4; nn++) {
-						const float* qq = tar + (size_t)(iy + nn) * w + ix;
-						const float row = fmaf(__ldg(qq + 3), wx[3], fmaf(__ldg(qq + 2), wx[2], fmaf(__ldg(qq + 1), wx[1], __ldg(qq) * wx[0])));
 						float rgx = 0.f, rgy = 0.f;
 #pragma unroll
 						for (int mm = 0; mm < 4; mm++) {
@@ -234,7 +227,6 @@ __global__ void __launch_bounds__(128) nr2d1_kernel(Image2D img, float* __restri
 							rgx = fmaf(gg.x, wx[mm], rgx);
 							rgy = fmaf(gg.y, wx[mm], rgy);
 						}
-						t = fmaf(row, wy[nn], t);
 						gx = fmaf(rgx, wy[nn], gx);
 						gy = fmaf(rgy, wy[nn], gy);
 					}

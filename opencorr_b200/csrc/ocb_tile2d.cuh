@@ -21,6 +21,20 @@ __device__ __forceinline__ void stage_tile(float* dst, const float* __restrict__
 	}
 }
 
+// The interpolant over one 4x4 block: each block row folded with the x weights, then the rows with the y weights, in this
+// FMA order.  pix(n, m) reads pixel m of block row n.  Every sampling path, and icgn2d_exact_negative's fused pre-check, goes
+// through this one fold, so the same block and weights give the same bits wherever they are evaluated.
+template <class Pix>
+__device__ __forceinline__ float bicubic_fold(const float* wx, const float* wy, Pix pix) {
+	float t = 0.f;
+#pragma unroll
+	for (int nn = 0; nn < 4; nn++) {
+		const float row = fmaf(pix(nn, 3), wx[3], fmaf(pix(nn, 2), wx[2], fmaf(pix(nn, 1), wx[1], pix(nn, 0) * wx[0])));
+		t = fmaf(row, wy[nn], t);
+	}
+	return t;
+}
+
 // Bicubic B-spline sample of the target at (X, Y), src/oc_cubic_bspline.cpp:134-181.
 // fast: the 4x4 support lies inside the staged tile.  Otherwise read the image (caller guarantees
 // 1 <= X < w-2, 1 <= Y < h-2).
@@ -31,24 +45,12 @@ __device__ __forceinline__ float bicubic_sample(const float* tile, int TW, int t
 	bicubic_weights(X - xf, wx);
 	bicubic_weights(Y - yf, wy);
 	const int ix = (int)xf - 1, iy = (int)yf - 1;
-	float t = 0.f;
 	if (fast) {
 		const float* q = tile + (iy - ty0) * TW + (ix - tx0);
-#pragma unroll
-		for (int nn = 0; nn < 4; nn++) {
-			float row = fmaf(q[nn * TW + 3], wx[3], fmaf(q[nn * TW + 2], wx[2], fmaf(q[nn * TW + 1], wx[1], q[nn * TW] * wx[0])));
-			t = fmaf(row, wy[nn], t);
-		}
-	} else {
-		const float* q = tar + (size_t)iy * w + ix;
-#pragma unroll
-		for (int nn = 0; nn < 4; nn++) {
-			const float* qq = q + (size_t)nn * w;
-			float row = fmaf(__ldg(qq + 3), wx[3], fmaf(__ldg(qq + 2), wx[2], fmaf(__ldg(qq + 1), wx[1], __ldg(qq) * wx[0])));
-			t = fmaf(row, wy[nn], t);
-		}
+		return bicubic_fold(wx, wy, [&](int n, int m) { return q[n * TW + m]; });
 	}
-	return t;
+	const float* q = tar + (size_t)iy * w + ix;
+	return bicubic_fold(wx, wy, [&](int n, int m) { return __ldg(q + (size_t)n * w + m); });
 }
 
 } // namespace ocb

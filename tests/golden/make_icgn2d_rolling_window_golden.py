@@ -1,6 +1,7 @@
 """Records tests/golden/icgn2d_rolling_window_parent.npz: the IC-GN records of every case in tests/rolling_window_cases.py,
-made by a library whose sampling loop reads the full 4x4 pixel block at every sample (no rolling window).  Needs a GPU and
-the whole-pixel fixture, whose images the cases use.
+made by a library whose sampling loop reads the full 4x4 pixel block at every sample (no rolling window).  The cases
+icgn2_r11 and iclm1_r13_wpp2 were added later and recorded by the rolling-window library, after checking that it reproduces
+every array already in the fixture byte for byte.  Needs a GPU and the whole-pixel fixture, whose images the cases use.
 
   OCB_LIB_PATH=<library without the rolling window> python tests/golden/make_icgn2d_rolling_window_golden.py [OUT.npz]
 

@@ -10,8 +10,9 @@ are kept small enough that the warped subset stays inside the staged target tile
 in x).  Larger ones, such as 1 + vy = 1.3, send the whole pass to the general loop, which reads each sample on its own.
 
 The 6-parameter cases cover the compiled-in radius 16 and generic ones (7: idle lanes; 19: a tail; 13 with two warps per POI:
-batches with one to three remaining rows), one and two warps per POI, centre offsets and ICLM2D1.  The 12-parameter kernels
-keep the full block load; their cases (radius 20, generic 11, two warps per POI, ICLM2D2) guard that loop on the same guesses.
+batches with one to three remaining rows), one and two warps per POI, centre offsets and ICLM2D1 with one and two warps per
+POI.  The 12-parameter kernels keep the full block load; their cases (radius 20, generic 11, each with one and two warps per
+POI, ICLM2D2) guard that loop on the same guesses.
 The images are those of the whole-pixel fixture (tests/golden/icgn2d_whole_pixel_parent.npz)."""
 import numpy as np
 
@@ -59,8 +60,10 @@ CASES = {
     "icgn1_r13_wpp2": ("speckle", "icgn", 1, 13, 2, wp.grid(13, 9)),
     "icgn2_r20": ("speckle2", "icgn", 2, 20, 1, wp.grid(20, 9)),
     "icgn2_r20_wpp2": ("speckle2", "icgn", 2, 20, 2, wp.grid(20, 9)),
+    "icgn2_r11": ("speckle2", "icgn", 2, 11, 1, wp.grid(11, 9)),
     "icgn2_r11_wpp2": ("speckle2", "icgn", 2, 11, 2, wp.grid(11, 9)),
     "iclm1_r16": ("speckle", "iclm", 1, 16, 1, wp.grid(16, 9)),
+    "iclm1_r13_wpp2": ("speckle", "iclm", 1, 13, 2, wp.grid(13, 9)),
     "iclm2_r20": ("speckle2", "iclm", 2, 20, 2, wp.grid(20, 9)),
     "offsets1_r16": ("speckle", "ex", 1, 16, 1, wp.grid(16, 9)),
     "offsets2_r20": ("speckle2", "ex", 2, 20, 1, wp.grid(20, 9)),
