@@ -151,6 +151,25 @@ int ocb_icgn2d_ex(ocb_ctx* ctx, int order, void* poi2d, size_t n, int rx, int ry
 	int self_adaptive);
 int ocb_icgn2d_ex_dev(ocb_ctx* ctx, int order, void* d_poi2d, size_t n, int rx, int ry, float conv, float stop, const float* d_center_offsets);
 
+/* ---- IC-GN over an image series: one reference, n_frames targets.  Replaces the loop a reference user writes over a load
+ *      series, carrying one queue from frame to frame:
+ *        for f: dic.setImages(ref, tar[f]) (src/oc_dic.cpp:22-26); icgn.prepare() (src/oc_icgn.cpp:138-142 / :679-683);
+ *               icgn.compute(queue) (:343-351 / :900-908)
+ *      Frame f's records are, bit for bit, what ocb_icgn2d1/2 gives on (ref, tars[f]) for frame f - 1's records (frame 0: the
+ *      seeds) in one launch over the same n POIs; a POI that fails in frame f keeps its code in every later frame.  The
+ *      reference subset of each POI (gradients, Hessian) is built once for the whole series.
+ * The series is context state of its own: the pair calls (ocb_set_images_2d*, ocb_icgn2d*) neither see nor disturb it.
+ * tars: n_frames row-major images, frame-major.  On a group context the first member holds the series and runs the calls.
+ * order = 1 (ICGN2D1) or 2 (ICGN2D2).  seeds: n POI2D records; out: n_frames x n POI2D records, frame-major (out[f n + i]),
+ *   not overlapping seeds.  A long series runs in chunks: the last frame's slice of out seeds the next chunk.
+ * The host variants copy (ocb_icgn2d_series blocks until out is filled); the _dev variants take BORROWED device pointers and
+ *   only enqueue.  Errors write nothing to out: OCB_ERR_STATE without a series, OCB_ERR_ARG for bad arguments or sizes,
+ *   OCB_ERR_UNSUPPORTED for radii past the shared-memory limit (as ocb_icgn2d1/2). */
+int ocb_set_series_2d(ocb_ctx* ctx, const float* ref, const float* tars, int n_frames, int width, int height);
+int ocb_set_series_2d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars, int n_frames, int width, int height);
+int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop);
+int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop);
+
 /* ---- IC-LM siblings (SURVEY.md section 8(f) N2): ICLM2D1::compute(std::vector<POI2D>&) src/oc_iclm.cpp:360-368
  *      (per POI :150-358) and ICLM2D2 :732-740 (:502-730).  Same prepare() as IC-GN (ocb_icgn2d_prepare).
  *      lambda, alpha, beta = DampingParameter (src/oc_iclm.h:32-37; defaults 100, 0.1, 10; setDamping()). */

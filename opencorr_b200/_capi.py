@@ -58,6 +58,10 @@ SIGNATURES = {
     "ocb_icgn3d1_dev": (_i, [_vp, _vp, _sz, _i, _i, _i, _f, _f]),
     "ocb_icgn2d_ex": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _vp, _i]),
     "ocb_icgn2d_ex_dev": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _vp]),
+    "ocb_set_series_2d": (_i, [_vp, _vp, _vp, _i, _i, _i]),
+    "ocb_set_series_2d_dev": (_i, [_vp, _vp, _vp, _i, _i, _i]),
+    "ocb_icgn2d_series": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f]),
+    "ocb_icgn2d_series_dev": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_iclm2d": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
     "ocb_iclm2d_dev": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
     "ocb_epipolar_search2d": (_i, [_vp, _vp, _sz, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f]),

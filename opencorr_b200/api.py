@@ -201,6 +201,31 @@ class Engine:
         self._ck(self._lib.ocb_icgn2d_ex(self._ctx, int(order), _vp(q), q.shape[0], rx, ry, conv, stop,
                                          _vp(off) if off is not None else None, int(bool(self_adaptive))))
 
+    def set_series_2d(self, ref, tars):
+        """An image series for icgn2d_series: ref (H, W) and tars (F, H, W), float32.  Kept apart from set_images_2d's pair."""
+        ref = np.ascontiguousarray(ref, dtype=np.float32)
+        tars = np.ascontiguousarray(tars, dtype=np.float32)
+        if ref.ndim != 2 or tars.ndim != 3 or tars.shape[1:] != ref.shape:
+            raise ValueError("ref must be (H, W) and tars (F, H, W)")
+        f, h, w = tars.shape
+        self._ck(self._lib.ocb_set_series_2d(self._ctx, _vp(ref), _vp(tars), f, w, h))
+        self._ck(self._lib.ocb_sync(self._ctx))
+        self._n_frames = f
+
+    def icgn2d_series(self, order, seeds, rx, ry, conv, stop):
+        """ICGN2D1 (order 1) / ICGN2D2 (order 2) over the series set by set_series_2d, frame f seeded by frame f - 1's records
+        (frame 0 by `seeds`, [n, 25]).  Returns the records of every frame, float32 (F, n, 25); seeds are not changed."""
+        _check_queue(seeds, POI2D_FLOATS)
+        n_frames = self._series_frames()
+        out = np.empty((n_frames, seeds.shape[0], POI2D_FLOATS), np.float32)
+        self._ck(self._lib.ocb_icgn2d_series(self._ctx, int(order), _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop))
+        return out
+
+    def _series_frames(self):
+        if getattr(self, "_n_frames", None) is None:
+            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn2d_series: no series set")
+        return self._n_frames
+
     def iclm2d(self, order, q, rx, ry, conv, stop, damping=(100.0, 0.1, 10.0)):
         """ICLM2D1 / ICLM2D2 (reference src/oc_iclm.cpp); damping = (lambda, alpha, beta)."""
         _check_queue(q, POI2D_FLOATS)
@@ -253,6 +278,15 @@ class Engine:
 
     def icgn2d2_dev(self, d_q, n, rx, ry, conv, stop):
         self._ck(self._lib.ocb_icgn2d2_dev(self._ctx, int(d_q), n, rx, ry, conv, stop))
+
+    def set_series_2d_dev(self, d_ref, d_tars, n_frames, width, height):
+        """Device pointers: ref (height x width) and the frame-major stack of n_frames targets; borrowed, not copied."""
+        self._ck(self._lib.ocb_set_series_2d_dev(self._ctx, int(d_ref), int(d_tars), n_frames, width, height))
+        self._n_frames = int(n_frames)
+
+    def icgn2d_series_dev(self, order, d_seeds, d_out, n, rx, ry, conv, stop):
+        """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
+        self._ck(self._lib.ocb_icgn2d_series_dev(self._ctx, int(order), int(d_seeds), int(d_out), n, rx, ry, conv, stop))
 
     def icgn3d1_dev(self, d_q, n, rx, ry, rz, conv, stop):
         self._ck(self._lib.ocb_icgn3d1_dev(self._ctx, int(d_q), n, rx, ry, rz, conv, stop))

@@ -140,6 +140,11 @@ struct ocb_ctx {
 	bool prepared2 = false;
 	bool prepared_nr2 = false;
 
+	// 2D image series (ocb_set_series_2d*): its own state, untouched by the pair calls.  series.tar is the frame-major stack.
+	DevBuf own_series[2]; // {ref, stack} uploaded from the host
+	ocb::Image2D series{ nullptr, nullptr, 0, 0 };
+	int series_frames = 0;
+
 	// 3D images + tables
 	DevBuf own3[2]; // {ref, tar} uploaded from the host
 	DevBuf rg3;     // float4: packed {ref, gx, gy, gz}
@@ -998,6 +1003,81 @@ int ocb_icgn2d2(ocb_ctx* ctx, void* p, size_t n, int rx, int ry, float conv, flo
 int ocb_icgn2d_ex_dev(ocb_ctx* ctx, int order, void* d_poi2d, size_t n, int rx, int ry, float conv, float stop, const float* d_center_offsets) {
 	if (order != 1 && order != 2) return set_error(ctx, OCB_ERR_ARG, "icgn2d_ex: order must be 1 or 2");
 	return icgn2d_dev(ctx, order == 1 ? 6 : 12, d_poi2d, n, rx, ry, conv, stop, d_center_offsets);
+}
+
+// ---- image series: one reference, n_frames targets, each frame seeded by the previous one ------------------------------
+// On a group context the first member holds the series and runs it.
+static int relay_error(ocb_ctx* ctx, const ocb_ctx* exec, int rc);
+static ocb_ctx* series_exec(ocb_ctx* ctx) { return is_group(ctx) ? ctx->members[0] : ctx; }
+
+int ocb_set_series_2d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars, int n_frames, int width, int height) {
+	OCB_NO_GROUP(ctx, "set_series_2d_dev");
+	if (!ctx || !d_ref || !d_tars || n_frames < 1 || width < 5 || height < 5) return set_error(ctx, OCB_ERR_ARG, "set_series_2d: bad arguments");
+	ctx->series = ocb::Image2D{ d_ref, d_tars, width, height };
+	ctx->series_frames = n_frames;
+	return OCB_OK;
+}
+
+int ocb_set_series_2d(ocb_ctx* ctx, const float* ref, const float* tars, int n_frames, int width, int height) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* x = series_exec(ctx);
+	const int rc = [&]() -> int {
+		if (!ref || !tars || n_frames < 1 || width < 5 || height < 5) return set_error(x, OCB_ERR_ARG, "set_series_2d: bad arguments");
+		const size_t elems = (size_t)width * height;
+		if ((size_t)n_frames > SIZE_MAX / sizeof(float) / elems) return set_error(x, OCB_ERR_ARG, "set_series_2d: series too large");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		int r;
+		if ((r = grow(x, x->own_series[0], elems * sizeof(float))) || (r = grow(x, x->own_series[1], (size_t)n_frames * elems * sizeof(float)))) return r;
+		OCB_CUDA(x, cudaMemcpyAsync(x->own_series[0].p, ref, elems * sizeof(float), cudaMemcpyHostToDevice, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(x->own_series[1].p, tars, (size_t)n_frames * elems * sizeof(float), cudaMemcpyHostToDevice, x->stream));
+		x->series = ocb::Image2D{ x->own_series[0].as<float>(), x->own_series[1].as<float>(), width, height };
+		x->series_frames = n_frames;
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop) {
+	OCB_NO_GROUP(ctx, "icgn2d_series_dev");
+	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1) return set_error(ctx, OCB_ERR_ARG, "icgn2d_series: bad arguments");
+	if (order != 1 && order != 2) return set_error(ctx, OCB_ERR_ARG, "icgn2d_series: order must be 1 or 2");
+	if (!ctx->series.ref) return set_error(ctx, OCB_ERR_STATE, "icgn2d_series: no series set");
+	if (n == 0) return OCB_OK;
+	if (n > 0x7fffffffull || (size_t)ctx->series_frames > SIZE_MAX / (n * OCB_POI2D_FLOATS * sizeof(float)))
+		return set_error(ctx, OCB_ERR_ARG, "icgn2d_series: too many POIs in one call");
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	cudaError_t err = cudaSuccess;
+	const int rc = ocb::icgn2d_series_launch(order == 1 ? 6 : 12, ctx->series, ctx->series_frames, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv,
+		stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter, ctx->stream, &err);
+	if (rc == -1) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
+	if (rc) return set_error(ctx, OCB_ERR_CUDA, "icgn2d_series launch failed: %s", cudaGetErrorString(err));
+	ctx->launches++;
+	return OCB_OK;
+}
+
+int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* x = series_exec(ctx);
+	const int rc = [&]() -> int {
+		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "icgn2d_series: bad arguments");
+		if (!x->series.ref) return set_error(x, OCB_ERR_STATE, "icgn2d_series: no series set");
+		if (n == 0) return ocb_icgn2d_series_dev(x, order, nullptr, nullptr, 0, rx, ry, conv, stop); // argument checks only
+		const size_t rec = OCB_POI2D_FLOATS * sizeof(float);
+		if (n > 0x7fffffffull || (size_t)x->series_frames + 1 > SIZE_MAX / (n * rec))
+			return set_error(x, OCB_ERR_ARG, "icgn2d_series: too many POIs in one call");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t out_bytes = (size_t)x->series_frames * n * rec;
+		int r;
+		if ((r = grow(x, x->d_poi, n * rec + out_bytes))) return r;
+		float* const d_seeds = x->d_poi.as<float>();
+		float* const d_out = d_seeds + n * OCB_POI2D_FLOATS;
+		OCB_CUDA(x, cudaMemcpyAsync(d_seeds, seeds, n * rec, cudaMemcpyHostToDevice, x->stream));
+		if ((r = ocb_icgn2d_series_dev(x, order, d_seeds, d_out, n, rx, ry, conv, stop))) return r;
+		OCB_CUDA(x, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
 }
 
 // one launch over a host queue (all POIs share the radius), optional host offsets
