@@ -43,28 +43,7 @@ namespace ocb {
 
 constexpr int ICGN2D_MIN_CTAS = 16; // resident one-warp CTAs the 6-parameter kernels' register budget is sized for (16 -> 128 registers)
 constexpr int ICGN2D_ROW_UNROLL = 3; // rows in flight per lane: whole-pixel loop, 12-parameter sampling loop
-constexpr int ICGN2D_TILE_MARGIN = 1; // slack (pixels) around subset+support in the target tile
-// TMA tile loads need the innermost coordinate 16-byte aligned (x multiple of 4 floats; seen: an
-// unaligned x raises 'illegal instruction'), so tile origins are rounded down to a multiple of 4 and
-// the boxes are 3 columns wider.
-
-__host__ __device__ inline int icgn2d_ref_w(int rx) { return round_up4(2 * rx + 1 + 4 + 3); }
-__host__ __device__ inline int icgn2d_ref_h(int ry) { return 2 * ry + 1 + 4; }
-__host__ __device__ inline int icgn2d_tar_w(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * ICGN2D_TILE_MARGIN + 3); }
-__host__ __device__ inline int icgn2d_tar_h(int ry) { return 2 * ry + 1 + 3 + 2 * ICGN2D_TILE_MARGIN; }
-// per-warp slab (floats): [0,32) mbarrier + pad | tile T (TMA destination, 128-B aligned) | R', gx, gy
-__host__ __device__ inline int icgn2d_tile_floats(int rx, int ry) {
-	const int a = icgn2d_ref_w(rx) * icgn2d_ref_h(ry), b = icgn2d_tar_w(rx) * icgn2d_tar_h(ry);
-	return round_up32(a > b ? a : b);
-}
-// lm: the Levenberg-Marquardt variant keeps the undamped Hessian (<= 78 floats) behind the constants;
-// wpp > 1 (warps per POI): a reduction area follows -- wpp x 96 floats of setup partials, 2 x wpp x 32 floats of
-// per-iteration partials (double-buffered by iteration parity)
-constexpr int ICGN2D_RED_SETUP = 96, ICGN2D_RED_ITER = 32;
-__host__ __device__ inline int icgn2d_slab_floats(int rx, int ry, bool lm, int wpp) {
-	const int n = (2 * rx + 1) * (2 * ry + 1);
-	return 32 + icgn2d_tile_floats(rx, ry) + round_up32(3 * n) + (lm ? 96 : 0) + (wpp > 1 ? wpp * (ICGN2D_RED_SETUP + 2 * ICGN2D_RED_ITER) : 0);
-}
+// tile extents and the slab layout (icgn2d_ref_w .. icgn2d_slab_floats) and the launch plan are in ocb_kernels.h
 
 // Shape functions: sd = g_a * phi_i, phi = [1, x, y, x^2/2, xy, y^2/2] (first 3 for NP == 6);
 // phi_i = c_i x^p_i y^q_i  (reference src/oc_icgn.cpp:191-196, :725-745)
@@ -1173,56 +1152,36 @@ typedef void (*Icgn2dKernel)(Image2D, float*, int, int, int, float, float, int*,
 typedef void (*Icgn2dSeriesKernel)(Image2D, const float*, float*, int, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int);
 
 template <int WPP>
-static Icgn2dKernel icgn2d_pick(int np, int rx, int ry, bool lm) {
+static Icgn2dKernel icgn2d_pick(int np, int rc, bool lm) {
 	if (lm) return (np == 6) ? icgn2d_kernel<6, 0, true, WPP> : icgn2d_kernel<12, 0, true, WPP>;
-	if (np == 6) return (rx == 16 && ry == 16) ? icgn2d_kernel<6, 16, false, WPP> : icgn2d_kernel<6, 0, false, WPP>;
-	return (rx == 20 && ry == 20) ? icgn2d_kernel<12, 20, false, WPP> : icgn2d_kernel<12, 0, false, WPP>;
+	if (np == 6) return rc == 16 ? icgn2d_kernel<6, 16, false, WPP> : icgn2d_kernel<6, 0, false, WPP>;
+	return rc == 20 ? icgn2d_kernel<12, 20, false, WPP> : icgn2d_kernel<12, 0, false, WPP>;
 }
 template <int WPP>
-static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rx, int ry) {
-	if (np == 6) return (rx == 16 && ry == 16) ? icgn2d_series_kernel<6, 16, WPP> : icgn2d_series_kernel<6, 0, WPP>;
-	return (rx == 20 && ry == 20) ? icgn2d_series_kernel<12, 20, WPP> : icgn2d_series_kernel<12, 0, WPP>;
+static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rc) {
+	if (np == 6) return rc == 16 ? icgn2d_series_kernel<6, 16, WPP> : icgn2d_series_kernel<6, 0, WPP>;
+	return rc == 20 ? icgn2d_series_kernel<12, 20, WPP> : icgn2d_series_kernel<12, 0, WPP>;
 }
 
 size_t icgn2d_slab_bytes(int rx, int ry) { return (size_t)icgn2d_slab_floats(rx, ry, false, 1) * sizeof(float); }
 
-// What a launch over n POIs runs with.  A series call takes the pair call's geometry for the same n, so that a frame splits its
-// sums between warps exactly as a pair call does.
+// What a launch over n POIs runs with (icgn2d_plan) and the work-queue head it uses.  A series call takes the pair call's
+// geometry for the same n, so that a frame splits its sums between warps exactly as a pair call does.
 struct Icgn2dGeometry {
-	int wpp, threads, grid;
-	size_t smem;
+	Icgn2dPlan plan;
 	int* counter;
 };
-static int icgn2d_geometry(size_t n, int rx, int ry, bool lm, int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream,
+static int icgn2d_geometry(size_t n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream,
 	Icgn2dGeometry* g, cudaError_t* err) {
-	// Warps per POI (tools/ab_icgn2d.sh compares the two): with the GPU full, one warp per POI wins -- the second warp
-	// doubles the resident warps but also the per-POI fixed work and adds a barrier per pass; with fewer POIs than resident
-	// slots, two warps per POI shorten the tail.  So: 2 only when the queue cannot fill the machine.
-	auto slots = [&](int wpp_) {
-		const size_t b = (size_t)icgn2d_slab_floats(rx, ry, lm, wpp_) * sizeof(float);
-		if (b > smem_optin) return 0;
-		int k = (int)((228 * 1024) / (b + 1024));
-		return k > 32 ? 32 : k;
-	};
-	int wpp = ((long long)n < (long long)sm_count * slots(1) && (2 * ry + 1) >= 8 && slots(2) > 0) ? 2 : 1;
-	if (const char* e = getenv("OCB_ICGN2D_WPP")) { // tuning knob
-		const int v = atoi(e);
-		if (v == 1 || (v == 2 && slots(2) > 0)) wpp = v;
-	}
-	size_t smem = (size_t)icgn2d_slab_floats(rx, ry, lm, wpp) * sizeof(float);
-	if (smem > smem_optin) return -1;
-	int blocks_per_sm = slots(wpp);
-	if (blocks_per_sm < 1) blocks_per_sm = 1;
-	if (wpp != 1) {
+	const char* e = getenv("OCB_ICGN2D_WPP"); // tuning knob: 1 or 2 forces the warps per POI
+	if (!icgn2d_plan(n, np, rx, ry, lm, sm_count, smem_optin, e ? atoi(e) : 0, &g->plan)) return -1;
+	if (g->plan.wpp != 1) {
 		*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
 		if (*err != cudaSuccess) return -2;
 	} else {
 		d_counter += 32; // the one-warp-per-POI kernels reset their queue head themselves: a set of heads nobody else touches
 	}
-	const long long resident = (long long)sm_count * blocks_per_sm;
-	int grid = (int)((long long)n < resident ? (long long)n : resident); // persistent: one wave, one POI per CTA at a time
-	if (grid < 1) grid = 1;
-	*g = Icgn2dGeometry{ wpp, wpp * 32, grid, smem, d_counter };
+	g->counter = d_counter;
 	return 0;
 }
 
@@ -1230,17 +1189,18 @@ int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, i
 	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err) {
 	const bool lm = lm_damping != nullptr;
 	Icgn2dGeometry g;
-	if (const int rc = icgn2d_geometry(n, rx, ry, lm, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
+	if (const int rc = icgn2d_geometry(n, np, rx, ry, lm, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
+	const Icgn2dPlan& p = g.plan;
 	CUtensorMap tm_ref, tm_tar;
 	memset(&tm_ref, 0, sizeof(tm_ref));
 	memset(&tm_tar, 0, sizeof(tm_tar));
 	const int dims[2] = { img.w, img.h };
 	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[2] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry) };
 	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
-	Icgn2dKernel kern = g.wpp == 2 ? icgn2d_pick<2>(np, rx, ry, lm) : icgn2d_pick<1>(np, rx, ry, lm);
-	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem);
+	Icgn2dKernel kern = p.wpp == 2 ? icgn2d_pick<2>(np, p.rc, lm) : icgn2d_pick<1>(np, p.rc, lm);
+	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
 	if (*err != cudaSuccess) return -2;
-	kern<<<g.grid, g.threads, g.smem, stream>>>(img, d_pois, (int)n, rx, ry, conv, stop, g.counter, tm_ref, tm_tar, use_tma, d_center_offsets,
+	kern<<<p.grid, p.wpp * 32, p.smem, stream>>>(img, d_pois, (int)n, rx, ry, conv, stop, g.counter, tm_ref, tm_tar, use_tma, d_center_offsets,
 		lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
 	*err = cudaGetLastError();
 	return *err == cudaSuccess ? 0 : -2;
@@ -1249,17 +1209,18 @@ int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, i
 int icgn2d_series_launch(int np, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
 	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err) {
 	Icgn2dGeometry g;
-	if (const int rc = icgn2d_geometry(n, rx, ry, false, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
+	if (const int rc = icgn2d_geometry(n, np, rx, ry, false, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
+	const Icgn2dPlan& p = g.plan;
 	CUtensorMap tm_ref, tm_tars;
 	memset(&tm_ref, 0, sizeof(tm_ref));
 	memset(&tm_tars, 0, sizeof(tm_tars));
 	const int dims[3] = { img.w, img.h, n_frames };
 	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[3] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry), 1 };
 	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tars, img.tar, 3, dims, box_tar);
-	Icgn2dSeriesKernel kern = g.wpp == 2 ? icgn2d_series_pick<2>(np, rx, ry) : icgn2d_series_pick<1>(np, rx, ry);
-	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem);
+	Icgn2dSeriesKernel kern = p.wpp == 2 ? icgn2d_series_pick<2>(np, p.rc) : icgn2d_series_pick<1>(np, p.rc);
+	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
 	if (*err != cudaSuccess) return -2;
-	kern<<<g.grid, g.threads, g.smem, stream>>>(img, d_seeds, d_out, n_frames, (int)n, rx, ry, conv, stop, g.counter, tm_ref, tm_tars, use_tma);
+	kern<<<p.grid, p.wpp * 32, p.smem, stream>>>(img, d_seeds, d_out, n_frames, (int)n, rx, ry, conv, stop, g.counter, tm_ref, tm_tars, use_tma);
 	*err = cudaGetLastError();
 	return *err == cudaSuccess ? 0 : -2;
 }

@@ -27,15 +27,7 @@
 
 namespace ocb {
 
-constexpr int NR2D_TILE_MARGIN = 1;
-
-__host__ __device__ inline int nr2d_tar_w(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * NR2D_TILE_MARGIN + 4 + 3); }
-__host__ __device__ inline int nr2d_tar_h(int ry) { return 2 * ry + 1 + 3 + 2 * NR2D_TILE_MARGIN + 4; }
-// per-warp slab (floats): [0,32) mbarrier + pad | tile T | gradient tile G (float2) | r~
-__host__ __device__ inline int nr2d_warp_floats(int rx, int ry) {
-	const int tw = nr2d_tar_w(rx), th = nr2d_tar_h(ry);
-	return 32 + round_up32(tw * th) + round_up32(2 * (tw - 4) * (th - 4)) + round_up32((2 * rx + 1) * (2 * ry + 1));
-}
+// tile extents, the per-warp slab (nr2d_tar_w .. nr2d_warp_floats) and the launch plan are in ocb_kernels.h
 
 // gradient pixel of the target at global (x, y), from global memory (slow path only)
 __device__ __forceinline__ float2 nr_grad_global(const float* __restrict__ tar, int w, int h, int x, int y) {
@@ -386,32 +378,22 @@ __global__ void __launch_bounds__(128) nr2d1_kernel(Image2D img, float* __restri
 // Returns 0, -1 when one warp's slab does not fit in shared memory, -2 on a CUDA error.
 int nr2d1_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count, size_t smem_optin,
 	int* d_counter, cudaStream_t stream, cudaError_t* err) {
-	const size_t per_warp = (size_t)nr2d_warp_floats(rx, ry) * sizeof(float);
-	int best_wpb = 0, best_warps = 0;
-	for (int wpb = 4; wpb >= 1; wpb >>= 1) {
-		size_t need = per_warp * wpb;
-		if (need > smem_optin) continue;
-		int blocks = (int)((228 * 1024) / (need + 1024));
-		if (blocks > 32) blocks = 32;
-		int warps = blocks * wpb;
-		if (warps > best_warps) { best_warps = warps; best_wpb = wpb; }
-	}
-	if (best_wpb == 0) return -1;
-	const size_t smem = per_warp * best_wpb;
+	Nr2dPlan p;
+	if (!nr2d1_plan(rx, ry, smem_optin, &p)) return -1;
 	CUtensorMap tm_tar;
 	memset(&tm_tar, 0, sizeof(tm_tar));
 	const int dims[2] = { img.w, img.h };
 	const int box_tar[2] = { nr2d_tar_w(rx), nr2d_tar_h(ry) };
 	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
-	*err = cudaFuncSetAttribute(nr2d1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	*err = cudaFuncSetAttribute(nr2d1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
 	if (*err != cudaSuccess) return -2;
 	*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
 	if (*err != cudaSuccess) return -2;
-	long long blocks_needed = ((long long)n + best_wpb - 1) / best_wpb;
-	long long resident = (long long)sm_count * (best_warps / best_wpb);
+	long long blocks_needed = ((long long)n + p.warps_per_cta - 1) / p.warps_per_cta;
+	long long resident = (long long)sm_count * p.ctas_per_sm;
 	int grid = (int)(blocks_needed < resident ? blocks_needed : resident);
 	if (grid < 1) grid = 1;
-	nr2d1_kernel<<<grid, best_wpb * 32, smem, stream>>>(img, d_pois, (int)n, rx, ry, conv, stop, d_counter, tm_tar, use_tma);
+	nr2d1_kernel<<<grid, p.warps_per_cta * 32, p.smem, stream>>>(img, d_pois, (int)n, rx, ry, conv, stop, d_counter, tm_tar, use_tma);
 	*err = cudaGetLastError();
 	return *err == cudaSuccess ? 0 : -2;
 }

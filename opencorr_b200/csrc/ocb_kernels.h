@@ -6,6 +6,7 @@
 #include <string>
 
 #include "ocb_common.cuh"
+#include "ocb_tma.cuh"
 
 namespace ocb {
 
@@ -47,6 +48,70 @@ const float* sift3d_stage_ms(const Sift3d* s);
 void sift3d_get_matches(const Sift3d* s, float* ref_xyz, float* tar_xyz);
 int sift3d_inspect(const Sift3d* s, int which, size_t* counts, int* cand, float* max_abs, float* kp, float* desc, cudaStream_t stream, std::string* err);
 // icgn2d.cu
+constexpr int ICGN2D_TILE_MARGIN = 1; // slack (pixels) around subset+support in the target tile
+// TMA tile loads need the innermost coordinate 16-byte aligned (x multiple of 4 floats; seen: an
+// unaligned x raises 'illegal instruction'), so tile origins are rounded down to a multiple of 4 and
+// the boxes are 3 columns wider.
+__host__ __device__ inline int icgn2d_ref_w(int rx) { return round_up4(2 * rx + 1 + 4 + 3); }
+__host__ __device__ inline int icgn2d_ref_h(int ry) { return 2 * ry + 1 + 4; }
+__host__ __device__ inline int icgn2d_tar_w(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * ICGN2D_TILE_MARGIN + 3); }
+__host__ __device__ inline int icgn2d_tar_h(int ry) { return 2 * ry + 1 + 3 + 2 * ICGN2D_TILE_MARGIN; }
+// per-warp slab (floats): [0,32) mbarrier + pad | tile T (TMA destination, 128-B aligned) | R', gx, gy
+__host__ __device__ inline int icgn2d_tile_floats(int rx, int ry) {
+	const int a = icgn2d_ref_w(rx) * icgn2d_ref_h(ry), b = icgn2d_tar_w(rx) * icgn2d_tar_h(ry);
+	return round_up32(a > b ? a : b);
+}
+// lm: the Levenberg-Marquardt variant keeps the undamped Hessian (<= 78 floats) behind the constants;
+// wpp > 1 (warps per POI): a reduction area follows -- wpp x 96 floats of setup partials, 2 x wpp x 32 floats of
+// per-iteration partials (double-buffered by iteration parity)
+constexpr int ICGN2D_RED_SETUP = 96, ICGN2D_RED_ITER = 32;
+__host__ __device__ inline int icgn2d_slab_floats(int rx, int ry, bool lm, int wpp) {
+	const int n = (2 * rx + 1) * (2 * ry + 1);
+	return 32 + icgn2d_tile_floats(rx, ry) + round_up32(3 * n) + (lm ? 96 : 0) + (wpp > 1 ? wpp * (ICGN2D_RED_SETUP + 2 * ICGN2D_RED_ITER) : 0);
+}
+
+// Resident one-POI CTAs per SM with wpp warps per POI (0: the slab exceeds the opt-in limit per block)
+inline int icgn2d_slots(int rx, int ry, bool lm, int wpp, size_t smem_optin) {
+	const size_t b = (size_t)icgn2d_slab_floats(rx, ry, lm, wpp) * sizeof(float);
+	if (b > smem_optin) return 0;
+	const int k = (int)((228 * 1024) / (b + 1024));
+	return k > 32 ? 32 : k;
+}
+
+// Launch geometry of icgn2d_kernel<NP, RC, LM, WPP> for a queue of n POIs: one CTA of wpp warps per POI at a time, persistent
+// CTAs (one wave) pulling POIs from a work counter.
+struct Icgn2dPlan {
+	int wpp;           // warps per POI (1 or 2)
+	int rc;            // radius baked into the kernel (16: ICGN2D1, 20: ICGN2D2), 0 for the generic and the LM kernels
+	int blocks_per_sm; // resident CTAs per SM
+	int grid;
+	size_t smem;       // dynamic shared memory per CTA
+};
+
+// false when the slab does not fit in shared memory (smem_optin: the device's opt-in limit per block).  wpp_override: 1 or 2
+// forces the warps per POI (2 only where its slab fits), anything else leaves the choice to the queue length.
+inline bool icgn2d_plan(size_t n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, int wpp_override, Icgn2dPlan* p) {
+	// Warps per POI (tools/ab_icgn2d.sh compares the two): with the GPU full, one warp per POI wins -- the second warp
+	// doubles the resident warps but also the per-POI fixed work and adds a barrier per pass; with fewer POIs than resident
+	// slots, two warps per POI shorten the tail.  So: 2 only when the queue cannot fill the machine.
+	const int s2 = icgn2d_slots(rx, ry, lm, 2, smem_optin);
+	int wpp = ((long long)n < (long long)sm_count * icgn2d_slots(rx, ry, lm, 1, smem_optin) && (2 * ry + 1) >= 8 && s2 > 0) ? 2 : 1;
+	if (wpp_override == 1 || (wpp_override == 2 && s2 > 0)) wpp = wpp_override;
+	const size_t smem = (size_t)icgn2d_slab_floats(rx, ry, lm, wpp) * sizeof(float);
+	if (smem > smem_optin) return false;
+	int blocks_per_sm = icgn2d_slots(rx, ry, lm, wpp, smem_optin);
+	if (blocks_per_sm < 1) blocks_per_sm = 1;
+	const long long resident = (long long)sm_count * blocks_per_sm;
+	int grid = (int)((long long)n < resident ? (long long)n : resident);
+	if (grid < 1) grid = 1;
+	p->wpp = wpp;
+	p->rc = lm ? 0 : (np == 6 ? (rx == 16 && ry == 16 ? 16 : 0) : (rx == 20 && ry == 20 ? 20 : 0));
+	p->blocks_per_sm = blocks_per_sm;
+	p->grid = grid;
+	p->smem = smem;
+	return true;
+}
+
 int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
 	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err);
 size_t icgn2d_slab_bytes(int rx, int ry); // shared memory one POI needs (plain IC-GN, one warp per POI)
@@ -54,6 +119,40 @@ size_t icgn2d_slab_bytes(int rx, int ry); // shared memory one POI needs (plain 
 int icgn2d_series_launch(int np, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
 	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err);
 // nr2d.cu
+constexpr int NR2D_TILE_MARGIN = 1;
+__host__ __device__ inline int nr2d_tar_w(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * NR2D_TILE_MARGIN + 4 + 3); }
+__host__ __device__ inline int nr2d_tar_h(int ry) { return 2 * ry + 1 + 3 + 2 * NR2D_TILE_MARGIN + 4; }
+// per-warp slab (floats): [0,32) mbarrier + pad | tile T | gradient tile G (float2) | r~
+__host__ __device__ inline int nr2d_warp_floats(int rx, int ry) {
+	const int tw = nr2d_tar_w(rx), th = nr2d_tar_h(ry);
+	return 32 + round_up32(tw * th) + round_up32(2 * (tw - 4) * (th - 4)) + round_up32((2 * rx + 1) * (2 * ry + 1));
+}
+
+// Launch geometry of nr2d1_kernel: CTAs of 4, 2 or 1 one-POI warps, whichever keeps the most warps resident per SM.
+struct Nr2dPlan {
+	int warps_per_cta;
+	int ctas_per_sm;
+	size_t smem; // dynamic shared memory per CTA
+};
+
+// false when one warp's slab does not fit in shared memory (smem_optin: the device's opt-in limit per block)
+inline bool nr2d1_plan(int rx, int ry, size_t smem_optin, Nr2dPlan* p) {
+	const size_t per_warp = (size_t)nr2d_warp_floats(rx, ry) * sizeof(float);
+	int best_wpb = 0, best_warps = 0;
+	for (int wpb = 4; wpb >= 1; wpb >>= 1) {
+		const size_t need = per_warp * wpb;
+		if (need > smem_optin) continue;
+		int blocks = (int)((228 * 1024) / (need + 1024));
+		if (blocks > 32) blocks = 32;
+		const int warps = blocks * wpb;
+		if (warps > best_warps) { best_warps = warps; best_wpb = wpb; }
+	}
+	if (best_wpb == 0) return false;
+	p->warps_per_cta = best_wpb;
+	p->ctas_per_sm = best_warps / best_wpb;
+	p->smem = per_warp * best_wpb;
+	return true;
+}
 int nr2d1_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count, size_t smem_optin,
 	int* d_counter, cudaStream_t stream, cudaError_t* err);
 // epipolar.cu

@@ -12,23 +12,6 @@ import util
 pytestmark = pytest.mark.gpu
 
 
-def _nr_compare(a, b, label, tol=1e-4, tol_z=1e-5):
-    """NR2D1 converges linearly, so POIs that stop within float noise of the threshold flip by one iteration more
-    often than IC-GN; the displacement bound applies to POIs with equal iteration counts."""
-    assert np.array_equal(a[:, 14:16], b[:, 14:16]), label
-    za, zb = a[:, 16], b[:, 16]
-    it_same = a[:, 17] == b[:, 17]
-    code_mismatch = ((za < 0) | (zb < 0)) & (za != zb) & ~(((za == -4) | (zb == -4)) & ~it_same)
-    assert not code_mismatch.any(), (label, np.where(code_mismatch)[0][:10], za[code_mismatch][:10], zb[code_mismatch][:10])
-    assert it_same.mean() > 0.98, (label, it_same.mean())
-    ok = it_same & (za >= 0) & (zb >= 0)
-    d = np.abs(a[ok][:, [2, 8]] - b[ok][:, [2, 8]]).max()
-    dz = np.abs(za[ok] - zb[ok]).max()
-    dg = np.abs(a[ok][:, [3, 4, 9, 10]] - b[ok][:, [3, 4, 9, 10]]).max()
-    assert d < tol and dz < tol_z and dg < 2e-5, (label, d, dz, dg)
-    return d, dz
-
-
 @pytest.mark.parametrize("r", [16, 10, 20])
 def test_nr2d1_matches_oracle(engine, r):
     ref, tar = synth.speckle_pair_2d(512, 512)
@@ -42,7 +25,7 @@ def test_nr2d1_matches_oracle(engine, r):
     nr.prepare()
     nr.compute(q_gpu)
     o.nr2d1(q_cpu, r, r, 0.001, 10)
-    _nr_compare(q_gpu, q_cpu, "nr2d1 r=%d" % r)
+    util.nr_compare(q_gpu, q_cpu, "nr2d1 r=%d" % r)
     assert (q_gpu[:, 16] > 0.9).mean() > 0.9
 
 
@@ -64,7 +47,7 @@ def test_nr2d1_nonsquare_and_sentinels(engine):
     Oracle2D(ref, tar).nr2d1(b, 14, 11, 0.001, 10)
     assert a[0, 16] == -1 and a[1, 16] == -1 and a[3, 16] == -2 and a[4, 16] == -5 and a[4, 2] == 1.5
     assert np.array_equal(a[:, 16] < 0, b[:, 16] < 0)
-    _nr_compare(a, b, "nr2d1 sentinels")
+    util.nr_compare(a, b, "nr2d1 sentinels")
     with pytest.raises(ob.OpenCorrB200Error):
         nr2 = ob.NR2D1(16, 16, 0.001, 10, engine=engine)
         nr2.set_images(ref, tar)
@@ -106,7 +89,7 @@ def test_nr2d1_large_image_coordinates(engine):
     nr.prepare()
     nr.compute(a)
     o.nr2d1(b, 16, 16, 0.001, 10, exact=True)
-    _nr_compare(a, b, "nr2d1 large coords", tol=1.5e-4)
+    util.nr_compare(a, b, "nr2d1 large coords", tol=1.5e-4)
 
 
 # ------------------------------------------------------------------------------------------------ Strain

@@ -77,6 +77,23 @@ def _check_iteration_flips(a, b, flip, cols, zc, ic, label, tol_disp, tol_zncc):
     assert dz <= tol_zncc, "%s one-iteration flips: max |dZNCC| = %.3g > %.3g" % (label, dz, tol_zncc)
 
 
+def nr_compare(a, b, label, tol=1e-4, tol_z=1e-5):
+    """NR2D1 parity.  NR2D1 converges linearly, so POIs that stop within float noise of the threshold flip by one iteration
+    more often than IC-GN; the displacement bound applies to POIs with equal iteration counts."""
+    assert np.array_equal(a[:, 14:16], b[:, 14:16]), label
+    za, zb = a[:, 16], b[:, 16]
+    it_same = a[:, 17] == b[:, 17]
+    code_mismatch = ((za < 0) | (zb < 0)) & (za != zb) & ~(((za == -4) | (zb == -4)) & ~it_same)
+    assert not code_mismatch.any(), (label, np.where(code_mismatch)[0][:10], za[code_mismatch][:10], zb[code_mismatch][:10])
+    assert it_same.mean() > 0.98, (label, it_same.mean())
+    ok = it_same & (za >= 0) & (zb >= 0)
+    d = np.abs(a[ok][:, [2, 8]] - b[ok][:, [2, 8]]).max()
+    dz = np.abs(za[ok] - zb[ok]).max()
+    dg = np.abs(a[ok][:, [3, 4, 9, 10]] - b[ok][:, [3, 4, 9, 10]]).max()
+    assert d < tol and dz < tol_z and dg < 2e-5, (label, d, dz, dg)
+    return d, dz
+
+
 def compare_3d(a, b, label="", tol_disp=1e-4, tol_zncc=1e-5, max_iter_mismatch_frac=0.01, flip_tol_disp=1e-3, flip_tol_zncc=1e-4):
     assert a.shape == b.shape
     za, zb = a[:, 18], b[:, 18]
