@@ -270,6 +270,10 @@ __global__ void __launch_bounds__(128) fftcc2d_kernel(Image2D img, float* __rest
 		for (int i = threadIdx.x; i < M; i += blockDim.x) argmax_merge(bv, bi, in[i].x, i);
 		block_argmax(bv, bi, red);
 		if (threadIdx.x == 0) {
+			// A window of constant grey is zero once its mean is taken off.  The reference transforms the two windows separately
+			// (src/oc_fftcc.cpp:233-243), so its surface is then zero everywhere: index 0 wins and ZNCC is 0 / 0.  The packed
+			// transform only cancels Z(k) + conj Z(-k) up to rounding, which would leave noise to pick the displacement.
+			if (na == 0.f || nb == 0.f) { bv = 0.f; bi = 0; }
 			int du = bi % sw, dv = bi / sw;
 			if (du > rx) du -= sw;
 			if (dv > ry) dv -= sh;
@@ -438,16 +442,11 @@ __global__ void __launch_bounds__(256) fftcc3d_kernel(Image3D img, float* __rest
 }
 
 // host side ------------------------------------------------------------------------------------
-size_t fftcc2d_smem_bytes(int rx, int ry) {
-	const size_t M = (size_t)4 * rx * ry;
-	return 2 * M * sizeof(float2) + (size_t)(2 * rx + 2 * ry) * sizeof(float2) + 64 * sizeof(float);
-}
-
-int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const FftAxis& ax, const FftAxis& ay,
-	const float2* tw_x, const float2* tw_y, int sm_count, cudaStream_t stream, cudaError_t* err) {
+int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const Fftcc2dPlan& plan, const float2* tw_x,
+	const float2* tw_y, int sm_count, cudaStream_t stream, cudaError_t* err) {
 	Fft2DParams fp;
-	fp.ax = ax; fp.ay = ay; fp.tw_x = tw_x; fp.tw_y = tw_y;
-	const size_t smem = fftcc2d_smem_bytes(rx, ry);
+	fp.ax = plan.ax; fp.ay = plan.ay; fp.tw_x = tw_x; fp.tw_y = tw_y;
+	const size_t smem = plan.smem;
 	*err = cudaFuncSetAttribute(fftcc2d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (*err != cudaSuccess) return -2;
 	int per_sm = (int)((228 * 1024) / (smem + 1024));

@@ -16,8 +16,6 @@
 
 namespace ocb {
 
-constexpr int FFTREG_THREADS = 128;
-
 template <int N>
 struct FftRegLayout {
 	static constexpr int PP = FFTREG_THREADS / N;         // POIs per CTA
@@ -25,6 +23,7 @@ struct FftRegLayout {
 	static constexpr int TILE = N * PITCH;                // floats per plane
 	static constexpr int RED = 4 * FFTREG_THREADS;        // per-thread partials: 4 floats
 	static constexpr size_t SMEM = ((size_t)2 * PP * TILE + RED) * sizeof(float);
+	static_assert(SMEM == fftcc2d_reg_smem_bytes(N), "the launch plan sizes the shared memory with fftcc2d_reg_smem_bytes");
 };
 
 // resident CTAs the register budget is sized for (2 N floats of transform data per thread + temporaries)
@@ -173,6 +172,9 @@ __global__ void __launch_bounds__(FFTREG_THREADS, fftreg_min_ctas(N)) fftcc2d_re
 				const int oi = ((int*)red)[FFTREG_THREADS + slot * N + j];
 				if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
 			}
+			// a window of constant grey: the reference's surface is zero everywhere, index 0 wins and ZNCC is 0 / 0 (see
+			// fftcc2d_w32.cu; the packed transform leaves rounding noise there instead)
+			if (sna == 0.f || snb == 0.f) { bv = 0.f; bi = 0; }
 			int du = bi % N, dv = bi / N;
 			if (du > R) du -= N;
 			if (dv > R) dv -= N;
@@ -186,47 +188,39 @@ __global__ void __launch_bounds__(FFTREG_THREADS, fftreg_min_ctas(N)) fftcc2d_re
 }
 
 template <int N>
-static int fftcc2d_reg_launch_n(const Image2D& img, float* d_pois, size_t n, int sm_count, cudaStream_t stream, cudaError_t* err) {
-	typedef FftRegLayout<N> L;
-	*err = cudaFuncSetAttribute(fftcc2d_reg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::SMEM);
+static int fftcc2d_reg_launch_n(const Image2D& img, float* d_pois, size_t n, const Fftcc2dPlan& plan, int sm_count, cudaStream_t stream, cudaError_t* err) {
+	*err = cudaFuncSetAttribute(fftcc2d_reg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
 	if (*err != cudaSuccess) return -2;
-	int per_sm = (int)((228 * 1024) / (L::SMEM + 1024));
+	int per_sm = (int)((228 * 1024) / (plan.smem + 1024));
 	if (per_sm > 8) per_sm = 8;
 	if (per_sm < 1) per_sm = 1;
-	const long long n_batch = ((long long)n + L::PP - 1) / L::PP;
+	const long long n_batch = ((long long)n + plan.pois_per_cta - 1) / plan.pois_per_cta;
 	long long grid = (long long)sm_count * per_sm;
 	if (grid > n_batch) grid = n_batch;
 	if (grid < 1) grid = 1;
-	fftcc2d_reg_kernel<N><<<(int)grid, FFTREG_THREADS, L::SMEM, stream>>>(img, d_pois, (int)n);
+	fftcc2d_reg_kernel<N><<<(int)grid, FFTREG_THREADS, plan.smem, stream>>>(img, d_pois, (int)n);
 	*err = cudaGetLastError();
 	return *err == cudaSuccess ? 0 : -2;
 }
 
-// true when a register kernel exists for the square window of 2r points
-bool fftcc2d_reg_supported(int r) {
+int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int sm_count, cudaStream_t stream,
+	cudaError_t* err) {
 	switch (2 * r) {
-	case 8: case 10: case 12: case 16: case 18: case 20: case 24: case 30: case 36: case 40: case 48: case 50: case 54: case 60: case 64: return true;
-	default: return false;
-	}
-}
-
-int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, int sm_count, cudaStream_t stream, cudaError_t* err) {
-	switch (2 * r) {
-	case 8: return fftcc2d_reg_launch_n<8>(img, d_pois, n, sm_count, stream, err);
-	case 10: return fftcc2d_reg_launch_n<10>(img, d_pois, n, sm_count, stream, err);
-	case 12: return fftcc2d_reg_launch_n<12>(img, d_pois, n, sm_count, stream, err);
-	case 16: return fftcc2d_reg_launch_n<16>(img, d_pois, n, sm_count, stream, err);
-	case 18: return fftcc2d_reg_launch_n<18>(img, d_pois, n, sm_count, stream, err);
-	case 20: return fftcc2d_reg_launch_n<20>(img, d_pois, n, sm_count, stream, err);
-	case 24: return fftcc2d_reg_launch_n<24>(img, d_pois, n, sm_count, stream, err);
-	case 30: return fftcc2d_reg_launch_n<30>(img, d_pois, n, sm_count, stream, err);
-	case 36: return fftcc2d_reg_launch_n<36>(img, d_pois, n, sm_count, stream, err);
-	case 40: return fftcc2d_reg_launch_n<40>(img, d_pois, n, sm_count, stream, err);
-	case 48: return fftcc2d_reg_launch_n<48>(img, d_pois, n, sm_count, stream, err);
-	case 50: return fftcc2d_reg_launch_n<50>(img, d_pois, n, sm_count, stream, err);
-	case 54: return fftcc2d_reg_launch_n<54>(img, d_pois, n, sm_count, stream, err);
-	case 60: return fftcc2d_reg_launch_n<60>(img, d_pois, n, sm_count, stream, err);
-	case 64: return fftcc2d_reg_launch_n<64>(img, d_pois, n, sm_count, stream, err);
+	case 8: return fftcc2d_reg_launch_n<8>(img, d_pois, n, plan, sm_count, stream, err);
+	case 10: return fftcc2d_reg_launch_n<10>(img, d_pois, n, plan, sm_count, stream, err);
+	case 12: return fftcc2d_reg_launch_n<12>(img, d_pois, n, plan, sm_count, stream, err);
+	case 16: return fftcc2d_reg_launch_n<16>(img, d_pois, n, plan, sm_count, stream, err);
+	case 18: return fftcc2d_reg_launch_n<18>(img, d_pois, n, plan, sm_count, stream, err);
+	case 20: return fftcc2d_reg_launch_n<20>(img, d_pois, n, plan, sm_count, stream, err);
+	case 24: return fftcc2d_reg_launch_n<24>(img, d_pois, n, plan, sm_count, stream, err);
+	case 30: return fftcc2d_reg_launch_n<30>(img, d_pois, n, plan, sm_count, stream, err);
+	case 36: return fftcc2d_reg_launch_n<36>(img, d_pois, n, plan, sm_count, stream, err);
+	case 40: return fftcc2d_reg_launch_n<40>(img, d_pois, n, plan, sm_count, stream, err);
+	case 48: return fftcc2d_reg_launch_n<48>(img, d_pois, n, plan, sm_count, stream, err);
+	case 50: return fftcc2d_reg_launch_n<50>(img, d_pois, n, plan, sm_count, stream, err);
+	case 54: return fftcc2d_reg_launch_n<54>(img, d_pois, n, plan, sm_count, stream, err);
+	case 60: return fftcc2d_reg_launch_n<60>(img, d_pois, n, plan, sm_count, stream, err);
+	case 64: return fftcc2d_reg_launch_n<64>(img, d_pois, n, plan, sm_count, stream, err);
 	default: *err = cudaErrorInvalidValue; return -2;
 	}
 }

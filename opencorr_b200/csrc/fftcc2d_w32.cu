@@ -27,7 +27,6 @@
 
 namespace ocb {
 
-constexpr int FFTW32_WARPS = 4;
 constexpr int FFTW32_PITCH = 33;
 constexpr int FFTW32_BOX_W = 36;                 // TMA box: 32 columns + up to 3 of alignment slack
 constexpr int FFTW32_TILE = 32 * FFTW32_BOX_W;   // floats per tile: holds a TMA box (36 x 32) or a transpose tile (32 x 33)
@@ -183,6 +182,10 @@ __global__ void __launch_bounds__(FFTW32_WARPS * 32) fftcc2d_w32_kernel(Image2D 
 			const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
 			if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
 		}
+		// A window of constant grey is zero once its mean is taken off.  The reference transforms the two windows separately
+		// (src/oc_fftcc.cpp:233-243), so its surface is then zero everywhere: index 0 wins and ZNCC is 0 / 0.  The packed
+		// transform only cancels Z(k) + conj Z(-k) up to rounding, which would leave noise to pick the displacement.
+		if (na == 0.f || nb == 0.f) { bv = 0.f; bi = 0; }
 		{ // one store instruction for the five result fields (the queue may sit in page-locked host memory)
 			int du = bi & 31, dv = bi >> 5;
 			if (du > R) du -= NW;

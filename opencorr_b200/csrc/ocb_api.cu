@@ -860,13 +860,9 @@ int ocb_set_images_3d(ocb_ctx* ctx, const float* ref, const float* tar, int dim_
 // ---- FFT-CC ----------------------------------------------------------------------------------
 // Which FFT-CC kernel runs: W32 is the register-FFT kernel specialised for the 32-point window (r = 16 on every axis), REG the
 // register FFT codelets for square / cubic windows of N = 2^a 3^b 5^c <= 64 points, GENERIC the shared-memory kernel for any
-// window whose prime factors are <= 31.  OCB_FFTCC2D_GENERIC / OCB_FFTCC3D_GENERIC select GENERIC for every window.
+// window whose prime factors are <= 31.  OCB_FFTCC2D_GENERIC / OCB_FFTCC3D_GENERIC select GENERIC for every window; the 2D
+// choice is ocb::fftcc2d_plan (ocb_kernels.h).
 enum class FftPath { W32, REG, GENERIC };
-static FftPath fftcc2d_path(int rx, int ry) {
-	if (getenv("OCB_FFTCC2D_GENERIC")) return FftPath::GENERIC;
-	if (rx == 16 && ry == 16) return FftPath::W32;
-	return rx == ry && ocb::fftcc2d_reg_supported(rx) ? FftPath::REG : FftPath::GENERIC;
-}
 static FftPath fftcc3d_path(int rx, int ry, int rz) {
 	if (getenv("OCB_FFTCC3D_GENERIC")) return FftPath::GENERIC;
 	if (rx == 16 && ry == 16 && rz == 16) return FftPath::W32;
@@ -883,22 +879,22 @@ int ocb_fftcc2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry) {
 	float* const q = (float*)d_poi2d;
 	cudaError_t err;
 	int failed;
-	const FftPath path = fftcc2d_path(rx, ry);
-	if (path == FftPath::W32) {
-		failed = ocb::fftcc2d_w32_launch(ctx->img2, q, n, ctx->sm_count, ctx->stream, &err);
-	} else if (path == FftPath::REG) { // one thread per row
-		failed = ocb::fftcc2d_reg_launch(ctx->img2, q, n, rx, ctx->sm_count, ctx->stream, &err);
-	} else {
-		ocb::FftAxis ax, ay;
-		if (!ocb::fft_plan_axis(2 * rx, &ax) || !ocb::fft_plan_axis(2 * ry, &ay))
+	ocb::Fftcc2dPlan plan;
+	if (!ocb::fftcc2d_plan(rx, ry, getenv("OCB_FFTCC2D_GENERIC") != nullptr, ctx->smem_optin, &plan)) {
+		if (plan.reject == ocb::Fftcc2dReject::PRIME_FACTOR)
 			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: window size %dx%d has a prime factor > 31", 2 * rx, 2 * ry);
-		if (ocb::fftcc2d_smem_bytes(rx, ry) > ctx->smem_optin)
-			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: %dx%d window needs %zu B of shared memory (> %zu)", 2 * rx, 2 * ry,
-				ocb::fftcc2d_smem_bytes(rx, ry), ctx->smem_optin);
+		return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: %dx%d window needs %zu B of shared memory (> %zu)", 2 * rx, 2 * ry, plan.smem,
+			ctx->smem_optin);
+	}
+	if (plan.path == ocb::Fftcc2dPath::W32) {
+		failed = ocb::fftcc2d_w32_launch(ctx->img2, q, n, ctx->sm_count, ctx->stream, &err);
+	} else if (plan.path == ocb::Fftcc2dPath::REG) { // one thread per row
+		failed = ocb::fftcc2d_reg_launch(ctx->img2, q, n, rx, plan, ctx->sm_count, ctx->stream, &err);
+	} else {
 		const float2 *twx, *twy;
 		int rc;
 		if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy))) return rc;
-		failed = ocb::fftcc2d_launch(ctx->img2, q, n, rx, ry, ax, ay, twx, twy, ctx->sm_count, ctx->stream, &err);
+		failed = ocb::fftcc2d_launch(ctx->img2, q, n, rx, ry, plan, twx, twy, ctx->sm_count, ctx->stream, &err);
 	}
 	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(err));
 	ctx->launches++;
@@ -907,7 +903,9 @@ int ocb_fftcc2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry) {
 
 int ocb_fftcc2d(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry) {
 	if (is_group(ctx) && poi2d) return group_shard(ctx, poi2d, n, OCB_POI2D_FLOATS * sizeof(float), OCB_GROUP_MIN_2D, [=](ocb_ctx* m, void* q, size_t c, size_t) { return ocb_fftcc2d(m, q, c, rx, ry); });
-	const QueuePolicy policy = { true, fftcc2d_path(rx, ry) == FftPath::W32, ry > 0 ? ry : 0 };
+	ocb::Fftcc2dPlan plan; // only the w32 kernel stores a record with one coalesced write
+	const bool w32 = rx >= 1 && ry >= 1 && ocb::fftcc2d_plan(rx, ry, getenv("OCB_FFTCC2D_GENERIC") != nullptr, (size_t)-1, &plan) && plan.path == ocb::Fftcc2dPath::W32;
+	const QueuePolicy policy = { true, w32, ry > 0 ? ry : 0 };
 	return run_host_queue(ctx, "fftcc2d", poi2d, n, OCB_POI2D_FLOATS, [&](float* d, size_t m, size_t) { return ocb_fftcc2d_dev(ctx, d, m, rx, ry); }, policy);
 }
 

@@ -165,15 +165,72 @@ void epipolar_select_launch(float* d_pois, size_t poi0, size_t n_poi, int slots,
 size_t strain_workspace_bytes(size_t n);
 int strain_launch(int dim, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only, void* workspace,
 	int sm_count, cudaStream_t stream, cudaError_t* err, long long* launches);
+// FFTCC2D: which of the three kernels a window takes, and what that kernel needs
+constexpr int FFTW32_WARPS = 4;     // fftcc2d_w32.cu: one-POI warps per CTA
+constexpr int FFTREG_THREADS = 128; // fftcc2d_reg.cu: one thread per window row, 128 / N POIs per CTA
+// fftcc2d_reg.cu, window of n x n points: two padded tiles (pitch n + 1) per POI and four partials per thread
+__host__ __device__ constexpr size_t fftcc2d_reg_smem_bytes(int n) {
+	return ((size_t)2 * (FFTREG_THREADS / n) * n * (n + 1) + 4 * FFTREG_THREADS) * sizeof(float);
+}
+// true when a register kernel exists for the square window of 2r points
+inline bool fftcc2d_reg_supported(int r) {
+	switch (2 * r) {
+	case 8: case 10: case 12: case 16: case 18: case 20: case 24: case 30: case 36: case 40: case 48: case 50: case 54: case 60: case 64: return true;
+	default: return false;
+	}
+}
+// fftcc.cu: two ping-pong windows of complex points, the twiddle tables of both axes, 64 floats of reduction scratch
+inline size_t fftcc2d_smem_bytes(int rx, int ry) {
+	const size_t M = (size_t)4 * rx * ry;
+	return 2 * M * sizeof(float2) + (size_t)(2 * rx + 2 * ry) * sizeof(float2) + 64 * sizeof(float);
+}
+
+// W32 is the register-FFT kernel specialised for the 32-point window (r = 16 on both axes), REG the register FFT codelets for
+// square windows of N = 2^a 3^b 5^c <= 64 points, GENERIC the shared-memory Stockham kernel for any window whose prime factors
+// are <= 31.
+enum class Fftcc2dPath { W32, REG, GENERIC };
+enum class Fftcc2dReject { NONE, PRIME_FACTOR, SHARED_MEMORY };
+struct Fftcc2dPlan {
+	Fftcc2dPath path;
+	FftAxis ax, ay;       // GENERIC: the Stockham stages of the 2rx- and 2ry-point transforms
+	size_t smem;          // dynamic shared memory per CTA (W32: none, its tiles are static)
+	int pois_per_cta;     // POIs a CTA carries at a time
+	Fftcc2dReject reject; // why the plan is refused (GENERIC only)
+};
+
+// false when no kernel takes the (2rx x 2ry) window: a prime factor above 31, or more shared memory than smem_optin (the
+// device's opt-in limit per block).  force_generic sends every window to the GENERIC kernel.  rx, ry >= 1.
+inline bool fftcc2d_plan(int rx, int ry, bool force_generic, size_t smem_optin, Fftcc2dPlan* p) {
+	p->reject = Fftcc2dReject::NONE;
+	p->smem = 0;
+	p->ax.n = p->ay.n = p->ax.nstage = p->ay.nstage = 0;
+	if (!force_generic && rx == 16 && ry == 16) {
+		p->path = Fftcc2dPath::W32;
+		p->pois_per_cta = FFTW32_WARPS;
+		return true;
+	}
+	if (!force_generic && rx == ry && fftcc2d_reg_supported(rx)) {
+		p->path = Fftcc2dPath::REG;
+		p->pois_per_cta = FFTREG_THREADS / (2 * rx);
+		p->smem = fftcc2d_reg_smem_bytes(2 * rx);
+		return true;
+	}
+	p->path = Fftcc2dPath::GENERIC;
+	p->pois_per_cta = 1;
+	p->smem = fftcc2d_smem_bytes(rx, ry);
+	if (!fft_plan_axis(2 * rx, &p->ax) || !fft_plan_axis(2 * ry, &p->ay)) p->reject = Fftcc2dReject::PRIME_FACTOR;
+	else if (p->smem > smem_optin) p->reject = Fftcc2dReject::SHARED_MEMORY;
+	return p->reject == Fftcc2dReject::NONE;
+}
+
 // fftcc.cu
-size_t fftcc2d_smem_bytes(int rx, int ry);
-int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const FftAxis& ax, const FftAxis& ay,
-	const float2* tw_x, const float2* tw_y, int sm_count, cudaStream_t stream, cudaError_t* err);
+int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const Fftcc2dPlan& plan, const float2* tw_x,
+	const float2* tw_y, int sm_count, cudaStream_t stream, cudaError_t* err);
 // fftcc2d_w32.cu (32x32 window, one warp per POI, register FFT)
 int fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int sm_count, cudaStream_t stream, cudaError_t* err);
 // fftcc2d_reg.cu (square windows of 2^a 3^b 5^c <= 64 points, one thread per row, register FFT codelets)
-bool fftcc2d_reg_supported(int r);
-int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, int sm_count, cudaStream_t stream, cudaError_t* err);
+int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int sm_count, cudaStream_t stream,
+	cudaError_t* err);
 // fftcc3d_reg.cu (cubic windows of 2^a 3^b 5^c <= 64 points, one thread per 1D transform, register FFT codelets)
 bool fftcc3d_reg_supported(int r);
 int fftcc3d_reg_grid(int r, int sm_count);

@@ -397,6 +397,11 @@ void fftcc2d_poi(const Ctx2D& c, float* poi, int rx, int ry, const FFT<T>& fx, c
 		}
 	fft_rows(fx, cc.data(), buf, scratch, sh, true);
 	fy.run(cc.data(), scratch, sw, true);
+	// A window of constant grey is zero after the mean is taken off, and the reference, which transforms the two windows
+	// separately (:233-243), then gets a surface that is zero everywhere: index 0 wins and ZNCC is 0 / 0.  The packed transform
+	// above only gives Z(k) + conj Z(-k) = 0 up to rounding.
+	if (ref_norm == 0 || tar_norm == 0)
+		for (int i = 0; i < size; i++) cc[i] = cpx(0, 0);
 	// argmax, :246-255
 	T max_zncc = (T)-2;
 	int idx = 0;
