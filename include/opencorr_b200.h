@@ -170,6 +170,28 @@ int ocb_set_series_2d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars,
 int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop);
 int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop);
 
+/* ---- ICGN3D1 over a volume series: one reference volume, n_frames target volumes (an in-situ CT load series).  Replaces
+ *        for f: dvc.setImages(ref, tar[f]); icgn.prepare() (src/oc_icgn.cpp:1264-1268); icgn.compute(queue) (:1492-1500)
+ *      Frame f's records are, bit for bit, what ocb_icgn3d1 gives on (ref, tars[f]) for frame f - 1's records (frame 0: the
+ *      seeds); a POI that fails in frame f keeps its code in every later frame.  The reference's gradients and each POI's
+ *      setup pass (Hessian, its Cholesky factor, the subvolume statistics) are built once per call; each frame runs the target's
+ *      B-spline prefilter and the IC-GN iterations.
+ * The series is context state of its own: the pair calls (ocb_set_images_3d*, ocb_icgn3d_prepare, ocb_icgn3d1*) neither see
+ *   nor disturb it.  tars: n_frames [z][y][x] volumes, frame-major.  On a group context the first member holds the series and
+ *   runs the calls.  ocb_set_series_3d_u8 keeps the stack as bytes on the device (1 B per voxel and frame).
+ * seeds: n POI3D records; out: n_frames x n POI3D records, frame-major (out[f n + i]), not overlapping seeds.  A long series
+ *   runs in chunks: the last frame's slice of out seeds the next chunk.
+ * Device footprint beyond the stack: about 28 B per voxel (reference, packed gradients, coefficients, scratch) and 420 B per
+ *   POI (cached setup state); the footprint does not grow with n_frames.  The host variant also stages seeds and out.
+ * The host variants copy (ocb_icgn3d_series blocks until out is filled); the _dev variants take BORROWED device pointers and
+ *   only enqueue.  Errors write nothing to out: OCB_ERR_STATE without a series, OCB_ERR_ARG for bad arguments or sizes,
+ *   OCB_ERR_UNSUPPORTED for subvolumes past the shared-memory limit (as ocb_icgn3d1; r >= 44 when cubic). */
+int ocb_set_series_3d(ocb_ctx* ctx, const float* ref, const float* tars, int n_frames, int dim_x, int dim_y, int dim_z);
+int ocb_set_series_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned char* tars, int n_frames, int dim_x, int dim_y, int dim_z);
+int ocb_set_series_3d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars, int n_frames, int dim_x, int dim_y, int dim_z);
+int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop);
+int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop);
+
 /* ---- IC-LM siblings (SURVEY.md section 8(f) N2): ICLM2D1::compute(std::vector<POI2D>&) src/oc_iclm.cpp:360-368
  *      (per POI :150-358) and ICLM2D2 :732-740 (:502-730).  Same prepare() as IC-GN (ocb_icgn2d_prepare).
  *      lambda, alpha, beta = DampingParameter (src/oc_iclm.h:32-37; defaults 100, 0.1, 10; setDamping()). */

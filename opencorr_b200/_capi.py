@@ -62,6 +62,11 @@ SIGNATURES = {
     "ocb_set_series_2d_dev": (_i, [_vp, _vp, _vp, _i, _i, _i]),
     "ocb_icgn2d_series": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_icgn2d_series_dev": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f]),
+    "ocb_set_series_3d": (_i, [_vp, _vp, _vp, _i, _i, _i, _i]),
+    "ocb_set_series_3d_u8": (_i, [_vp, _vp, _vp, _i, _i, _i, _i]),
+    "ocb_set_series_3d_dev": (_i, [_vp, _vp, _vp, _i, _i, _i, _i]),
+    "ocb_icgn3d_series": (_i, [_vp, _vp, _vp, _sz, _i, _i, _i, _f, _f]),
+    "ocb_icgn3d_series_dev": (_i, [_vp, _vp, _vp, _sz, _i, _i, _i, _f, _f]),
     "ocb_iclm2d": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
     "ocb_iclm2d_dev": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
     "ocb_epipolar_search2d": (_i, [_vp, _vp, _sz, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f]),

@@ -226,6 +226,33 @@ class Engine:
             raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn2d_series: no series set")
         return self._n_frames
 
+    def set_series_3d(self, ref, tars):
+        """A volume series for icgn3d_series: ref (Z, Y, X) and tars (F, Z, Y, X).  uint8 volumes stay 8-bit on the device (one
+        byte per voxel and frame); anything else becomes float32.  Kept apart from set_images_3d's pair."""
+        ref, tars = np.asarray(ref), np.asarray(tars)
+        if ref.ndim != 3 or tars.ndim != 4 or tars.shape[1:] != ref.shape:
+            raise ValueError("ref must be (Z, Y, X) and tars (F, Z, Y, X)")
+        f, dz, dy, dx = tars.shape
+        if ref.dtype == np.uint8 and tars.dtype == np.uint8:
+            ref, tars = np.ascontiguousarray(ref), np.ascontiguousarray(tars)
+            self._ck(self._lib.ocb_set_series_3d_u8(self._ctx, _vp(ref), _vp(tars), f, dx, dy, dz))
+        else:
+            ref = np.ascontiguousarray(ref, dtype=np.float32)
+            tars = np.ascontiguousarray(tars, dtype=np.float32)
+            self._ck(self._lib.ocb_set_series_3d(self._ctx, _vp(ref), _vp(tars), f, dx, dy, dz))
+        self._ck(self._lib.ocb_sync(self._ctx))
+        self._n_frames_3d = f
+
+    def icgn3d_series(self, seeds, rx, ry, rz, conv, stop):
+        """ICGN3D1 over the series set by set_series_3d, frame f seeded by frame f - 1's records (frame 0 by `seeds`, [n, 31]).
+        Returns the records of every frame, float32 (F, n, 31); seeds are not changed."""
+        _check_queue(seeds, POI3D_FLOATS)
+        if getattr(self, "_n_frames_3d", None) is None:
+            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn3d_series: no series set")
+        out = np.empty((self._n_frames_3d, seeds.shape[0], POI3D_FLOATS), np.float32)
+        self._ck(self._lib.ocb_icgn3d_series(self._ctx, _vp(seeds), _vp(out), seeds.shape[0], rx, ry, rz, conv, stop))
+        return out
+
     def iclm2d(self, order, q, rx, ry, conv, stop, damping=(100.0, 0.1, 10.0)):
         """ICLM2D1 / ICLM2D2 (reference src/oc_iclm.cpp); damping = (lambda, alpha, beta)."""
         _check_queue(q, POI2D_FLOATS)
@@ -290,6 +317,15 @@ class Engine:
 
     def icgn3d1_dev(self, d_q, n, rx, ry, rz, conv, stop):
         self._ck(self._lib.ocb_icgn3d1_dev(self._ctx, int(d_q), n, rx, ry, rz, conv, stop))
+
+    def set_series_3d_dev(self, d_ref, d_tars, n_frames, dim_x, dim_y, dim_z):
+        """Device pointers: the float32 reference volume and the frame-major stack of n_frames targets; borrowed, not copied."""
+        self._ck(self._lib.ocb_set_series_3d_dev(self._ctx, int(d_ref), int(d_tars), n_frames, dim_x, dim_y, dim_z))
+        self._n_frames_3d = int(n_frames)
+
+    def icgn3d_series_dev(self, d_seeds, d_out, n, rx, ry, rz, conv, stop):
+        """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
+        self._ck(self._lib.ocb_icgn3d_series_dev(self._ctx, int(d_seeds), int(d_out), n, rx, ry, rz, conv, stop))
 
     # SIFT3D --------------------------------------------------------------------------------------
     def sift3d(self, config=None, unit=(1.0, 1.0, 1.0), matching_ratio=0.85):

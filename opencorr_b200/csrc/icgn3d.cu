@@ -214,11 +214,30 @@ __device__ __forceinline__ void bspline_basis_fast2(float2 t, float2* b) {
 	b[2] = fsub2(fsub2(fsub2(bcast2(1.f), b[0]), b[1]), b[3]);
 }
 
+// Float k of a POI's cached setup state (ICGN3D_SETUP_FLOATS: L, S, SF, rbar, f2, c0)
+__device__ __forceinline__ float* icgn3d_setup_slot(Icgn3dShared& sh, int k) {
+	if (k < NH3) return sh.L + k;
+	if (k < NH3 + NP3) return sh.S + (k - NH3);
+	if (k < NH3 + 2 * NP3) return sh.SF + (k - NH3 - NP3);
+	return k == NH3 + 2 * NP3 ? &sh.rbar : (k == NH3 + 2 * NP3 + 1 ? &sh.f2 : &sh.c0);
+}
+
 // RC > 0: radius known at compile time (rx == ry == rz == RC): tile pitches become immediates.
 // THREADS: 256 (two CTAs per SM) or 512 (large radii: the slab leaves room for one CTA only, which then brings 16 warps)
-template <int RC, int THREADS>
+// SETUP: an Icgn3dSetup.  COMPUTE is the whole algorithm.  STORE runs only the guard and the setup pass, writes each accepted
+// POI's setup state to setup_cache and leaves the records alone (no iterations: its registers stay below the pair kernels').
+// LOAD restores that state instead of running the setup pass, then iterates as COMPUTE does.  A volume series runs STORE once on
+// the seeds, then LOAD once per frame on the same queue positions, frame 0 on a copy of the seeds.
+// LOAD is safe because a POI without a cache entry never gets past the guard.  Only a POI the guard rejects on the seeds has
+// none; frame 0's guard sees the same record and rejects it too, and the guard leaves a record unchanged except for the ZNCC,
+// which becomes -3, stays negative or (a NaN seed ZNCC, rejected for its coordinates or guess) stays NaN with those
+// coordinates and that guess kept, so every later frame's guard rejects it again.  The kernel never writes a POI's
+// coordinates, so the cached state (it depends only on the reference, the coordinates and the radii) is the state the POI
+// would build in any frame.
+template <int RC, int THREADS, int SETUP = ICGN3D_SETUP_COMPUTE>
 __global__ void __launch_bounds__(THREADS, 512 / THREADS) icgn3d1_kernel(Image3D img, float* __restrict__ pois, int n_poi, int rx_arg, int ry_arg, int rz_arg,
-	float conv_criterion, float stop_condition, int slab_k, int* __restrict__ work_counter, const __grid_constant__ CUtensorMap tm_coef, int use_tma) {
+	float conv_criterion, float stop_condition, int slab_k, int* __restrict__ work_counter, const __grid_constant__ CUtensorMap tm_coef, int use_tma,
+	float* __restrict__ setup_cache) {
 	constexpr int ICGN3D_THREADS = THREADS, ICGN3D_WARPS = THREADS / 32;
 	extern __shared__ __align__(128) float dsmem[];
 	__shared__ Icgn3dShared sh;
@@ -253,7 +272,7 @@ __global__ void __launch_bounds__(THREADS, 512 / THREADS) icgn3d1_kernel(Image3D
 		if ((px - rx) < 0 || (py - ry) < 0 || (pz - rz) < 0 || (px + rx) > (dx - 1) || (py + ry) > (dy - 1) || (pz + rz) > (dz - 1)
 			|| fabsf(u_in) >= dx || fabsf(v_in) >= dy || fabsf(w_in) >= dz || zncc_in < 0
 			|| is_nan_f(u_in) || is_nan_f(v_in) || is_nan_f(w_in) || is_nan_f(px) || is_nan_f(py) || is_nan_f(pz)) {
-			if (tid == 0) P[P3_ZNCC] = zncc_in >= 0 ? -3.f : zncc_in;
+			if (tid == 0 && SETUP != ICGN3D_SETUP_STORE) P[P3_ZNCC] = zncc_in >= 0 ? -3.f : zncc_in;
 			continue;
 		}
 		const int x0 = (int)px - rx, y0 = (int)py - ry, z0 = (int)pz - rz;
@@ -261,7 +280,7 @@ __global__ void __launch_bounds__(THREADS, 512 / THREADS) icgn3d1_kernel(Image3D
 		const float c0 = __ldg(img.ref + ((size_t)(int)pz * dy + (int)py) * dx + (int)px); // pilot value: centre voxel
 
 		// ---- reference subset statistics + steepest-descent images + Hessian (src/oc_icgn.cpp:1291-1337)
-		{
+		if constexpr (SETUP != ICGN3D_SETUP_LOAD) {
 			float acc[NSETUP];
 #pragma unroll
 			for (int k = 0; k < NSETUP; k++) acc[k] = 0.f;
@@ -394,15 +413,22 @@ __global__ void __launch_bounds__(THREADS, 512 / THREADS) icgn3d1_kernel(Image3D
 				float v = warp_sum(acc[k]);
 				if (lane == 0) sh.part[warp][k] = v;
 			}
+			__syncthreads();
+			if (tid < NSETUP) {
+				float t = 0.f;
+				for (int i = 0; i < ICGN3D_WARPS; i++) t += sh.part[i][tid];
+				sh.tot[tid] = t;
+			}
+			__syncthreads();
 		}
-		__syncthreads();
-		if (tid < NSETUP) {
-			float t = 0.f;
-			for (int i = 0; i < ICGN3D_WARPS; i++) t += sh.part[i][tid];
-			sh.tot[tid] = t;
-		}
-		__syncthreads();
-		if (tid == 0) {
+		if constexpr (SETUP == ICGN3D_SETUP_LOAD) {
+			if (tid < ICGN3D_SETUP_FLOATS) *icgn3d_setup_slot(sh, tid) = __ldg(setup_cache + (size_t)poi * ICGN3D_SETUP_FLOATS + tid);
+			if (tid == 0) { // initial warp, as below (spelled out twice: a shared lambda changes the pair kernels' register allocation)
+				sh.A[0] = 1.f + P[P3_DEF + 1]; sh.A[1] = P[P3_DEF + 2]; sh.A[2] = P[P3_DEF + 3]; sh.A[3] = u_in;
+				sh.A[4] = P[P3_DEF + 5]; sh.A[5] = 1.f + P[P3_DEF + 6]; sh.A[6] = P[P3_DEF + 7]; sh.A[7] = v_in;
+				sh.A[8] = P[P3_DEF + 9]; sh.A[9] = P[P3_DEF + 10]; sh.A[10] = 1.f + P[P3_DEF + 11]; sh.A[11] = w_in;
+			}
+		} else if (tid == 0) {
 			float Hh[NH3];
 #pragma unroll
 			for (int k = 0; k < NH3; k++) Hh[k] = sh.tot[k];
@@ -424,6 +450,10 @@ __global__ void __launch_bounds__(THREADS, 512 / THREADS) icgn3d1_kernel(Image3D
 			sh.A[8] = P[P3_DEF + 9]; sh.A[9] = P[P3_DEF + 10]; sh.A[10] = 1.f + P[P3_DEF + 11]; sh.A[11] = w_in;
 		}
 		__syncthreads();
+		if constexpr (SETUP == ICGN3D_SETUP_STORE) { // nothing writes these fields before the next POI's setup pass
+			if (tid < ICGN3D_SETUP_FLOATS) setup_cache[(size_t)poi * ICGN3D_SETUP_FLOATS + tid] = *icgn3d_setup_slot(sh, tid);
+			continue;
+		}
 
 		// ---- IC-GN iterations (src/oc_icgn.cpp:1355-1447)
 		const float xmax = (float)(dx - 2), ymax = (float)(dy - 2), zmax = (float)(dz - 2);
@@ -715,9 +745,18 @@ __global__ void __launch_bounds__(THREADS, 512 / THREADS) icgn3d1_kernel(Image3D
 	}
 }
 
+typedef void (*Icgn3dKernel)(Image3D, float*, int, int, int, int, float, float, int, int*, const CUtensorMap, int, float*);
+
+template <int RC, int THREADS>
+static Icgn3dKernel icgn3d1_kernel_for(int setup) {
+	if (setup == ICGN3D_SETUP_STORE) return icgn3d1_kernel<RC, THREADS, ICGN3D_SETUP_STORE>;
+	if (setup == ICGN3D_SETUP_LOAD) return icgn3d1_kernel<RC, THREADS, ICGN3D_SETUP_LOAD>;
+	return icgn3d1_kernel<RC, THREADS>;
+}
+
 // Returns 0, -1 when even a one-layer slab does not fit in shared memory, -2 on a CUDA error.
 int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop, int sm_count, size_t smem_optin,
-	int* d_counter, cudaStream_t stream, cudaError_t* err) {
+	int* d_counter, cudaStream_t stream, cudaError_t* err, int setup, float* setup_cache) {
 	Icgn3dPlan plan;
 	if (!icgn3d1_plan(rx, ry, rz, smem_optin, &plan)) return -1;
 	const int slab_k = plan.slab_k;
@@ -727,10 +766,10 @@ int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, 
 	const int dims[3] = { img.dx, img.dy, img.dz };
 	const int box[3] = { icgn3d_tile_x(rx), icgn3d_tile_y(ry), icgn3d_tile_z(slab_k) };
 	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm, img.coef, 3, dims, box);
-	void (*kern)(Image3D, float*, int, int, int, int, float, float, int, int*, const CUtensorMap, int);
+	Icgn3dKernel kern;
 	const int threads = plan.threads;
-	if (plan.threads == 512) kern = plan.rc == 30 ? icgn3d1_kernel<30, 512> : icgn3d1_kernel<0, 512>;
-	else kern = plan.rc == 16 ? icgn3d1_kernel<16, 256> : icgn3d1_kernel<0, 256>;
+	if (plan.threads == 512) kern = plan.rc == 30 ? icgn3d1_kernel_for<30, 512>(setup) : icgn3d1_kernel_for<0, 512>(setup);
+	else kern = plan.rc == 16 ? icgn3d1_kernel_for<16, 256>(setup) : icgn3d1_kernel_for<0, 256>(setup);
 	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (*err != cudaSuccess) return -2;
 	*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
@@ -738,7 +777,7 @@ int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, 
 	long long grid = (long long)sm_count * plan.ctas_per_sm;
 	if (grid > (long long)n) grid = (long long)n;
 	if (grid < 1) grid = 1;
-	kern<<<(int)grid, threads, smem, stream>>>(img, d_pois, (int)n, rx, ry, rz, conv, stop, slab_k, d_counter, tm, use_tma);
+	kern<<<(int)grid, threads, smem, stream>>>(img, d_pois, (int)n, rx, ry, rz, conv, stop, slab_k, d_counter, tm, use_tma, setup_cache);
 	*err = cudaGetLastError();
 	return *err == cudaSuccess ? 0 : -2;
 }

@@ -153,6 +153,15 @@ struct ocb_ctx {
 	ocb::Image3D img3{ nullptr, nullptr, nullptr, nullptr, 0, 0, 0 };
 	bool prepared3 = false;
 
+	// 3D volume series (ocb_set_series_3d*): its own state and buffers, untouched by the pair calls.  series3.ref is the
+	// reference, series3_tars the frame-major stack (floats, or bytes with frames series3_u8_pitch bytes apart).
+	DevBuf own_series3[2]; // {ref, stack} uploaded from the host
+	DevBuf series3_rg, series3_coef, series3_tmp, series3_cache;
+	ocb::Image3D series3{ nullptr, nullptr, nullptr, nullptr, 0, 0, 0 };
+	const void* series3_tars = nullptr;
+	size_t series3_u8_pitch = 0; // 0: a float stack
+	int series3_frames = 0;
+
 	// FFT
 	std::map<int, float2*> twiddles;
 	DevBuf fft_scratch; // float2
@@ -1337,6 +1346,163 @@ int ocb_icgn3d1(ocb_ctx* ctx, void* poi3d, size_t n, int rx, int ry, int rz, flo
 	if (is_group(ctx) && poi3d) return group_shard(ctx, poi3d, n, OCB_POI3D_FLOATS * sizeof(float), OCB_GROUP_MIN_3D, [=](ocb_ctx* m, void* q, size_t c, size_t) { return ocb_icgn3d1(m, q, c, rx, ry, rz, conv, stop); });
 	return run_host_queue(ctx, "icgn3d1", poi3d, n, OCB_POI3D_FLOATS, [&](float* d, size_t m, size_t) { return ocb_icgn3d1_dev(ctx, d, m, rx, ry, rz, conv, stop); },
 		STAGED);
+}
+
+// ---- volume series: one reference volume, n_frames target volumes, each frame seeded by the previous one ------------------
+// Voxels per volume, or 0 when a dimension is < 15 (TricubicBspline, src/oc_cubic_bspline.cpp:201) or n_frames volumes of
+// `voxel` bytes each would not fit in a size_t.
+static size_t series3_elems(int n_frames, int dim_x, int dim_y, int dim_z, size_t voxel) {
+	if (n_frames < 1 || dim_x < 15 || dim_y < 15 || dim_z < 15) return 0;
+	const size_t xy = (size_t)dim_x * dim_y;
+	if (xy > SIZE_MAX / (size_t)dim_z) return 0;
+	const size_t elems = xy * (size_t)dim_z;
+	return elems > SIZE_MAX / voxel / (size_t)n_frames ? 0 : elems;
+}
+
+static void series3_set(ocb_ctx* x, const float* ref, const void* tars, size_t u8_pitch, int n_frames, int dim_x, int dim_y, int dim_z) {
+	x->series3 = ocb::Image3D{ ref, nullptr, nullptr, nullptr, dim_x, dim_y, dim_z };
+	x->series3_tars = tars;
+	x->series3_u8_pitch = u8_pitch;
+	x->series3_frames = n_frames;
+}
+
+int ocb_set_series_3d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars, int n_frames, int dim_x, int dim_y, int dim_z) {
+	OCB_NO_GROUP(ctx, "set_series_3d_dev");
+	if (!ctx || !d_ref || !d_tars || !series3_elems(n_frames, dim_x, dim_y, dim_z, sizeof(float)))
+		return set_error(ctx, OCB_ERR_ARG, "set_series_3d: bad arguments (each dimension must be >= 15, n_frames >= 1)");
+	series3_set(ctx, d_ref, d_tars, 0, n_frames, dim_x, dim_y, dim_z);
+	return OCB_OK;
+}
+
+int ocb_set_series_3d(ocb_ctx* ctx, const float* ref, const float* tars, int n_frames, int dim_x, int dim_y, int dim_z) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* x = series_exec(ctx);
+	const int rc = [&]() -> int {
+		const size_t elems = series3_elems(n_frames, dim_x, dim_y, dim_z, sizeof(float));
+		if (!ref || !tars || !elems) return set_error(x, OCB_ERR_ARG, "set_series_3d: bad arguments (each dimension must be >= 15, n_frames >= 1)");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t bytes = elems * sizeof(float);
+		int r;
+		if ((r = grow(x, x->own_series3[0], bytes)) || (r = grow(x, x->own_series3[1], (size_t)n_frames * bytes))) return r;
+		OCB_CUDA(x, cudaMemcpyAsync(x->own_series3[0].p, ref, bytes, cudaMemcpyHostToDevice, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(x->own_series3[1].p, tars, (size_t)n_frames * bytes, cudaMemcpyHostToDevice, x->stream));
+		series3_set(x, x->own_series3[0].as<float>(), x->own_series3[1].p, 0, n_frames, dim_x, dim_y, dim_z);
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+int ocb_set_series_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned char* tars, int n_frames, int dim_x, int dim_y, int dim_z) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* x = series_exec(ctx);
+	const int rc = [&]() -> int {
+		// frames start on 16-byte boundaries: the widening kernel reads uchar4
+		const size_t elems = series3_elems(n_frames, dim_x, dim_y, dim_z, 16);
+		if (!ref || !tars || !elems)
+			return set_error(x, OCB_ERR_ARG, "set_series_3d_u8: bad arguments (each dimension must be >= 15, n_frames >= 1)");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t pitch = (elems + 15) & ~(size_t)15;
+		int r;
+		// the reference crosses PCIe as bytes too, staged in the series' scratch volume and widened into the reference buffer
+		if ((r = grow(x, x->own_series3[0], elems * sizeof(float))) || (r = grow(x, x->series3_tmp, elems * sizeof(float)))
+			|| (r = grow(x, x->own_series3[1], (size_t)n_frames * pitch)))
+			return r;
+		unsigned char* const stack = x->own_series3[1].as<unsigned char>();
+		OCB_CUDA(x, cudaMemcpyAsync(x->series3_tmp.p, ref, elems, cudaMemcpyHostToDevice, x->stream));
+		ocb::widen_u8_kernel<<<x->sm_count * 8, 256, 0, x->stream>>>(x->series3_tmp.as<unsigned char>(), x->own_series3[0].as<float>(), elems);
+		x->launches++;
+		OCB_CUDA(x, cudaGetLastError());
+		for (int f = 0; f < n_frames; f++)
+			OCB_CUDA(x, cudaMemcpyAsync(stack + (size_t)f * pitch, tars + (size_t)f * elems, elems, cudaMemcpyHostToDevice, x->stream));
+		series3_set(x, x->own_series3[0].as<float>(), stack, pitch, n_frames, dim_x, dim_y, dim_z);
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop) {
+	OCB_NO_GROUP(ctx, "icgn3d_series_dev");
+	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1 || rz < 1) return set_error(ctx, OCB_ERR_ARG, "icgn3d_series: bad arguments");
+	if (!ctx->series3.ref) return set_error(ctx, OCB_ERR_STATE, "icgn3d_series: no series set");
+	if (n == 0) return OCB_OK;
+	const size_t rec = OCB_POI3D_FLOATS * sizeof(float);
+	if (n > 0x7fffffffull || (size_t)ctx->series3_frames > SIZE_MAX / (n * rec))
+		return set_error(ctx, OCB_ERR_ARG, "icgn3d_series: too many POIs in one call");
+	if ((size_t)(2 * rx + 1) * (2 * ry + 1) * (2 * rz + 1) > 0x3fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn3d1: subset too large");
+	ocb::Icgn3dPlan plan;
+	if (!ocb::icgn3d1_plan(rx, ry, rz, ctx->smem_optin, &plan))
+		return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn3d1: subset radius (%d,%d,%d) exceeds the shared-memory design limit", rx, ry, rz);
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	const int dx = ctx->series3.dx, dy = ctx->series3.dy, dz = ctx->series3.dz;
+	const size_t elems = (size_t)dx * dy * dz;
+	int rc;
+	if ((rc = grow(ctx, ctx->series3_rg, elems * sizeof(float4))) || (rc = grow(ctx, ctx->series3_coef, elems * sizeof(float)))
+		|| (rc = grow(ctx, ctx->series3_tmp, elems * sizeof(float))) || (rc = grow(ctx, ctx->series3_cache, n * ocb::ICGN3D_SETUP_FLOATS * sizeof(float))))
+		return rc;
+	float4* const rg = ctx->series3_rg.as<float4>();
+	float* const coef = ctx->series3_coef.as<float>();
+	float* const tmp = ctx->series3_tmp.as<float>();
+	float* const cache = ctx->series3_cache.as<float>();
+	const ocb::Image3D img{ ctx->series3.ref, nullptr, rg, coef, dx, dy, dz };
+	cudaError_t err = cudaSuccess;
+	auto icgn = [&](float* q, int setup) {
+		const int r3 = ocb::icgn3d1_launch(img, q, n, rx, ry, rz, conv, stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter + 1, ctx->stream, &err, setup,
+			cache);
+		if (r3) return set_error(ctx, OCB_ERR_CUDA, "icgn3d_series launch failed: %s", cudaGetErrorString(err));
+		ctx->launches++;
+		return (int)OCB_OK;
+	};
+	// the reference's products, once per call: packed gradients, then each POI's setup pass (records are not written)
+	ocb::gradient3d_launch(ctx->series3.ref, rg, dx, dy, dz, ctx->sm_count, ctx->stream);
+	ctx->launches++;
+	if ((rc = icgn(const_cast<float*>((const float*)d_seeds), ocb::ICGN3D_SETUP_STORE))) return rc;
+	for (int f = 0; f < ctx->series3_frames; f++) {
+		// TricubicBspline::prepare of frame f as in ocb_icgn3d_prepare: x -> coefficient, y -> scratch, z -> coefficient
+		const float* tar;
+		if (ctx->series3_u8_pitch) {
+			ocb::widen_u8_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const unsigned char*)ctx->series3_tars + (size_t)f * ctx->series3_u8_pitch,
+				tmp, elems);
+			ctx->launches++;
+			tar = tmp;
+		} else {
+			tar = (const float*)ctx->series3_tars + (size_t)f * elems;
+		}
+		ocb::prefilter3d_launch(tar, coef, dx, dy, dz, 0, ctx->sm_count, ctx->stream);
+		ocb::prefilter3d_launch(coef, tmp, dx, dy, dz, 1, ctx->sm_count, ctx->stream);
+		ocb::prefilter3d_launch(tmp, coef, dx, dy, dz, 2, ctx->sm_count, ctx->stream);
+		ctx->launches += 3;
+		OCB_CUDA(ctx, cudaGetLastError());
+		float* const q = (float*)d_out + (size_t)f * n * OCB_POI3D_FLOATS;
+		const void* prev = f == 0 ? d_seeds : (const void*)(q - n * OCB_POI3D_FLOATS);
+		OCB_CUDA(ctx, cudaMemcpyAsync(q, prev, n * rec, cudaMemcpyDeviceToDevice, ctx->stream));
+		if ((rc = icgn(q, ocb::ICGN3D_SETUP_LOAD))) return rc;
+	}
+	return OCB_OK;
+}
+
+int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* x = series_exec(ctx);
+	const int rc = [&]() -> int {
+		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "icgn3d_series: bad arguments");
+		if (!x->series3.ref) return set_error(x, OCB_ERR_STATE, "icgn3d_series: no series set");
+		if (n == 0) return ocb_icgn3d_series_dev(x, nullptr, nullptr, 0, rx, ry, rz, conv, stop); // argument checks only
+		const size_t rec = OCB_POI3D_FLOATS * sizeof(float);
+		if (n > 0x7fffffffull || (size_t)x->series3_frames + 1 > SIZE_MAX / (n * rec))
+			return set_error(x, OCB_ERR_ARG, "icgn3d_series: too many POIs in one call");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t out_bytes = (size_t)x->series3_frames * n * rec;
+		int r;
+		if ((r = grow(x, x->d_poi, n * rec + out_bytes))) return r;
+		float* const d_seeds = x->d_poi.as<float>();
+		float* const d_out = d_seeds + n * OCB_POI3D_FLOATS;
+		OCB_CUDA(x, cudaMemcpyAsync(d_seeds, seeds, n * rec, cudaMemcpyHostToDevice, x->stream));
+		if ((r = ocb_icgn3d_series_dev(x, d_seeds, d_out, n, rx, ry, rz, conv, stop))) return r;
+		OCB_CUDA(x, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
 }
 
 int ocb_get_tables_3d(ocb_ctx* ctx, float* gx, float* gy, float* gz, float* coefficient) {

@@ -263,6 +263,12 @@ struct Icgn3dShared {
 	int poi;
 };
 
+// What icgn3d1_kernel does with a POI's setup pass (the reference-only state: Cholesky factor L, S, SF, rbar, f2, c0).
+// COMPUTE: build it, then iterate (pair calls).  STORE: build it and write it to a per-POI device cache, records untouched.
+// LOAD: restore it from the cache bit for bit, then iterate (volume series, every frame).
+enum Icgn3dSetup { ICGN3D_SETUP_COMPUTE = 0, ICGN3D_SETUP_STORE = 1, ICGN3D_SETUP_LOAD = 2 };
+constexpr int ICGN3D_SETUP_FLOATS = NH3 + 2 * NP3 + 3; // cached floats per POI: L, S, SF, rbar, f2, c0 (105, 420 B)
+
 // extents of the staged B-spline coefficient tile: x padded to a multiple of 4 floats (16-byte TMA rows)
 __host__ __device__ inline int icgn3d_tile_x(int rx) { return (2 * rx + 1 + 3 + 2 * ICGN3D_TILE_MARGIN + 3 + 3) & ~3; }
 __host__ __device__ inline int icgn3d_tile_y(int ry) { return 2 * ry + 1 + 3 + 2 * ICGN3D_TILE_MARGIN; }
@@ -323,7 +329,8 @@ void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* 
 
 void gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s);
 void prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s);
+// setup: an Icgn3dSetup; STORE and LOAD need setup_cache, n x ICGN3D_SETUP_FLOATS floats indexed by queue position
 int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop, int sm_count, size_t smem_optin,
-	int* d_counter, cudaStream_t stream, cudaError_t* err);
+	int* d_counter, cudaStream_t stream, cudaError_t* err, int setup = ICGN3D_SETUP_COMPUTE, float* setup_cache = nullptr);
 
 } // namespace ocb

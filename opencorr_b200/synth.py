@@ -114,6 +114,24 @@ def speckle_pair_3d(dim_x, dim_y, dim_z, rho=2.0, seed=REF_SEED, quantise=True, 
     return out[0], out[1]
 
 
+def speckle_series_3d(dim_x, dim_y, dim_z, n_frames, rho=2.0, seed=REF_SEED, device=None, background=BACKGROUND):
+    """(ref [dim_z, dim_y, dim_x], tars [n_frames, dim_z, dim_y, dim_x]) float32, 8-bit valued: the speckles of speckle_pair_3d
+    moved by (f + 1) / n_frames of displacement_3d in frame f, so the last frame carries the whole field."""
+    rng = np.random.default_rng(seed)
+    n = int(0.35 * dim_x * dim_y * dim_z / (4.0 / 3.0 * np.pi * rho ** 3))
+    cx = rng.uniform(-8, dim_x + 8, n)
+    cy = rng.uniform(-8, dim_y + 8, n)
+    cz = rng.uniform(-8, dim_z + 8, n)
+    amp = rng.uniform(0.4, 1.0, n)
+    u, v, w = displacement_3d(cx, cy, cz, dim_x, dim_y, dim_z)
+
+    def volume(s):
+        im = _render((dim_z, dim_y, dim_x), np.stack([cz + s * w, cy + s * v, cx + s * u], 1), amp, rho, device)
+        return np.round(np.clip(background + (255.0 - background) * im, 0, 255)).astype(np.float32)
+
+    return volume(0.0), np.stack([volume((f + 1) / n_frames) for f in range(n_frames)])
+
+
 def grid_2d(x0, y0, nx, ny, sx, sy):
     """POI grid, row-major over y then x like the reference examples (test_2d_dic_fftcc_icgn1.cpp:57-66)."""
     ys, xs = np.meshgrid(y0 + sy * np.arange(ny), x0 + sx * np.arange(nx), indexing="ij")

@@ -1,14 +1,16 @@
-"""Image-series IC-GN benchmark: one reference against F targets, two arms on the same synthetic series, alternated over
-rounds in one process and timed with CUDA events.
+"""Image- and volume-series IC-GN benchmark: one reference against F targets, two arms on the same synthetic series, alternated
+over rounds in one process and timed with CUDA events.
 
-  (a) the device-resident loop of pair calls: per frame set_images_2d_dev + icgn2d_prepare + icgn2d1/2_dev on one carried
-      queue, and a device copy of the frame's records;
-  (b) one icgn2d_series_dev call.
+  (a) the device-resident loop of pair calls: per frame set_images_2d_dev / set_images_3d_dev + icgn2d_prepare /
+      icgn3d_prepare + icgn2d1/2_dev / icgn3d1_dev on one carried queue, and a device copy of the frame's records;
+  (b) one icgn2d_series_dev / icgn3d_series_dev call.
 
-Geometries: bench.py's config B (2048^2, 50 k POIs, r = 16, ICGN2D1) and C (r = 20, ICGN2D2), F = 8 frames whose
-displacement is (f + 1) / F of synth's field.  Both arms' records are compared as uint32 in the same run.
+Geometries: bench.py's config B (2048^2, 50 k POIs, r = 16, ICGN2D1) and C (r = 20, ICGN2D2), and for volumes config D
+(256^3, 20 k POIs, r = 16) and F (288^3, 1728 POIs, r = 30); F = 8 frames whose displacement is (f + 1) / F of synth's field.
+Both arms' records are compared as uint32 in the same run.
 
     python tools/bench_series.py --out profiles/h100_bench_series.json
+    python tools/bench_series.py --configs D,F --out profiles/h100_bench_series_3d.json
 """
 import argparse
 import json
@@ -51,6 +53,8 @@ def render_series(width, height, n_frames, second_order, rho=2.0, seed=synth.REF
 
 
 def run(config, n_frames, rounds, reps, eng):
+    if synth.CONFIGS[config]["kind"] == "3d":
+        return run_3d(config, n_frames, rounds, reps, eng)
     import torch
     cfg = synth.CONFIGS[config]
     w, h = cfg["size"]
@@ -106,6 +110,63 @@ def run(config, n_frames, rounds, reps, eng):
                 loop_ms=[round(x, 4) for x in ms_a], series_ms=[round(x, 4) for x in ms_b],
                 loop_over_series=[round(a / b, 4) for a, b in zip(ms_a, ms_b)],
                 records_identical=bool(identical), last_frame_valid_frac=float((last[:, 16] >= 0).mean()))
+
+
+def run_3d(config, n_frames, rounds, reps, eng):
+    import torch
+    cfg = synth.CONFIGS[config]
+    dx, dy, dz = cfg["size"]
+    r, conv, stop = cfg["r"], cfg["conv"], cfg["stop"]
+    ref, tars = synth.speckle_series_3d(dx, dy, dz, n_frames, device="cuda")
+    xyz = synth.grid_3d(*cfg["grid"])
+    n = len(xyz)
+    seeds = ob.make_poi3d(xyz)
+    eng.set_images_3d(ref, tars[0])
+    eng.fftcc3d(seeds, r, r, r)
+    dev = torch.device("cuda")
+    d_ref, d_tars, d_seeds = (torch.from_numpy(a).to(dev) for a in (ref, tars, seeds))
+    d_q = torch.empty_like(d_seeds)
+    out_a = torch.empty((n_frames, n, ob.POI3D_FLOATS), dtype=torch.float32, device=dev)
+    out_b = torch.empty_like(out_a)
+    stream = torch.cuda.current_stream()
+    eng.set_stream(stream.cuda_stream)
+
+    def loop():
+        d_q.copy_(d_seeds)
+        for f in range(n_frames):
+            eng.set_images_3d_dev(d_ref.data_ptr(), d_tars[f].data_ptr(), dx, dy, dz)
+            eng.icgn3d_prepare()
+            eng.icgn3d1_dev(d_q.data_ptr(), n, r, r, r, conv, stop)
+            out_a[f].copy_(d_q)
+
+    def series():
+        eng.set_series_3d_dev(d_ref.data_ptr(), d_tars.data_ptr(), n_frames, dx, dy, dz)
+        eng.icgn3d_series_dev(d_seeds.data_ptr(), out_b.data_ptr(), n, r, r, r, conv, stop)
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(reps):
+            fn()
+        e1.record(stream)
+        e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    loop()
+    series()  # warm-up: module load, buffers, every kernel
+    torch.cuda.synchronize()
+    identical = torch.equal(out_a.view(torch.int32), out_b.view(torch.int32))
+    ms_a, ms_b = [], []
+    for _ in range(rounds):
+        ms_a.append(timed(loop))
+        ms_b.append(timed(series))
+    identical = identical and torch.equal(out_a.view(torch.int32), out_b.view(torch.int32))
+    eng.use_own_stream()
+    last = out_b[-1].cpu().numpy()
+    return dict(config=config, size=[dx, dy, dz], n_poi=n, r=r, order=1, n_frames=n_frames, reps_per_round=reps,
+                loop_ms=[round(x, 4) for x in ms_a], series_ms=[round(x, 4) for x in ms_b],
+                loop_over_series=[round(a / b, 4) for a, b in zip(ms_a, ms_b)],
+                records_identical=bool(identical), last_frame_valid_frac=float((last[:, 18] >= 0).mean()))
 
 
 def main():
