@@ -192,6 +192,41 @@ int ocb_set_series_3d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars,
 int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop);
 int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop);
 
+/* ---- Series that re-seed lost POIs with FFT-CC in the frame where they are lost.  Replaces the loop a reference user writes
+ *      to keep a field alive over a load series (a crack opening under a subset, glare on one frame, a jump past IC-GN's basin):
+ *        for f: dic.setImages(ref, tar[f]); icgn.prepare(); icgn.compute(queue);
+ *               lost = the POIs with !(zncc >= zncc_min); rebuild each from its seed;
+ *               fftcc.compute(lost) (src/oc_fftcc.cpp); icgn.compute(lost); put them back into queue
+ *      over the series set by ocb_set_series_2d* / ocb_set_series_3d*, frames f = 0 ... n_frames - 1 in order:
+ *        1. every POI is registered from its frame f - 1 record (frame 0: its seed), as ocb_icgn2d_series / ocb_icgn3d_series do;
+ *        2. POI i is lost in frame f when its record has !(zncc >= zncc_min): a NaN ZNCC and every code below zncc_min;
+ *        3. its anchor is the translation (u, v[, w]) of its latest record before frame f with zncc >= zncc_min, else the seed's;
+ *        4. the lost POIs, in ascending order, are rebuilt from their seeds (x, y[, z] and the subset radii copied, the
+ *           translation set to the anchor, every other field 0), then FFT-CC (radii fft_r*) and IC-GN (the series' order,
+ *           radii, conv, stop) run on them against (ref, tars[f]) with the pair calls' kernels.  The result replaces the frame-f
+ *           record whatever its ZNCC: a POI lost again keeps its new code and is tried again in frame f + 1;
+ *        5. frame f + 1 starts from every POI's final frame-f record.
+ *      reseeded[f] (n_frames counts, may be NULL) is the number of POIs re-seeded in frame f.  With zncc_min below every code
+ *      (e.g. -10) nothing is lost and out is byte-identical to the plain series call.
+ *      3D: the records are bit-identical to the loop of ocb_set_images_3d, ocb_icgn3d_prepare, ocb_icgn3d1 on all n POIs, then
+ *      ocb_fftcc3d and ocb_icgn3d1 on the rebuilt lost POIs.  2D: the same holds when OCB_ICGN2D_WPP forces the warps per POI;
+ *      otherwise every IC-GN launch of the call takes the warps per POI of a launch over all n POIs.
+ * Cost: a call that loses nothing adds one scan kernel and one synchronisation (2D) or one of each per frame (3D) to the plain
+ *   series; each frame with losses costs one more synchronisation.
+ * The _dev variants take BORROWED device seeds and out (reseeded is a host pointer); unlike every other series call they
+ *   synchronise ctx's stream, because the per-frame counts size their launches.  Pair state (images, prepared tables) is not
+ *   touched.  Errors are detected before any work and write nothing to out or reseeded: OCB_ERR_STATE without a series,
+ *   OCB_ERR_ARG for bad arguments or sizes, a bad order, a NaN zncc_min or an FFT-CC radius < 1, OCB_ERR_UNSUPPORTED for an FFT-CC
+ *   window or a subset the pair calls reject (with their messages). */
+int ocb_icgn2d_series_reseed(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, int fft_rx,
+	int fft_ry, float zncc_min, size_t* reseeded);
+int ocb_icgn2d_series_reseed_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
+	int fft_rx, int fft_ry, float zncc_min, size_t* reseeded);
+int ocb_icgn3d_series_reseed(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop, int fft_rx,
+	int fft_ry, int fft_rz, float zncc_min, size_t* reseeded);
+int ocb_icgn3d_series_reseed_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop,
+	int fft_rx, int fft_ry, int fft_rz, float zncc_min, size_t* reseeded);
+
 /* ---- IC-LM siblings (SURVEY.md section 8(f) N2): ICLM2D1::compute(std::vector<POI2D>&) src/oc_iclm.cpp:360-368
  *      (per POI :150-358) and ICLM2D2 :732-740 (:502-730).  Same prepare() as IC-GN (ocb_icgn2d_prepare).
  *      lambda, alpha, beta = DampingParameter (src/oc_iclm.h:32-37; defaults 100, 0.1, 10; setDamping()). */

@@ -253,6 +253,30 @@ class Engine:
         self._ck(self._lib.ocb_icgn3d_series(self._ctx, _vp(seeds), _vp(out), seeds.shape[0], rx, ry, rz, conv, stop))
         return out
 
+    def icgn2d_series_reseed(self, order, seeds, rx, ry, conv, stop, fft_rx, fft_ry, zncc_min):
+        """icgn2d_series that re-seeds lost POIs: a POI whose frame-f record has !(zncc >= zncc_min) is rebuilt from its seed at
+        its latest good translation and registered again in frame f by FFTCC2D (radii fft_rx, fft_ry) and IC-GN.  Returns
+        (records float32 (F, n, 25), reseeded int64 (F,): the POIs re-seeded in each frame)."""
+        _check_queue(seeds, POI2D_FLOATS)
+        n_frames = self._series_frames()
+        out = np.empty((n_frames, seeds.shape[0], POI2D_FLOATS), np.float32)
+        counts = np.zeros(n_frames, np.uint64)
+        self._ck(self._lib.ocb_icgn2d_series_reseed(self._ctx, int(order), _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop, int(fft_rx),
+                                                    int(fft_ry), float(zncc_min), _vp(counts)))
+        return out, counts.astype(np.int64)
+
+    def icgn3d_series_reseed(self, seeds, rx, ry, rz, conv, stop, fft_rx, fft_ry, fft_rz, zncc_min):
+        """icgn3d_series that re-seeds lost POIs with FFTCC3D (radii fft_rx, fft_ry, fft_rz) in the frame where they are lost (see
+        icgn2d_series_reseed).  Returns (records float32 (F, n, 31), reseeded int64 (F,))."""
+        _check_queue(seeds, POI3D_FLOATS)
+        if getattr(self, "_n_frames_3d", None) is None:
+            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn3d_series_reseed: no series set")
+        out = np.empty((self._n_frames_3d, seeds.shape[0], POI3D_FLOATS), np.float32)
+        counts = np.zeros(self._n_frames_3d, np.uint64)
+        self._ck(self._lib.ocb_icgn3d_series_reseed(self._ctx, _vp(seeds), _vp(out), seeds.shape[0], rx, ry, rz, conv, stop, int(fft_rx), int(fft_ry),
+                                                    int(fft_rz), float(zncc_min), _vp(counts)))
+        return out, counts.astype(np.int64)
+
     def iclm2d(self, order, q, rx, ry, conv, stop, damping=(100.0, 0.1, 10.0)):
         """ICLM2D1 / ICLM2D2 (reference src/oc_iclm.cpp); damping = (lambda, alpha, beta)."""
         _check_queue(q, POI2D_FLOATS)
@@ -315,6 +339,13 @@ class Engine:
         """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
         self._ck(self._lib.ocb_icgn2d_series_dev(self._ctx, int(order), int(d_seeds), int(d_out), n, rx, ry, conv, stop))
 
+    def icgn2d_series_reseed_dev(self, order, d_seeds, d_out, n, rx, ry, conv, stop, fft_rx, fft_ry, zncc_min):
+        """icgn2d_series_reseed on device pointers; synchronises the stream.  Returns reseeded, int64 (F,)."""
+        counts = np.zeros(self._series_frames(), np.uint64)
+        self._ck(self._lib.ocb_icgn2d_series_reseed_dev(self._ctx, int(order), int(d_seeds), int(d_out), n, rx, ry, conv, stop, int(fft_rx), int(fft_ry),
+                                                        float(zncc_min), _vp(counts)))
+        return counts.astype(np.int64)
+
     def icgn3d1_dev(self, d_q, n, rx, ry, rz, conv, stop):
         self._ck(self._lib.ocb_icgn3d1_dev(self._ctx, int(d_q), n, rx, ry, rz, conv, stop))
 
@@ -326,6 +357,15 @@ class Engine:
     def icgn3d_series_dev(self, d_seeds, d_out, n, rx, ry, rz, conv, stop):
         """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
         self._ck(self._lib.ocb_icgn3d_series_dev(self._ctx, int(d_seeds), int(d_out), n, rx, ry, rz, conv, stop))
+
+    def icgn3d_series_reseed_dev(self, d_seeds, d_out, n, rx, ry, rz, conv, stop, fft_rx, fft_ry, fft_rz, zncc_min):
+        """icgn3d_series_reseed on device pointers; synchronises the stream.  Returns reseeded, int64 (F,)."""
+        if getattr(self, "_n_frames_3d", None) is None:
+            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn3d_series_reseed: no series set")
+        counts = np.zeros(self._n_frames_3d, np.uint64)
+        self._ck(self._lib.ocb_icgn3d_series_reseed_dev(self._ctx, int(d_seeds), int(d_out), n, rx, ry, rz, conv, stop, int(fft_rx), int(fft_ry),
+                                                        int(fft_rz), float(zncc_min), _vp(counts)))
+        return counts.astype(np.int64)
 
     # SIFT3D --------------------------------------------------------------------------------------
     def sift3d(self, config=None, unit=(1.0, 1.0, 1.0), matching_ratio=0.85):

@@ -1166,15 +1166,17 @@ static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rc) {
 size_t icgn2d_slab_bytes(int rx, int ry) { return (size_t)icgn2d_slab_floats(rx, ry, false, 1) * sizeof(float); }
 
 // What a launch over n POIs runs with (icgn2d_plan) and the work-queue head it uses.  A series call takes the pair call's
-// geometry for the same n, so that a frame splits its sums between warps exactly as a pair call does.
+// geometry for the same n, so that a frame splits its sums between warps exactly as a pair call does.  The warps per POI are
+// those of a launch over plan_n POIs (plan_n = n but for a re-seeded sub-queue); the grid never exceeds n.
 struct Icgn2dGeometry {
 	Icgn2dPlan plan;
 	int* counter;
 };
-static int icgn2d_geometry(size_t n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream,
-	Icgn2dGeometry* g, cudaError_t* err) {
+static int icgn2d_geometry(size_t n, size_t plan_n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, int* d_counter,
+	cudaStream_t stream, Icgn2dGeometry* g, cudaError_t* err) {
 	const char* e = getenv("OCB_ICGN2D_WPP"); // tuning knob: 1 or 2 forces the warps per POI
-	if (!icgn2d_plan(n, np, rx, ry, lm, sm_count, smem_optin, e ? atoi(e) : 0, &g->plan)) return -1;
+	if (!icgn2d_plan(plan_n, np, rx, ry, lm, sm_count, smem_optin, e ? atoi(e) : 0, &g->plan)) return -1;
+	if ((size_t)g->plan.grid > n) g->plan.grid = n > 0 ? (int)n : 1;
 	if (g->plan.wpp != 1) {
 		*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
 		if (*err != cudaSuccess) return -2;
@@ -1186,10 +1188,11 @@ static int icgn2d_geometry(size_t n, int np, int rx, int ry, bool lm, int sm_cou
 }
 
 int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
-	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err) {
+	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err,
+	size_t plan_n) {
 	const bool lm = lm_damping != nullptr;
 	Icgn2dGeometry g;
-	if (const int rc = icgn2d_geometry(n, np, rx, ry, lm, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
+	if (const int rc = icgn2d_geometry(n, plan_n, np, rx, ry, lm, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
 	const Icgn2dPlan& p = g.plan;
 	CUtensorMap tm_ref, tm_tar;
 	memset(&tm_ref, 0, sizeof(tm_ref));
@@ -1207,9 +1210,9 @@ int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, i
 }
 
 int icgn2d_series_launch(int np, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
-	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err) {
+	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err, size_t plan_n) {
 	Icgn2dGeometry g;
-	if (const int rc = icgn2d_geometry(n, np, rx, ry, false, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
+	if (const int rc = icgn2d_geometry(n, plan_n, np, rx, ry, false, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
 	const Icgn2dPlan& p = g.plan;
 	CUtensorMap tm_ref, tm_tars;
 	memset(&tm_ref, 0, sizeof(tm_ref));

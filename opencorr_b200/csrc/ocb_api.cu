@@ -161,6 +161,9 @@ struct ocb_ctx {
 	const void* series3_tars = nullptr;
 	size_t series3_u8_pitch = 0; // 0: a float stack
 	int series3_frames = 0;
+	// series calls that re-seed lost POIs: lost-frame/index/histogram/anchor workspace, the rebuilt sub-queue and (2D) the
+	// sub-queue's continuation over the later frames
+	DevBuf reseed_ws, reseed_sub, reseed_cont;
 
 	// FFT
 	std::map<int, float2*> twiddles;
@@ -878,6 +881,37 @@ static FftPath fftcc3d_path(int rx, int ry, int rz) {
 	return rx == ry && ry == rz && ocb::fftcc3d_reg_supported(rx) ? FftPath::REG : FftPath::GENERIC;
 }
 
+// The kernel that takes a (2rx x 2ry) window, or OCB_ERR_UNSUPPORTED with the reason none does.
+static int fftcc2d_plan_or_error(ocb_ctx* ctx, int rx, int ry, ocb::Fftcc2dPlan* plan) {
+	if (ocb::fftcc2d_plan(rx, ry, getenv("OCB_FFTCC2D_GENERIC") != nullptr, ctx->smem_optin, plan)) return OCB_OK;
+	if (plan->reject == ocb::Fftcc2dReject::PRIME_FACTOR)
+		return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: window size %dx%d has a prime factor > 31", 2 * rx, 2 * ry);
+	return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: %dx%d window needs %zu B of shared memory (> %zu)", 2 * rx, 2 * ry, plan->smem,
+		ctx->smem_optin);
+}
+
+// FFT-CC of the n device records q (1 <= n < 2^31) against img, on ctx's device (current) and stream.  The pair calls pass their
+// image pair, the re-seeding series calls one frame of the series.
+static int fftcc2d_run(ocb_ctx* ctx, const ocb::Image2D& img, float* q, size_t n, int rx, int ry) {
+	cudaError_t err;
+	int failed;
+	ocb::Fftcc2dPlan plan;
+	if (const int rc = fftcc2d_plan_or_error(ctx, rx, ry, &plan)) return rc;
+	if (plan.path == ocb::Fftcc2dPath::W32) {
+		failed = ocb::fftcc2d_w32_launch(img, q, n, ctx->sm_count, ctx->stream, &err);
+	} else if (plan.path == ocb::Fftcc2dPath::REG) { // one thread per row
+		failed = ocb::fftcc2d_reg_launch(img, q, n, rx, plan, ctx->sm_count, ctx->stream, &err);
+	} else {
+		const float2 *twx, *twy;
+		int rc;
+		if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy))) return rc;
+		failed = ocb::fftcc2d_launch(img, q, n, rx, ry, plan, twx, twy, ctx->sm_count, ctx->stream, &err);
+	}
+	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(err));
+	ctx->launches++;
+	return OCB_OK;
+}
+
 int ocb_fftcc2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry) {
 	OCB_NO_GROUP(ctx, "fftcc2d_dev");
 	if (!ctx || (!d_poi2d && n) || rx < 1 || ry < 1) return set_error(ctx, OCB_ERR_ARG, "fftcc2d: bad arguments");
@@ -885,29 +919,7 @@ int ocb_fftcc2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry) {
 	if (n == 0) return OCB_OK;
 	if (n > 0x7fffffffull) return set_error(ctx, OCB_ERR_ARG, "fftcc2d: too many POIs in one call");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	float* const q = (float*)d_poi2d;
-	cudaError_t err;
-	int failed;
-	ocb::Fftcc2dPlan plan;
-	if (!ocb::fftcc2d_plan(rx, ry, getenv("OCB_FFTCC2D_GENERIC") != nullptr, ctx->smem_optin, &plan)) {
-		if (plan.reject == ocb::Fftcc2dReject::PRIME_FACTOR)
-			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: window size %dx%d has a prime factor > 31", 2 * rx, 2 * ry);
-		return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc2d: %dx%d window needs %zu B of shared memory (> %zu)", 2 * rx, 2 * ry, plan.smem,
-			ctx->smem_optin);
-	}
-	if (plan.path == ocb::Fftcc2dPath::W32) {
-		failed = ocb::fftcc2d_w32_launch(ctx->img2, q, n, ctx->sm_count, ctx->stream, &err);
-	} else if (plan.path == ocb::Fftcc2dPath::REG) { // one thread per row
-		failed = ocb::fftcc2d_reg_launch(ctx->img2, q, n, rx, plan, ctx->sm_count, ctx->stream, &err);
-	} else {
-		const float2 *twx, *twy;
-		int rc;
-		if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy))) return rc;
-		failed = ocb::fftcc2d_launch(ctx->img2, q, n, rx, ry, plan, twx, twy, ctx->sm_count, ctx->stream, &err);
-	}
-	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(err));
-	ctx->launches++;
-	return OCB_OK;
+	return fftcc2d_run(ctx, ctx->img2, (float*)d_poi2d, n, rx, ry);
 }
 
 int ocb_fftcc2d(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry) {
@@ -918,6 +930,61 @@ int ocb_fftcc2d(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry) {
 	return run_host_queue(ctx, "fftcc2d", poi2d, n, OCB_POI2D_FLOATS, [&](float* d, size_t m, size_t) { return ocb_fftcc2d_dev(ctx, d, m, rx, ry); }, policy);
 }
 
+// The kernel that takes a (2rx x 2ry x 2rz) window, with its grid and scratch per CTA, or OCB_ERR_UNSUPPORTED with the reason none
+// does (a window of < 2^31 points).
+struct Fftcc3dLaunch {
+	FftPath path;
+	ocb::FftAxis ax, ay, az;
+	int grid;
+	size_t cta_scratch; // float2 scratch elements per CTA
+};
+static int fftcc3d_plan_or_error(ocb_ctx* ctx, int rx, int ry, int rz, Fftcc3dLaunch* L) {
+	L->path = fftcc3d_path(rx, ry, rz);
+	if (L->path == FftPath::W32) {
+		L->grid = ocb::fftcc3d_w32_grid(ctx->sm_count);
+		L->cta_scratch = 32768;
+	} else if (L->path == FftPath::REG) {
+		L->grid = ocb::fftcc3d_reg_grid(rx, ctx->sm_count);
+		L->cta_scratch = (size_t)2 * 8 * rx * ry * rz; // two scratch volumes of (2r)^3 complex
+	} else {
+		if (!ocb::fft_plan_axis(2 * rx, &L->ax) || !ocb::fft_plan_axis(2 * ry, &L->ay) || !ocb::fft_plan_axis(2 * rz, &L->az))
+			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window size has a prime factor > 31");
+		if (ocb::fftcc3d_smem_bytes(rx, ry, rz) > ctx->smem_optin)
+			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window needs %zu B of shared memory (> %zu)", ocb::fftcc3d_smem_bytes(rx, ry, rz),
+				ctx->smem_optin);
+		L->grid = ocb::fftcc3d_grid(rx, ry, rz, ctx->sm_count);
+		L->cta_scratch = (size_t)8 * rx * ry * rz;
+	}
+	return OCB_OK;
+}
+
+// FFT-CC of the n device records q (1 <= n < 2^31) against img.ref / img.tar, on ctx's device (current) and stream, with
+// ctx->fft_scratch.  The pair calls pass their volume pair, the re-seeding series call one frame of the series.
+static int fftcc3d_run(ocb_ctx* ctx, const ocb::Image3D& img, float* q, size_t n, int rx, int ry, int rz) {
+	Fftcc3dLaunch L;
+	int rc;
+	if ((rc = fftcc3d_plan_or_error(ctx, rx, ry, rz, &L))) return rc;
+	const float2 *twx = nullptr, *twy = nullptr, *twz = nullptr;
+	if (L.path == FftPath::GENERIC
+		&& ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy)) || (rc = get_twiddles(ctx, 2 * rz, &twz))))
+		return rc;
+	int grid = L.grid;
+	if ((size_t)grid > n) grid = (int)n;
+	if ((rc = grow(ctx, ctx->fft_scratch, (size_t)grid * L.cta_scratch * sizeof(float2)))) return rc;
+	float2* const scratch = ctx->fft_scratch.as<float2>();
+	cudaError_t err;
+	int failed;
+	if (L.path == FftPath::W32)
+		failed = ocb::fftcc3d_w32_launch(img, q, n, scratch, grid, ctx->stream, &err);
+	else if (L.path == FftPath::REG)
+		failed = ocb::fftcc3d_reg_launch(img, q, n, rx, scratch, grid, ctx->stream, &err);
+	else
+		failed = ocb::fftcc3d_launch(img, q, n, rx, ry, rz, L.ax, L.ay, L.az, twx, twy, twz, scratch, grid, ctx->stream, &err);
+	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc3d launch failed: %s", cudaGetErrorString(err));
+	ctx->launches++;
+	return OCB_OK;
+}
+
 int ocb_fftcc3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int rz) {
 	OCB_NO_GROUP(ctx, "fftcc3d_dev");
 	if (!ctx || (!d_poi3d && n) || rx < 1 || ry < 1 || rz < 1) return set_error(ctx, OCB_ERR_ARG, "fftcc3d: bad arguments");
@@ -926,42 +993,7 @@ int ocb_fftcc3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int r
 	if (n > 0x7fffffffull) return set_error(ctx, OCB_ERR_ARG, "fftcc3d: too many POIs in one call");
 	if ((size_t)8 * rx * ry * rz > 0x7fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window too large");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	const FftPath path = fftcc3d_path(rx, ry, rz);
-	ocb::FftAxis ax, ay, az;
-	const float2 *twx = nullptr, *twy = nullptr, *twz = nullptr;
-	int grid, rc;
-	size_t cta_scratch; // float2 scratch elements per CTA
-	if (path == FftPath::W32) {
-		grid = ocb::fftcc3d_w32_grid(ctx->sm_count);
-		cta_scratch = 32768;
-	} else if (path == FftPath::REG) {
-		grid = ocb::fftcc3d_reg_grid(rx, ctx->sm_count);
-		cta_scratch = (size_t)2 * 8 * rx * ry * rz; // two scratch volumes of (2r)^3 complex
-	} else {
-		if (!ocb::fft_plan_axis(2 * rx, &ax) || !ocb::fft_plan_axis(2 * ry, &ay) || !ocb::fft_plan_axis(2 * rz, &az))
-			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window size has a prime factor > 31");
-		if (ocb::fftcc3d_smem_bytes(rx, ry, rz) > ctx->smem_optin)
-			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window needs %zu B of shared memory (> %zu)", ocb::fftcc3d_smem_bytes(rx, ry, rz),
-				ctx->smem_optin);
-		if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy)) || (rc = get_twiddles(ctx, 2 * rz, &twz))) return rc;
-		grid = ocb::fftcc3d_grid(rx, ry, rz, ctx->sm_count);
-		cta_scratch = (size_t)8 * rx * ry * rz;
-	}
-	if ((size_t)grid > n) grid = (int)n;
-	if ((rc = grow(ctx, ctx->fft_scratch, (size_t)grid * cta_scratch * sizeof(float2)))) return rc;
-	float* const q = (float*)d_poi3d;
-	float2* const scratch = ctx->fft_scratch.as<float2>();
-	cudaError_t err;
-	int failed;
-	if (path == FftPath::W32)
-		failed = ocb::fftcc3d_w32_launch(ctx->img3, q, n, scratch, grid, ctx->stream, &err);
-	else if (path == FftPath::REG)
-		failed = ocb::fftcc3d_reg_launch(ctx->img3, q, n, rx, scratch, grid, ctx->stream, &err);
-	else
-		failed = ocb::fftcc3d_launch(ctx->img3, q, n, rx, ry, rz, ax, ay, az, twx, twy, twz, scratch, grid, ctx->stream, &err);
-	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc3d launch failed: %s", cudaGetErrorString(err));
-	ctx->launches++;
-	return OCB_OK;
+	return fftcc3d_run(ctx, ctx->img3, (float*)d_poi3d, n, rx, ry, rz);
 }
 
 int ocb_fftcc3d(ocb_ctx* ctx, void* poi3d, size_t n, int rx, int ry, int rz) {
@@ -978,6 +1010,19 @@ int ocb_icgn2d_prepare(ocb_ctx* ctx) {
 	return OCB_OK;
 }
 
+// IC-GN (lm_damping: IC-LM) of the n device records q (1 <= n < 2^31) against img, on ctx's device (current) and stream, with the
+// warps per POI of a launch over plan_n POIs (ocb::icgn2d_launch).
+static int icgn2d_run(ocb_ctx* ctx, int np, const ocb::Image2D& img, float* q, size_t n, size_t plan_n, int rx, int ry, float conv, float stop,
+	const float* d_offsets, const float* lm_damping) {
+	cudaError_t err = cudaSuccess;
+	int rc = ocb::icgn2d_launch(np, img, q, n, rx, ry, conv, stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter, d_offsets, lm_damping, ctx->stream,
+		&err, plan_n);
+	if (rc == -1) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
+	if (rc) return set_error(ctx, OCB_ERR_CUDA, "icgn2d launch failed: %s", cudaGetErrorString(err));
+	ctx->launches++;
+	return OCB_OK;
+}
+
 static int icgn2d_dev(ocb_ctx* ctx, int np, void* d_poi2d, size_t n, int rx, int ry, float conv, float stop, const float* d_offsets = nullptr,
 	const float* lm_damping = nullptr) {
 	OCB_NO_GROUP(ctx, "icgn2d_dev");
@@ -987,13 +1032,7 @@ static int icgn2d_dev(ocb_ctx* ctx, int np, void* d_poi2d, size_t n, int rx, int
 	if (n == 0) return OCB_OK;
 	if (n > 0x7fffffffull) return set_error(ctx, OCB_ERR_ARG, "icgn2d: too many POIs in one call");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	cudaError_t err = cudaSuccess;
-	int rc = ocb::icgn2d_launch(np, ctx->img2, (float*)d_poi2d, n, rx, ry, conv, stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter, d_offsets, lm_damping,
-		ctx->stream, &err);
-	if (rc == -1) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
-	if (rc) return set_error(ctx, OCB_ERR_CUDA, "icgn2d launch failed: %s", cudaGetErrorString(err));
-	ctx->launches++;
-	return OCB_OK;
+	return icgn2d_run(ctx, np, ctx->img2, (float*)d_poi2d, n, n, rx, ry, conv, stop, d_offsets, lm_damping);
 }
 
 int ocb_icgn2d1_dev(ocb_ctx* ctx, void* d, size_t n, int rx, int ry, float conv, float stop) { return icgn2d_dev(ctx, 6, d, n, rx, ry, conv, stop); }
@@ -1044,34 +1083,164 @@ int ocb_set_series_2d(ocb_ctx* ctx, const float* ref, const float* tars, int n_f
 	return relay_error(ctx, x, rc);
 }
 
-int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop) {
-	OCB_NO_GROUP(ctx, "icgn2d_series_dev");
-	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1) return set_error(ctx, OCB_ERR_ARG, "icgn2d_series: bad arguments");
-	if (order != 1 && order != 2) return set_error(ctx, OCB_ERR_ARG, "icgn2d_series: order must be 1 or 2");
-	if (!ctx->series.ref) return set_error(ctx, OCB_ERR_STATE, "icgn2d_series: no series set");
-	if (n == 0) return OCB_OK;
-	if (n > 0x7fffffffull || (size_t)ctx->series_frames > SIZE_MAX / (n * OCB_POI2D_FLOATS * sizeof(float)))
-		return set_error(ctx, OCB_ERR_ARG, "icgn2d_series: too many POIs in one call");
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	cudaError_t err = cudaSuccess;
-	const int rc = ocb::icgn2d_series_launch(order == 1 ? 6 : 12, ctx->series, ctx->series_frames, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv,
-		stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter, ctx->stream, &err);
-	if (rc == -1) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
-	if (rc) return set_error(ctx, OCB_ERR_CUDA, "icgn2d_series launch failed: %s", cudaGetErrorString(err));
-	ctx->launches++;
+// What a series call that re-seeds lost POIs adds to the plain series (a null SeriesReseed: the plain series).  POI i is lost in
+// frame f when its frame-f record has !(zncc >= zncc_min); its record is then rebuilt from the seed with the translation of its
+// latest good record (the seed's without one), and FFT-CC (radii fft_r) and IC-GN run on it against that frame.  The result
+// replaces the frame-f record and seeds frame f + 1.  counts[f]: the POIs re-seeded in frame f.
+struct SeriesReseed {
+	int fft_r[3];
+	float zncc_min;
+	size_t* counts; // n_frames host counts, zero on entry
+};
+
+// Argument checks shared by the re-seeding entry points (the FFT-CC window is checked against the plan of the pair call)
+static int reseed_check(ocb_ctx* ctx, const char* what, int dim, const SeriesReseed& rs) {
+	if (rs.zncc_min != rs.zncc_min) return set_error(ctx, OCB_ERR_ARG, "%s: zncc_min is NaN", what);
+	for (int a = 0; a < dim; a++)
+		if (rs.fft_r[a] < 1) return set_error(ctx, OCB_ERR_ARG, "%s: FFT-CC radii must be >= 1", what);
+	if (dim == 2) {
+		ocb::Fftcc2dPlan plan;
+		return fftcc2d_plan_or_error(ctx, rs.fft_r[0], rs.fft_r[1], &plan);
+	}
+	if ((size_t)8 * rs.fft_r[0] * rs.fft_r[1] * rs.fft_r[2] > 0x7fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window too large");
+	Fftcc3dLaunch L;
+	return fftcc3d_plan_or_error(ctx, rs.fft_r[0], rs.fft_r[1], rs.fft_r[2], &L);
+}
+
+// Device workspace of a re-seeding call over n POIs and `frames` frames (ctx->reseed_ws): each POI's first lost frame, the
+// compacted sub-queue indices, the per-frame histogram of first lost frames, the sub-queue length, dim anchor floats per POI
+// and the compaction's temporary storage.
+struct ReseedWs {
+	int *first, *idx, *hist, *count;
+	float* anchor;
+	void* temp;
+	size_t temp_bytes;
+	std::vector<int> h_hist;
+};
+static int reseed_workspace(ocb_ctx* ctx, size_t n, int frames, int dim, ReseedWs* w) {
+	auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+	w->temp_bytes = ocb::reseed_select_bytes(n);
+	const size_t o_idx = up(n * sizeof(int)), o_hist = o_idx + up(n * sizeof(int)), o_count = o_hist + up((size_t)frames * sizeof(int));
+	const size_t o_anchor = o_count + 256, o_temp = o_anchor + up(n * dim * sizeof(float));
+	if (const int rc = grow(ctx, ctx->reseed_ws, o_temp + up(w->temp_bytes))) return rc;
+	char* const b = ctx->reseed_ws.as<char>();
+	w->first = (int*)b;
+	w->idx = (int*)(b + o_idx);
+	w->hist = (int*)(b + o_hist);
+	w->count = (int*)(b + o_count);
+	w->anchor = (float*)(b + o_anchor);
+	w->temp = b + o_temp;
+	w->h_hist.assign(frames, 0);
+	OCB_CUDA(ctx, cudaMemsetAsync(w->hist, 0, (size_t)frames * sizeof(int), ctx->stream));
+	return OCB_OK;
+}
+// the histogram of first lost frames, back on the host (the one synchronisation per scan)
+static int reseed_read_hist(ocb_ctx* ctx, ReseedWs* w) {
+	OCB_CUDA(ctx, cudaMemcpyAsync(w->h_hist.data(), w->hist, w->h_hist.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+	OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return OCB_OK;
+}
+// one launch of a series_reseed.cu kernel
+#define OCB_RESEED(ctx, call) \
+	do { \
+		ctx->launches++; \
+		OCB_CUDA(ctx, call); \
+	} while (0)
+
+// gather the POIs whose first lost frame is f (m of them) into the sub-queue, rebuilt from the seeds; prev: frame f - 1's records
+static int reseed_gather(ocb_ctx* ctx, int dim, ReseedWs* w, const float* d_seeds, const float* prev, size_t n, int f, size_t m, float zncc_min,
+	float* sub) {
+	OCB_RESEED(ctx, ocb::reseed_select_launch(w->first, f, n, w->idx, w->count, w->temp, w->temp_bytes, ctx->stream));
+	OCB_RESEED(ctx, ocb::reseed_rebuild_launch(dim, d_seeds, prev, w->idx, m, zncc_min, w->anchor, sub, ctx->sm_count, ctx->stream));
 	return OCB_OK;
 }
 
-int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop) {
+// The 2D series over the n device seeds into d_out (n_frames x n records, frame-major), re-seeding lost POIs when rs is set.
+// Without rs this is one series launch.  With it:
+//   1. the same series launch over all n POIs and frames;
+//   2. one scan of every record for each POI's first lost frame, whose per-frame counts come back in one copy (none: done);
+//   3. for the smallest frame f with losses: its m lost POIs are gathered and rebuilt, FFT-CC and IC-GN run on them against
+//      frame f and the results go to out[f]; then one series launch carries those m records through frames f + 1 ... F - 1
+//      (into ctx->reseed_cont) and they are scattered into out; those m POIs alone are scanned again for a later loss;
+//   4. step 3 repeats for the next frame with losses: one synchronisation per such frame.
+// Every IC-GN launch takes the warps per POI of a launch over all n POIs, so each POI splits its sums as in step 1.
+static int icgn2d_series_run(ocb_ctx* ctx, int np, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
+	const SeriesReseed* rs) {
+	const int F = ctx->series_frames;
+	const ocb::Image2D& s = ctx->series;
+	const size_t frame_px = (size_t)s.w * s.h;
+	auto series = [&](const ocb::Image2D& img, int frames, const float* seeds, float* out, size_t m) -> int {
+		cudaError_t err = cudaSuccess;
+		const int r = ocb::icgn2d_series_launch(np, img, frames, seeds, out, m, rx, ry, conv, stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter,
+			ctx->stream, &err, n);
+		if (r == -1) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
+		if (r) return set_error(ctx, OCB_ERR_CUDA, "icgn2d_series launch failed: %s", cudaGetErrorString(err));
+		ctx->launches++;
+		return (int)OCB_OK;
+	};
+	int rc;
+	if ((rc = series(s, F, d_seeds, d_out, n))) return rc;
+	if (!rs) return OCB_OK;
+	const size_t rec = OCB_POI2D_FLOATS;
+	const float zmin = rs->zncc_min;
+	ReseedWs w;
+	if ((rc = reseed_workspace(ctx, n, F, 2, &w))) return rc;
+	OCB_RESEED(ctx, ocb::reseed_scan_launch(2, d_out, n, 0, F, nullptr, n, zmin, w.first, w.hist, ctx->sm_count, ctx->stream));
+	if ((rc = reseed_read_hist(ctx, &w))) return rc;
+	bool any = false;
+	for (int f = 0; f < F; f++) any = any || w.h_hist[f] > 0;
+	if (!any) return OCB_OK;
+	if ((rc = grow(ctx, ctx->reseed_sub, n * rec * sizeof(float)))) return rc;
+	float* const sub = ctx->reseed_sub.as<float>();
+	OCB_RESEED(ctx, ocb::reseed_anchor_init_launch(2, d_seeds, n, w.anchor, ctx->sm_count, ctx->stream));
+	for (int f = 0; f < F; f++) {
+		const size_t m = (size_t)w.h_hist[f];
+		if (!m) continue;
+		if ((rc = reseed_gather(ctx, 2, &w, d_seeds, f ? d_out + (size_t)(f - 1) * n * rec : nullptr, n, f, m, zmin, sub))) return rc;
+		const ocb::Image2D frame{ s.ref, s.tar + (size_t)f * frame_px, s.w, s.h };
+		if ((rc = fftcc2d_run(ctx, frame, sub, m, rs->fft_r[0], rs->fft_r[1]))) return rc;
+		if ((rc = icgn2d_run(ctx, np, frame, sub, m, n, rx, ry, conv, stop, nullptr, nullptr))) return rc;
+		OCB_RESEED(ctx, ocb::reseed_scatter_launch(2, sub, m, 1, w.idx, d_out, n, f, ctx->sm_count, ctx->stream));
+		rs->counts[f] = m;
+		if (f + 1 == F) break;
+		const int rest = F - f - 1;
+		if ((rc = grow(ctx, ctx->reseed_cont, (size_t)rest * m * rec * sizeof(float)))) return rc;
+		float* const cont = ctx->reseed_cont.as<float>();
+		if ((rc = series(ocb::Image2D{ s.ref, s.tar + (size_t)(f + 1) * frame_px, s.w, s.h }, rest, sub, cont, m))) return rc;
+		OCB_RESEED(ctx, ocb::reseed_scatter_launch(2, cont, m, rest, w.idx, d_out, n, f + 1, ctx->sm_count, ctx->stream));
+		OCB_RESEED(ctx, ocb::reseed_scan_launch(2, d_out, n, f + 1, F, w.idx, m, zmin, w.first, w.hist, ctx->sm_count, ctx->stream));
+		if ((rc = reseed_read_hist(ctx, &w))) return rc;
+	}
+	return OCB_OK;
+}
+
+// Checks and runs a 2D series call on a single-device context: device seeds and output; rs null for the plain series.
+static int icgn2d_series_dev(ocb_ctx* ctx, const char* what, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv,
+	float stop, const SeriesReseed* rs) {
+	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
+	if (order != 1 && order != 2) return set_error(ctx, OCB_ERR_ARG, "%s: order must be 1 or 2", what);
+	if (!ctx->series.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
+	int rc;
+	if (rs && (rc = reseed_check(ctx, what, 2, *rs))) return rc;
+	if (n == 0) return OCB_OK;
+	if (n > 0x7fffffffull || (size_t)ctx->series_frames > SIZE_MAX / (n * OCB_POI2D_FLOATS * sizeof(float)))
+		return set_error(ctx, OCB_ERR_ARG, "%s: too many POIs in one call", what);
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	return icgn2d_series_run(ctx, order == 1 ? 6 : 12, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv, stop, rs);
+}
+
+// Host seeds and output, on the series' executing member: seeds in, the series, every frame's records out
+static int icgn2d_series_host(ocb_ctx* ctx, const char* what, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop,
+	const SeriesReseed* rs) {
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
 	ocb_ctx* x = series_exec(ctx);
 	const int rc = [&]() -> int {
-		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "icgn2d_series: bad arguments");
-		if (!x->series.ref) return set_error(x, OCB_ERR_STATE, "icgn2d_series: no series set");
-		if (n == 0) return ocb_icgn2d_series_dev(x, order, nullptr, nullptr, 0, rx, ry, conv, stop); // argument checks only
+		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "%s: bad arguments", what);
+		if (!x->series.ref) return set_error(x, OCB_ERR_STATE, "%s: no series set", what);
+		if (n == 0) return icgn2d_series_dev(x, what, order, nullptr, nullptr, 0, rx, ry, conv, stop, rs); // argument checks only
 		const size_t rec = OCB_POI2D_FLOATS * sizeof(float);
 		if (n > 0x7fffffffull || (size_t)x->series_frames + 1 > SIZE_MAX / (n * rec))
-			return set_error(x, OCB_ERR_ARG, "icgn2d_series: too many POIs in one call");
+			return set_error(x, OCB_ERR_ARG, "%s: too many POIs in one call", what);
 		if (ensure_device(x)) return OCB_ERR_CUDA;
 		const size_t out_bytes = (size_t)x->series_frames * n * rec;
 		int r;
@@ -1079,12 +1248,45 @@ int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, siz
 		float* const d_seeds = x->d_poi.as<float>();
 		float* const d_out = d_seeds + n * OCB_POI2D_FLOATS;
 		OCB_CUDA(x, cudaMemcpyAsync(d_seeds, seeds, n * rec, cudaMemcpyHostToDevice, x->stream));
-		if ((r = ocb_icgn2d_series_dev(x, order, d_seeds, d_out, n, rx, ry, conv, stop))) return r;
+		if ((r = icgn2d_series_dev(x, what, order, d_seeds, d_out, n, rx, ry, conv, stop, rs))) return r;
 		OCB_CUDA(x, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, x->stream));
 		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
 		return OCB_OK;
 	}();
 	return relay_error(ctx, x, rc);
+}
+
+int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop) {
+	OCB_NO_GROUP(ctx, "icgn2d_series_dev");
+	return icgn2d_series_dev(ctx, "icgn2d_series", order, d_seeds, d_out, n, rx, ry, conv, stop, nullptr);
+}
+
+int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop) {
+	return icgn2d_series_host(ctx, "icgn2d_series", order, seeds, out, n, rx, ry, conv, stop, nullptr);
+}
+
+// The re-seeding calls count into a zeroed vector and copy it to `reseeded` only when the call succeeds.
+static int series_reseed_counts(int rc, const std::vector<size_t>& counts, size_t* reseeded) {
+	if (rc == OCB_OK && reseeded) memcpy(reseeded, counts.data(), counts.size() * sizeof(size_t));
+	return rc;
+}
+
+int ocb_icgn2d_series_reseed_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
+	int fft_rx, int fft_ry, float zncc_min, size_t* reseeded) {
+	OCB_NO_GROUP(ctx, "icgn2d_series_reseed_dev");
+	std::vector<size_t> counts(ctx && ctx->series.ref ? ctx->series_frames : 0, 0);
+	SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts.data() };
+	int rc = icgn2d_series_dev(ctx, "icgn2d_series_reseed", order, d_seeds, d_out, n, rx, ry, conv, stop, &rs);
+	if (rc == OCB_OK && n) OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return series_reseed_counts(rc, counts, reseeded);
+}
+
+int ocb_icgn2d_series_reseed(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, int fft_rx,
+	int fft_ry, float zncc_min, size_t* reseeded) {
+	const ocb_ctx* x = ctx ? series_exec(ctx) : nullptr;
+	std::vector<size_t> counts(x && x->series.ref ? x->series_frames : 0, 0);
+	SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts.data() };
+	return series_reseed_counts(icgn2d_series_host(ctx, "icgn2d_series_reseed", order, seeds, out, n, rx, ry, conv, stop, &rs), counts, reseeded);
 }
 
 // one launch over a host queue (all POIs share the radius), optional host offsets
@@ -1420,49 +1622,69 @@ int ocb_set_series_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned 
 	return relay_error(ctx, x, rc);
 }
 
-int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop) {
-	OCB_NO_GROUP(ctx, "icgn3d_series_dev");
-	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1 || rz < 1) return set_error(ctx, OCB_ERR_ARG, "icgn3d_series: bad arguments");
-	if (!ctx->series3.ref) return set_error(ctx, OCB_ERR_STATE, "icgn3d_series: no series set");
+// Checks and runs a volume series on a single-device context: device seeds and output; rs null for the plain series.  Per frame:
+// the target's prefilter, a copy of the previous frame's records and one LOAD launch; with rs, then a scan of that frame's
+// records (one synchronisation), and for its m lost POIs a rebuild, FFT-CC against the raw frame, IC-GN (COMPUTE) and a scatter.
+static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv,
+	float stop, const SeriesReseed* rs) {
+	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1 || rz < 1) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
+	if (!ctx->series3.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
+	int rc;
+	if (rs && (rc = reseed_check(ctx, what, 3, *rs))) return rc;
 	if (n == 0) return OCB_OK;
 	const size_t rec = OCB_POI3D_FLOATS * sizeof(float);
 	if (n > 0x7fffffffull || (size_t)ctx->series3_frames > SIZE_MAX / (n * rec))
-		return set_error(ctx, OCB_ERR_ARG, "icgn3d_series: too many POIs in one call");
+		return set_error(ctx, OCB_ERR_ARG, "%s: too many POIs in one call", what);
 	if ((size_t)(2 * rx + 1) * (2 * ry + 1) * (2 * rz + 1) > 0x3fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn3d1: subset too large");
 	ocb::Icgn3dPlan plan;
 	if (!ocb::icgn3d1_plan(rx, ry, rz, ctx->smem_optin, &plan))
 		return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn3d1: subset radius (%d,%d,%d) exceeds the shared-memory design limit", rx, ry, rz);
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	const int F = ctx->series3_frames;
 	const int dx = ctx->series3.dx, dy = ctx->series3.dy, dz = ctx->series3.dz;
 	const size_t elems = (size_t)dx * dy * dz;
-	int rc;
 	if ((rc = grow(ctx, ctx->series3_rg, elems * sizeof(float4))) || (rc = grow(ctx, ctx->series3_coef, elems * sizeof(float)))
 		|| (rc = grow(ctx, ctx->series3_tmp, elems * sizeof(float))) || (rc = grow(ctx, ctx->series3_cache, n * ocb::ICGN3D_SETUP_FLOATS * sizeof(float))))
 		return rc;
+	ReseedWs w;
+	if (rs && ((rc = reseed_workspace(ctx, n, F, 3, &w)) || (rc = grow(ctx, ctx->reseed_sub, n * rec)))) return rc;
+	float* const sub = rs ? ctx->reseed_sub.as<float>() : nullptr;
 	float4* const rg = ctx->series3_rg.as<float4>();
 	float* const coef = ctx->series3_coef.as<float>();
 	float* const tmp = ctx->series3_tmp.as<float>();
 	float* const cache = ctx->series3_cache.as<float>();
 	const ocb::Image3D img{ ctx->series3.ref, nullptr, rg, coef, dx, dy, dz };
 	cudaError_t err = cudaSuccess;
-	auto icgn = [&](float* q, int setup) {
-		const int r3 = ocb::icgn3d1_launch(img, q, n, rx, ry, rz, conv, stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter + 1, ctx->stream, &err, setup,
+	auto icgn = [&](float* q, size_t m, int setup) {
+		const int r3 = ocb::icgn3d1_launch(img, q, m, rx, ry, rz, conv, stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter + 1, ctx->stream, &err, setup,
 			cache);
 		if (r3) return set_error(ctx, OCB_ERR_CUDA, "icgn3d_series launch failed: %s", cudaGetErrorString(err));
 		ctx->launches++;
 		return (int)OCB_OK;
 	};
-	// the reference's products, once per call: packed gradients, then each POI's setup pass (records are not written)
+	auto widen = [&](int f) {
+		ocb::widen_u8_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const unsigned char*)ctx->series3_tars + (size_t)f * ctx->series3_u8_pitch, tmp,
+			elems);
+		ctx->launches++;
+	};
+	// the reference's products, once per call: packed gradients, then each POI's setup pass (records are not written).
+	// A re-seeding call stores the setup state of neutral copies of the seeds (zero translation, ZNCC 0), so every POI whose
+	// subvolume lies inside the volume gets an entry, a seed the guard rejects included: re-seeded in frame f, such a POI
+	// reaches frame f + 1's LOAD with a good record.  The setup state depends only on the reference, the coordinates and the
+	// radii, so the entries of the POIs the plain series stores are the same; a POI without one (coordinates outside the
+	// volume or NaN) is still rejected by every guard.
 	ocb::gradient3d_launch(ctx->series3.ref, rg, dx, dy, dz, ctx->sm_count, ctx->stream);
 	ctx->launches++;
-	if ((rc = icgn(const_cast<float*>((const float*)d_seeds), ocb::ICGN3D_SETUP_STORE))) return rc;
-	for (int f = 0; f < ctx->series3_frames; f++) {
+	if (rs) {
+		OCB_RESEED(ctx, ocb::reseed_rebuild_launch(3, (const float*)d_seeds, nullptr, nullptr, n, 0.f, nullptr, sub, ctx->sm_count, ctx->stream));
+		OCB_RESEED(ctx, ocb::reseed_anchor_init_launch(3, (const float*)d_seeds, n, w.anchor, ctx->sm_count, ctx->stream));
+	}
+	if ((rc = icgn(rs ? sub : const_cast<float*>((const float*)d_seeds), n, ocb::ICGN3D_SETUP_STORE))) return rc;
+	for (int f = 0; f < F; f++) {
 		// TricubicBspline::prepare of frame f as in ocb_icgn3d_prepare: x -> coefficient, y -> scratch, z -> coefficient
 		const float* tar;
 		if (ctx->series3_u8_pitch) {
-			ocb::widen_u8_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const unsigned char*)ctx->series3_tars + (size_t)f * ctx->series3_u8_pitch,
-				tmp, elems);
-			ctx->launches++;
+			widen(f);
 			tar = tmp;
 		} else {
 			tar = (const float*)ctx->series3_tars + (size_t)f * elems;
@@ -1473,23 +1695,36 @@ int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t
 		ctx->launches += 3;
 		OCB_CUDA(ctx, cudaGetLastError());
 		float* const q = (float*)d_out + (size_t)f * n * OCB_POI3D_FLOATS;
-		const void* prev = f == 0 ? d_seeds : (const void*)(q - n * OCB_POI3D_FLOATS);
+		const float* prev = f == 0 ? (const float*)d_seeds : q - n * OCB_POI3D_FLOATS;
 		OCB_CUDA(ctx, cudaMemcpyAsync(q, prev, n * rec, cudaMemcpyDeviceToDevice, ctx->stream));
-		if ((rc = icgn(q, ocb::ICGN3D_SETUP_LOAD))) return rc;
+		if ((rc = icgn(q, n, ocb::ICGN3D_SETUP_LOAD))) return rc;
+		if (!rs) continue;
+		OCB_RESEED(ctx, ocb::reseed_scan_launch(3, (const float*)d_out, n, f, f + 1, nullptr, n, rs->zncc_min, w.first, w.hist, ctx->sm_count, ctx->stream));
+		if ((rc = reseed_read_hist(ctx, &w))) return rc;
+		const size_t m = (size_t)w.h_hist[f];
+		if (!m) continue;
+		if ((rc = reseed_gather(ctx, 3, &w, (const float*)d_seeds, f ? prev : nullptr, n, f, m, rs->zncc_min, sub))) return rc;
+		if (ctx->series3_u8_pitch) widen(f); // the prefilter's y pass overwrote the widened frame
+		const ocb::Image3D raw{ ctx->series3.ref, ctx->series3_u8_pitch ? tmp : tar, rg, coef, dx, dy, dz };
+		if ((rc = fftcc3d_run(ctx, raw, sub, m, rs->fft_r[0], rs->fft_r[1], rs->fft_r[2]))) return rc;
+		if ((rc = icgn(sub, m, ocb::ICGN3D_SETUP_COMPUTE))) return rc;
+		OCB_RESEED(ctx, ocb::reseed_scatter_launch(3, sub, m, 1, w.idx, (float*)d_out, n, f, ctx->sm_count, ctx->stream));
+		rs->counts[f] = m;
 	}
 	return OCB_OK;
 }
 
-int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop) {
+static int icgn3d_series_host(ocb_ctx* ctx, const char* what, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop,
+	const SeriesReseed* rs) {
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
 	ocb_ctx* x = series_exec(ctx);
 	const int rc = [&]() -> int {
-		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "icgn3d_series: bad arguments");
-		if (!x->series3.ref) return set_error(x, OCB_ERR_STATE, "icgn3d_series: no series set");
-		if (n == 0) return ocb_icgn3d_series_dev(x, nullptr, nullptr, 0, rx, ry, rz, conv, stop); // argument checks only
+		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "%s: bad arguments", what);
+		if (!x->series3.ref) return set_error(x, OCB_ERR_STATE, "%s: no series set", what);
+		if (n == 0) return icgn3d_series_dev(x, what, nullptr, nullptr, 0, rx, ry, rz, conv, stop, rs); // argument checks only
 		const size_t rec = OCB_POI3D_FLOATS * sizeof(float);
 		if (n > 0x7fffffffull || (size_t)x->series3_frames + 1 > SIZE_MAX / (n * rec))
-			return set_error(x, OCB_ERR_ARG, "icgn3d_series: too many POIs in one call");
+			return set_error(x, OCB_ERR_ARG, "%s: too many POIs in one call", what);
 		if (ensure_device(x)) return OCB_ERR_CUDA;
 		const size_t out_bytes = (size_t)x->series3_frames * n * rec;
 		int r;
@@ -1497,12 +1732,39 @@ int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int 
 		float* const d_seeds = x->d_poi.as<float>();
 		float* const d_out = d_seeds + n * OCB_POI3D_FLOATS;
 		OCB_CUDA(x, cudaMemcpyAsync(d_seeds, seeds, n * rec, cudaMemcpyHostToDevice, x->stream));
-		if ((r = ocb_icgn3d_series_dev(x, d_seeds, d_out, n, rx, ry, rz, conv, stop))) return r;
+		if ((r = icgn3d_series_dev(x, what, d_seeds, d_out, n, rx, ry, rz, conv, stop, rs))) return r;
 		OCB_CUDA(x, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, x->stream));
 		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
 		return OCB_OK;
 	}();
 	return relay_error(ctx, x, rc);
+}
+
+int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop) {
+	OCB_NO_GROUP(ctx, "icgn3d_series_dev");
+	return icgn3d_series_dev(ctx, "icgn3d_series", d_seeds, d_out, n, rx, ry, rz, conv, stop, nullptr);
+}
+
+int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop) {
+	return icgn3d_series_host(ctx, "icgn3d_series", seeds, out, n, rx, ry, rz, conv, stop, nullptr);
+}
+
+int ocb_icgn3d_series_reseed_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop, int fft_rx,
+	int fft_ry, int fft_rz, float zncc_min, size_t* reseeded) {
+	OCB_NO_GROUP(ctx, "icgn3d_series_reseed_dev");
+	std::vector<size_t> counts(ctx && ctx->series3.ref ? ctx->series3_frames : 0, 0);
+	SeriesReseed rs{ { fft_rx, fft_ry, fft_rz }, zncc_min, counts.data() };
+	int rc = icgn3d_series_dev(ctx, "icgn3d_series_reseed", d_seeds, d_out, n, rx, ry, rz, conv, stop, &rs);
+	if (rc == OCB_OK && n) OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return series_reseed_counts(rc, counts, reseeded);
+}
+
+int ocb_icgn3d_series_reseed(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop, int fft_rx,
+	int fft_ry, int fft_rz, float zncc_min, size_t* reseeded) {
+	const ocb_ctx* x = ctx ? series_exec(ctx) : nullptr;
+	std::vector<size_t> counts(x && x->series3.ref ? x->series3_frames : 0, 0);
+	SeriesReseed rs{ { fft_rx, fft_ry, fft_rz }, zncc_min, counts.data() };
+	return series_reseed_counts(icgn3d_series_host(ctx, "icgn3d_series_reseed", seeds, out, n, rx, ry, rz, conv, stop, &rs), counts, reseeded);
 }
 
 int ocb_get_tables_3d(ocb_ctx* ctx, float* gx, float* gy, float* gz, float* coefficient) {

@@ -112,12 +112,34 @@ inline bool icgn2d_plan(size_t n, int np, int rx, int ry, bool lm, int sm_count,
 	return true;
 }
 
+// plan_n: the queue length whose warps per POI the launch takes (icgn2d_plan); n for a plain call.  A re-seeded sub-queue passes
+// the length of the whole queue, so that its POIs split their sums as they do in the launch over all of them.
 int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
-	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err);
+	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err,
+	size_t plan_n);
 size_t icgn2d_slab_bytes(int rx, int ry); // shared memory one POI needs (plain IC-GN, one warp per POI)
 // one reference (img.ref) against the frame-major stack img.tar [n_frames][h][w]: n seeds in, n_frames x n records out (frame-major)
 int icgn2d_series_launch(int np, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
-	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err);
+	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err, size_t plan_n);
+// series_reseed.cu: the lost-POI scan, compaction, rebuild and scatter of the re-seeding series calls (dim: 2 or 3; records
+// frame-major, out[f * n + i]).  Each returns the launch's CUDA error.
+// scan: for the POIs idx[0..m) (0..m when idx is null), first[i] = the first frame in [f_begin, f_end) with !(zncc >= zncc_min), or
+// -1; hist[f] += the POIs whose first lost frame is f.
+cudaError_t reseed_scan_launch(int dim, const float* d_out, size_t n, int f_begin, int f_end, const int* d_idx, size_t m, float zncc_min, int* d_first,
+	int* d_hist, int sm_count, cudaStream_t stream);
+// select: idx = the POIs i < n with first[i] == f, in ascending order (stable compaction), *d_count = how many
+size_t reseed_select_bytes(size_t n); // temporary storage reseed_select_launch needs
+cudaError_t reseed_select_launch(const int* d_first, int f, size_t n, int* d_idx, int* d_count, void* d_temp, size_t temp_bytes, cudaStream_t stream);
+// anchor_init: anchor[i] = seed i's translation (dim floats per POI)
+cudaError_t reseed_anchor_init_launch(int dim, const float* d_seeds, size_t n, float* d_anchor, int sm_count, cudaStream_t stream);
+// rebuild: sub[k] = POI idx[k]'s seed with every field but the position and the subset radii zeroed and the translation set to its
+// anchor; when prev (the frame before's records) holds a good record for the POI, its translation becomes the anchor first.
+// idx null: the first m POIs; anchor null: zero translation.
+cudaError_t reseed_rebuild_launch(int dim, const float* d_seeds, const float* d_prev, const int* d_idx, size_t m, float zncc_min, float* d_anchor,
+	float* d_sub, int sm_count, cudaStream_t stream);
+// scatter: record k of frame g of src (frames x m records, frame-major) -> out[(f0 + g) * n + idx[k]]
+cudaError_t reseed_scatter_launch(int dim, const float* d_src, size_t m, int frames, const int* d_idx, float* d_out, size_t n, int f0, int sm_count,
+	cudaStream_t stream);
 // nr2d.cu
 constexpr int NR2D_TILE_MARGIN = 1;
 __host__ __device__ inline int nr2d_tar_w(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * NR2D_TILE_MARGIN + 4 + 3); }
