@@ -297,6 +297,39 @@ int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* i
 int ocb_stereo_reconstruct_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
 	const float* intrinsics2, const float* projection2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n);
 
+/* ---- Stereo DIC over a load series of stereo pairs: both views of every frame registered against reference view 1 and
+ *      triangulated, the loop of the reference's 3D-DIC example (examples/test_3d_dic_epipolar_sift.cpp:178-317) over frames,
+ *      each frame seeded by the previous one instead of by SIFT features.
+ * State (ocb_set_stereo_series_2d*): ref1, reference view 1 (width x height), and tars1 / tars2, n_frames row-major images each,
+ *   frame-major: view 1 and view 2 of frames 0 ... n_frames - 1.  All images have the same size.  The reference view-2 image is
+ *   not part of it: the r1 -> r2 match is an input (from the pair calls: ocb_set_images_2d(r1, r2), ocb_icgn2d_prepare,
+ *   ocb_epipolar_search2d, ocb_icgn2d2).  The state is the context's own: the pair calls and ocb_set_series_2d* neither see nor
+ *   change it, and it changes neither.  On a group context the first member holds it and runs the calls.
+ * Inputs: stereo, n POI2D records of the r1 -> r2 match; seeds1 / seeds2, n POI2D frame-0 guesses of view 1 / view 2; order1,
+ *   order2 = 1 (ICGN2D1) or 2 (ICGN2D2); rx, ry, conv, stop shared by both views; the cameras as ocb_stereo_reconstruct takes them.
+ * For every frame f:
+ *   out1[f] = IC-GN (order1) of (ref1, tars1[f]) from out1[f - 1] (frame 0: seeds1): bit for bit ocb_icgn2d_series on (ref1, tars1);
+ *   out2[f] = IC-GN (order2) of (ref1, tars2[f]) from out2[f - 1] (frame 0: seeds2): bit for bit ocb_icgn2d_series on (ref1, tars2);
+ *   out2ds[f][i], a POI2DS record, all float32: x, y of seeds1[i]; r2 = stereo location + (u, v), t1 = out1[f] location + (u, v),
+ *   t2 = out2[f] location + (u, v), stored unclamped; ZNCCs r1r2 / r1t1 / r1t2 of stereo / out1[f] / out2[f] (failure codes
+ *   included); ref_coor = reconstruct((x, y), r2), tar_coor = reconstruct(t1, t2), where reconstruct is ocb_stereo_reconstruct on
+ *   copies of the points (clamped per camera; a NaN coordinate gives (0, 0, 0)); u, v, w = tar_coor - ref_coor; strain and
+ *   subset_radius 0.  Strain over frame f: ocb_strain2ds(ctx, out2ds + f * n * OCB_POI2DS_FLOATS, n, ...).
+ * out1, out2: n_frames x n POI2D records, out2ds: n_frames x n POI2DS records, frame-major, overlapping no input.  A long series
+ *   runs in chunks: the last frame's slices of out1 and out2 seed the next chunk.
+ * The host variants copy (ocb_stereo_series blocks until the outputs are filled); the _dev variants take BORROWED device images,
+ *   records and outputs (the camera arrays stay host pointers) and only enqueue.  Errors are detected before any work and write
+ *   nothing to any output: OCB_ERR_STATE without a stereo series, OCB_ERR_ARG for a bad order, NULL pointers, sizes or a calibration
+ *   handle of another context, OCB_ERR_UNSUPPORTED for radii the pair calls reject. */
+int ocb_set_stereo_series_2d(ocb_ctx* ctx, const float* ref1, const float* tars1, const float* tars2, int n_frames, int width, int height);
+int ocb_set_stereo_series_2d_dev(ocb_ctx* ctx, const float* d_ref1, const float* d_tars1, const float* d_tars2, int n_frames, int width, int height);
+int ocb_stereo_series(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, int order1, int order2, const void* stereo, const void* seeds1, const void* seeds2,
+	void* out1, void* out2, void* out2ds, size_t n, int rx, int ry, float conv, float stop);
+int ocb_stereo_series_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, int order1, int order2, const void* d_stereo, const void* d_seeds1, const void* d_seeds2,
+	void* d_out1, void* d_out2, void* d_out2ds, size_t n, int rx, int ry, float conv, float stop);
+
 /* ---- SIFT3D: SIFT3D::compute() src/oc_sift.cpp:234-293 on the volumes of ocb_set_images_3d / _u8 / _dev --------------------
  * Extracts the keypoints of the reference and of the target volume (Gaussian pyramid :676-754 built one octave at a time, DoG
  * extrema :795-847, orientation :849-1049, descriptors :1051-1249) and matches them (monodirectionalMatch :1251-1418).

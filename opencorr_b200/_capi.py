@@ -93,6 +93,10 @@ SIGNATURES = {
     "ocb_calib_undistort": (_i, [_vp, _vp, _vp, _vp, _vp, _sz]),
     "ocb_stereo_reconstruct": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz]),
     "ocb_stereo_reconstruct_dev": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz]),
+    "ocb_set_stereo_series_2d": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i]),
+    "ocb_set_stereo_series_2d_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i]),
+    "ocb_stereo_series": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i, _i, _f, _f]),
+    "ocb_stereo_series_dev": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_sift3d": (_i, [_vp, _vp, _vp, _f, ctypes.POINTER(_sz), ctypes.POINTER(_i)]),
     "ocb_sift3d_get_matches": (_i, [_vp, _vp, _vp]),
     "ocb_sift3d_inspect": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp]),

@@ -22,6 +22,7 @@ from . import _capi
 # ---- POI record layout (reference src/oc_poi.h) ------------------------------------------------
 POI2D_FLOATS = 25
 POI3D_FLOATS = 31
+POI2DS_FLOATS = 28
 P2 = dict(x=0, y=1, u=2, ux=3, uy=4, uxx=5, uxy=6, uyy=7, v=8, vx=9, vy=10, vxx=11, vxy=12, vyy=13,
           u0=14, v0=15, zncc=16, iteration=17, convergence=18, feature=19, exx=20, eyy=21, exy=22,
           subset_rx=23, subset_ry=24)
@@ -277,6 +278,46 @@ class Engine:
                                                     int(fft_rz), float(zncc_min), _vp(counts)))
         return out, counts.astype(np.int64)
 
+    def set_stereo_series(self, ref1, tars1, tars2):
+        """A stereo load series for stereo_series: reference view 1 (H, W) and the two views of every frame, tars1 and tars2
+        (F, H, W), float32.  Kept apart from set_images_2d's pair and set_series_2d's series."""
+        ref1 = np.ascontiguousarray(ref1, dtype=np.float32)
+        tars1 = np.ascontiguousarray(tars1, dtype=np.float32)
+        tars2 = np.ascontiguousarray(tars2, dtype=np.float32)
+        if ref1.ndim != 2 or tars1.ndim != 3 or tars1.shape[1:] != ref1.shape or tars2.shape != tars1.shape:
+            raise ValueError("ref1 must be (H, W) and tars1, tars2 (F, H, W)")
+        f, h, w = tars1.shape
+        self._ck(self._lib.ocb_set_stereo_series_2d(self._ctx, _vp(ref1), _vp(tars1), _vp(tars2), f, w, h))
+        self._ck(self._lib.ocb_sync(self._ctx))
+        self._n_frames_stereo = f
+
+    def _stereo_frames(self):
+        if getattr(self, "_n_frames_stereo", None) is None:
+            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "stereo_series: no stereo series set")
+        return self._n_frames_stereo
+
+    def stereo_series(self, rig, stereo, seeds1, seeds2, order1, order2, rx, ry, conv, stop):
+        """Both views of every frame of the series set by set_stereo_series, registered against reference view 1 and
+        triangulated by `rig` (a Stereovision whose cameras were prepared on this engine):
+        out1[f] = ICGN2D<order1> of (ref1, tars1[f]) from out1[f - 1] (frame 0: seeds1), out2[f] the same for view 2 with
+        order2 and seeds2, and out2ds[f] the POI2DS records of frame f (include/opencorr_b200.h ocb_stereo_series).  stereo:
+        the r1 -> r2 records, [n, 25].  Returns (out1 (F, n, 25), out2 (F, n, 25), out2ds (F, n, 28)), float32; the inputs are
+        not changed."""
+        for q in (stereo, seeds1, seeds2):
+            _check_queue(q, POI2D_FLOATS)
+        n = seeds1.shape[0]
+        if stereo.shape[0] != n or seeds2.shape[0] != n:
+            raise ValueError("stereo, seeds1 and seeds2 must hold the same number of POIs")
+        rig._engine()
+        h1, i1, p1, h2, i2, p2 = rig._cameras()
+        f = self._stereo_frames()
+        out1 = np.empty((f, n, POI2D_FLOATS), np.float32)
+        out2 = np.empty((f, n, POI2D_FLOATS), np.float32)
+        out2ds = np.empty((f, n, POI2DS_FLOATS), np.float32)
+        self._ck(self._lib.ocb_stereo_series(self._ctx, h1, _vp(i1), _vp(p1), h2, _vp(i2), _vp(p2), int(order1), int(order2), _vp(stereo),
+                                             _vp(seeds1), _vp(seeds2), _vp(out1), _vp(out2), _vp(out2ds), n, rx, ry, conv, stop))
+        return out1, out2, out2ds
+
     def iclm2d(self, order, q, rx, ry, conv, stop, damping=(100.0, 0.1, 10.0)):
         """ICLM2D1 / ICLM2D2 (reference src/oc_iclm.cpp); damping = (lambda, alpha, beta)."""
         _check_queue(q, POI2D_FLOATS)
@@ -366,6 +407,21 @@ class Engine:
         self._ck(self._lib.ocb_icgn3d_series_reseed_dev(self._ctx, int(d_seeds), int(d_out), n, rx, ry, rz, conv, stop, int(fft_rx), int(fft_ry),
                                                         int(fft_rz), float(zncc_min), _vp(counts)))
         return counts.astype(np.int64)
+
+    def set_stereo_series_dev(self, d_ref1, d_tars1, d_tars2, n_frames, width, height):
+        """Device pointers: reference view 1 (height x width) and the frame-major stacks of view 1 and view 2 (n_frames images
+        each); borrowed, not copied."""
+        self._ck(self._lib.ocb_set_stereo_series_2d_dev(self._ctx, int(d_ref1), int(d_tars1), int(d_tars2), n_frames, width, height))
+        self._n_frames_stereo = int(n_frames)
+
+    def stereo_series_dev(self, rig, d_stereo, d_seeds1, d_seeds2, d_out1, d_out2, d_out2ds, n, order1, order2, rx, ry, conv, stop):
+        """stereo_series on device pointers: n records each of stereo, seeds1, seeds2 in; n_frames x n POI2D records into d_out1
+        and d_out2 and n_frames x n POI2DS records into d_out2ds (frame-major); enqueue only."""
+        rig._engine()
+        h1, i1, p1, h2, i2, p2 = rig._cameras()
+        self._ck(self._lib.ocb_stereo_series_dev(self._ctx, h1, _vp(i1), _vp(p1), h2, _vp(i2), _vp(p2), int(order1), int(order2), int(d_stereo),
+                                                 int(d_seeds1), int(d_seeds2), int(d_out1), int(d_out2), int(d_out2ds), int(n), rx, ry, conv,
+                                                 stop))
 
     # SIFT3D --------------------------------------------------------------------------------------
     def sift3d(self, config=None, unit=(1.0, 1.0, 1.0), matching_ratio=0.85):

@@ -144,6 +144,11 @@ struct ocb_ctx {
 	DevBuf own_series[2]; // {ref, stack} uploaded from the host
 	ocb::Image2D series{ nullptr, nullptr, 0, 0 };
 	int series_frames = 0;
+	// stereo image series (ocb_set_stereo_series_2d*): its own state, untouched by the pair calls and the 2D series.  stereo1 /
+	// stereo2 share the reference view-1 image; their .tar are the frame-major stacks of view 1 and view 2.
+	DevBuf own_stereo[3]; // {ref1, view-1 stack, view-2 stack} uploaded from the host
+	ocb::Image2D stereo1{ nullptr, nullptr, 0, 0 }, stereo2{ nullptr, nullptr, 0, 0 };
+	int stereo_frames = 0;
 
 	// 3D images + tables
 	DevBuf own3[2]; // {ref, tar} uploaded from the host
@@ -1155,7 +1160,8 @@ static int reseed_gather(ocb_ctx* ctx, int dim, ReseedWs* w, const float* d_seed
 	return OCB_OK;
 }
 
-// The 2D series over the n device seeds into d_out (n_frames x n records, frame-major), re-seeding lost POIs when rs is set.
+// The 2D series of reference s.ref against the F frames of the stack s.tar, over the n device seeds into d_out (F x n records,
+// frame-major), re-seeding lost POIs when rs is set.
 // Without rs this is one series launch.  With it:
 //   1. the same series launch over all n POIs and frames;
 //   2. one scan of every record for each POI's first lost frame, whose per-frame counts come back in one copy (none: done);
@@ -1164,10 +1170,8 @@ static int reseed_gather(ocb_ctx* ctx, int dim, ReseedWs* w, const float* d_seed
 //      (into ctx->reseed_cont) and they are scattered into out; those m POIs alone are scanned again for a later loss;
 //   4. step 3 repeats for the next frame with losses: one synchronisation per such frame.
 // Every IC-GN launch takes the warps per POI of a launch over all n POIs, so each POI splits its sums as in step 1.
-static int icgn2d_series_run(ocb_ctx* ctx, int np, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
-	const SeriesReseed* rs) {
-	const int F = ctx->series_frames;
-	const ocb::Image2D& s = ctx->series;
+static int icgn2d_series_run(ocb_ctx* ctx, int np, const ocb::Image2D& s, int F, const float* d_seeds, float* d_out, size_t n, int rx, int ry,
+	float conv, float stop, const SeriesReseed* rs) {
 	const size_t frame_px = (size_t)s.w * s.h;
 	auto series = [&](const ocb::Image2D& img, int frames, const float* seeds, float* out, size_t m) -> int {
 		cudaError_t err = cudaSuccess;
@@ -1226,7 +1230,8 @@ static int icgn2d_series_dev(ocb_ctx* ctx, const char* what, int order, const vo
 	if (n > 0x7fffffffull || (size_t)ctx->series_frames > SIZE_MAX / (n * OCB_POI2D_FLOATS * sizeof(float)))
 		return set_error(ctx, OCB_ERR_ARG, "%s: too many POIs in one call", what);
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	return icgn2d_series_run(ctx, order == 1 ? 6 : 12, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv, stop, rs);
+	return icgn2d_series_run(ctx, order == 1 ? 6 : 12, ctx->series, ctx->series_frames, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv, stop,
+		rs);
 }
 
 // Host seeds and output, on the series' executing member: seeds in, the series, every frame's records out
@@ -1941,6 +1946,136 @@ int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* i
 		OCB_CUDA(x, cudaMemcpyAsync(pts1, d1, b2, cudaMemcpyDeviceToHost, x->stream));
 		OCB_CUDA(x, cudaMemcpyAsync(pts2, d2, b2, cudaMemcpyDeviceToHost, x->stream));
 		OCB_CUDA(x, cudaMemcpyAsync(pts3d, d3, b3, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+// ---- Stereo series: both views of every frame registered against reference view 1, triangulated into POI2DS records ---------
+// On a group context the first member holds the series and runs the calls; the calibration maps of a group live there too.
+static void stereo_series_set(ocb_ctx* x, const float* ref1, const float* tars1, const float* tars2, int n_frames, int width, int height) {
+	x->stereo1 = ocb::Image2D{ ref1, tars1, width, height };
+	x->stereo2 = ocb::Image2D{ ref1, tars2, width, height };
+	x->stereo_frames = n_frames;
+}
+
+int ocb_set_stereo_series_2d_dev(ocb_ctx* ctx, const float* d_ref1, const float* d_tars1, const float* d_tars2, int n_frames, int width, int height) {
+	OCB_NO_GROUP(ctx, "set_stereo_series_2d_dev");
+	if (!ctx || !d_ref1 || !d_tars1 || !d_tars2 || n_frames < 1 || width < 5 || height < 5)
+		return set_error(ctx, OCB_ERR_ARG, "set_stereo_series_2d: bad arguments");
+	stereo_series_set(ctx, d_ref1, d_tars1, d_tars2, n_frames, width, height);
+	return OCB_OK;
+}
+
+int ocb_set_stereo_series_2d(ocb_ctx* ctx, const float* ref1, const float* tars1, const float* tars2, int n_frames, int width, int height) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* x = series_exec(ctx);
+	const int rc = [&]() -> int {
+		if (!ref1 || !tars1 || !tars2 || n_frames < 1 || width < 5 || height < 5) return set_error(x, OCB_ERR_ARG, "set_stereo_series_2d: bad arguments");
+		const size_t elems = (size_t)width * height;
+		if ((size_t)n_frames > SIZE_MAX / sizeof(float) / elems) return set_error(x, OCB_ERR_ARG, "set_stereo_series_2d: series too large");
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		stereo_series_set(x, nullptr, nullptr, nullptr, 0, 0, 0); // a failed growth below leaves no series rather than a stale one
+		const size_t frame = elems * sizeof(float), stack = (size_t)n_frames * frame;
+		int r;
+		if ((r = grow(x, x->own_stereo[0], frame)) || (r = grow(x, x->own_stereo[1], stack)) || (r = grow(x, x->own_stereo[2], stack))) return r;
+		OCB_CUDA(x, cudaMemcpyAsync(x->own_stereo[0].p, ref1, frame, cudaMemcpyHostToDevice, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(x->own_stereo[1].p, tars1, stack, cudaMemcpyHostToDevice, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(x->own_stereo[2].p, tars2, stack, cudaMemcpyHostToDevice, x->stream));
+		stereo_series_set(x, x->own_stereo[0].as<float>(), x->own_stereo[1].as<float>(), x->own_stereo[2].as<float>(), n_frames, width, height);
+		return OCB_OK;
+	}();
+	return relay_error(ctx, x, rc);
+}
+
+// The cameras, checked on the caller's context as ocb_stereo_reconstruct checks them
+static int stereo_series_cams(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2) {
+	int rc = calib_check(ctx, calib1, "stereo_series");
+	if (!rc) rc = calib_check(ctx, calib2, "stereo_series");
+	if (rc) return rc;
+	if (!intrinsics1 || !projection1 || !intrinsics2 || !projection2) return set_error(ctx, OCB_ERR_ARG, "stereo_series: bad arguments");
+	return OCB_OK;
+}
+
+// Everything else, on the context x that holds the series, before any work: pointers, orders, the series, sizes and the radii
+// (both IC-GN plans, so that a radius one order rejects stops the call before the other view runs).
+static int stereo_series_check(ocb_ctx* x, bool pointers_ok, int order1, int order2, size_t n, int rx, int ry) {
+	if (!pointers_ok || rx < 1 || ry < 1) return set_error(x, OCB_ERR_ARG, "stereo_series: bad arguments");
+	if ((order1 != 1 && order1 != 2) || (order2 != 1 && order2 != 2)) return set_error(x, OCB_ERR_ARG, "stereo_series: order must be 1 or 2");
+	if (!x->stereo1.ref) return set_error(x, OCB_ERR_STATE, "stereo_series: no stereo series set");
+	if (n == 0) return OCB_OK;
+	const size_t rec = (2 * OCB_POI2D_FLOATS + OCB_POI2DS_FLOATS) * sizeof(float); // per frame and POI; the host call stages 3 n records more
+	if (n > 0x7fffffffull || (size_t)x->stereo_frames + 1 > SIZE_MAX / (n * rec)) return set_error(x, OCB_ERR_ARG, "stereo_series: too many POIs in one call");
+	const char* e = getenv("OCB_ICGN2D_WPP"); // as icgn2d_series_launch plans
+	for (const int order : { order1, order2 }) {
+		ocb::Icgn2dPlan plan;
+		if (!ocb::icgn2d_plan(n, order == 1 ? 6 : 12, rx, ry, false, x->sm_count, x->smem_optin, e ? atoi(e) : 0, &plan))
+			return set_error(x, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
+	}
+	return OCB_OK;
+}
+
+// The two registrations (each one 2D series launch) and the records, on x (device current), after the checks above
+static int stereo_series_run(ocb_ctx* x, const ocb::StereoCam& c1, const ocb::StereoCam& c2, int order1, int order2, const float* d_stereo,
+	const float* d_seeds1, const float* d_seeds2, float* d_out1, float* d_out2, float* d_out2ds, size_t n, int rx, int ry, float conv, float stop) {
+	const int F = x->stereo_frames;
+	int rc;
+	if ((rc = icgn2d_series_run(x, order1 == 1 ? 6 : 12, x->stereo1, F, d_seeds1, d_out1, n, rx, ry, conv, stop, nullptr))) return rc;
+	if ((rc = icgn2d_series_run(x, order2 == 1 ? 6 : 12, x->stereo2, F, d_seeds2, d_out2, n, rx, ry, conv, stop, nullptr))) return rc;
+	ocb::stereo_poi2ds_launch(c1, c2, d_stereo, d_seeds1, d_out1, d_out2, d_out2ds, n, F, x->stream);
+	OCB_CUDA(x, cudaGetLastError());
+	x->launches++;
+	return OCB_OK;
+}
+
+int ocb_stereo_series_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, int order1, int order2, const void* d_stereo, const void* d_seeds1, const void* d_seeds2,
+	void* d_out1, void* d_out2, void* d_out2ds, size_t n, int rx, int ry, float conv, float stop) {
+	OCB_NO_GROUP(ctx, "stereo_series_dev");
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	int rc = stereo_series_cams(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2);
+	if (rc) return rc;
+	const bool ptrs = (d_stereo && d_seeds1 && d_seeds2 && d_out1 && d_out2 && d_out2ds) || n == 0;
+	if ((rc = stereo_series_check(ctx, ptrs, order1, order2, n, rx, ry)) || n == 0) return rc;
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	ocb::StereoCam s1, s2;
+	stereo_cams(calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2);
+	return stereo_series_run(ctx, s1, s2, order1, order2, (const float*)d_stereo, (const float*)d_seeds1, (const float*)d_seeds2, (float*)d_out1,
+		(float*)d_out2, (float*)d_out2ds, n, rx, ry, conv, stop);
+}
+
+int ocb_stereo_series(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
+	const float* intrinsics2, const float* projection2, int order1, int order2, const void* stereo, const void* seeds1, const void* seeds2,
+	void* out1, void* out2, void* out2ds, size_t n, int rx, int ry, float conv, float stop) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	int rc = stereo_series_cams(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2);
+	if (rc) return rc;
+	ocb_ctx* x = series_exec(ctx);
+	rc = [&]() -> int {
+		const bool ptrs = (stereo && seeds1 && seeds2 && out1 && out2 && out2ds) || n == 0;
+		int r;
+		if ((r = stereo_series_check(x, ptrs, order1, order2, n, rx, ry)) || n == 0) return r;
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t rec = OCB_POI2D_FLOATS * sizeof(float), F = (size_t)x->stereo_frames;
+		const size_t out_bytes = F * n * rec, ds_bytes = F * n * OCB_POI2DS_FLOATS * sizeof(float);
+		if ((r = grow(x, x->d_poi, 3 * n * rec + 2 * out_bytes + ds_bytes))) return r;
+		float* const d_stereo = x->d_poi.as<float>();
+		float* const d_seeds1 = d_stereo + n * OCB_POI2D_FLOATS;
+		float* const d_seeds2 = d_seeds1 + n * OCB_POI2D_FLOATS;
+		float* const d_out1 = d_seeds2 + n * OCB_POI2D_FLOATS;
+		float* const d_out2 = d_out1 + F * n * OCB_POI2D_FLOATS;
+		float* const d_out2ds = d_out2 + F * n * OCB_POI2D_FLOATS;
+		OCB_CUDA(x, cudaMemcpyAsync(d_stereo, stereo, n * rec, cudaMemcpyHostToDevice, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(d_seeds1, seeds1, n * rec, cudaMemcpyHostToDevice, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(d_seeds2, seeds2, n * rec, cudaMemcpyHostToDevice, x->stream));
+		ocb::StereoCam s1, s2;
+		stereo_cams(calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2);
+		if ((r = stereo_series_run(x, s1, s2, order1, order2, d_stereo, d_seeds1, d_seeds2, d_out1, d_out2, d_out2ds, n, rx, ry, conv, stop))) return r;
+		OCB_CUDA(x, cudaMemcpyAsync(out1, d_out1, out_bytes, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(out2, d_out2, out_bytes, cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaMemcpyAsync(out2ds, d_out2ds, ds_bytes, cudaMemcpyDeviceToHost, x->stream));
 		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
 		return OCB_OK;
 	}();

@@ -348,6 +348,10 @@ void calib_undistort_launch(const float* d_map_x, const float* d_map_y, int heig
 	size_t n, cudaStream_t stream);
 void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
 	cudaStream_t stream);
+// the POI2DS records of a stereo series (ocb_stereo_series): n_frames x n, frame-major, from the r1 -> r2 records d_stereo (n), the
+// view-1 seeds (n, for x and y) and the two registrations d_out1, d_out2 (n_frames x n POI2D each)
+void stereo_poi2ds_launch(const StereoCam& c1, const StereoCam& c2, const float* d_stereo, const float* d_seeds1, const float* d_out1,
+	const float* d_out2, float* d_out2ds, size_t n, int n_frames, cudaStream_t stream);
 
 void gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s);
 void prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s);

@@ -8,6 +8,7 @@
 //
 // Intrinsics are passed as the 13 floats of CameraIntrinsics (src/oc_calibration.h:25-35):
 //   fx fy fs cx cy k1 k2 k3 k4 k5 k6 p1 p2
+#include "../../include/opencorr_b200.h"
 #include "ocb_kernels.h"
 
 namespace ocb {
@@ -188,15 +189,12 @@ __device__ __forceinline__ void lsq43(const float (&Af)[4][3], const float (&bf)
 	out[2] = (float)x2;
 }
 
-// Stereovision::reconstruct(Point2D&, Point2D&), one thread per point pair.  NaN in either view: (0, 0, 0), points untouched
-// (:72-76).  Otherwise both points are clamped in place and undistorted (:79-80), A and b are formed in float32 (:87-112) and
-// the least-squares solution is rounded to float.
-__global__ void __launch_bounds__(256) stereo_reconstruct_kernel(StereoView v1, StereoView v2, float2* __restrict__ pts1, float2* __restrict__ pts2,
-	float* __restrict__ pts3d, long long n) {
-	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	float2 p1 = pts1[i], p2 = pts2[i];
-	float* o = pts3d + 3 * i;
+// Stereovision::reconstruct(Point2D&, Point2D&) of the pair (*pt1, *pt2) into o[0..2].  NaN in either view: (0, 0, 0), points
+// untouched (:72-76).  Otherwise both points are clamped in place and undistorted (:79-80), A and b are formed in float32
+// (:87-112) and the least-squares solution is rounded to float.  The one triangulation of stereo_reconstruct_kernel and
+// stereo_poi2ds_kernel, so that both give the same bits.
+__device__ __forceinline__ void reconstruct_pair(const StereoView& v1, const StereoView& v2, float2* pt1, float2* pt2, float* o) {
+	float2 p1 = *pt1, p2 = *pt2;
 	if (isnan(p1.x) || isnan(p1.y) || isnan(p2.x) || isnan(p2.y)) {
 		o[0] = 0.f;
 		o[1] = 0.f;
@@ -206,8 +204,8 @@ __global__ void __launch_bounds__(256) stereo_reconstruct_kernel(StereoView v1, 
 	float x1, y1, x2, y2;
 	undistort_point(v1.map_x, v1.map_y, v1.height, v1.width, v1.I, &p1.x, &p1.y, &x1, &y1);
 	undistort_point(v2.map_x, v2.map_y, v2.height, v2.width, v2.I, &p2.x, &p2.y, &x2, &y2);
-	pts1[i] = p1;
-	pts2[i] = p2;
+	*pt1 = p1;
+	*pt2 = p2;
 	const float* P = v1.P;
 	const float* Q = v2.P;
 	float A[4][3], b[4];
@@ -229,6 +227,57 @@ __global__ void __launch_bounds__(256) stereo_reconstruct_kernel(StereoView v1, 
 	o[2] = x[2];
 }
 
+// Stereovision::reconstruct(queue, queue, queue), one thread per point pair.
+__global__ void __launch_bounds__(256) stereo_reconstruct_kernel(StereoView v1, StereoView v2, float2* __restrict__ pts1, float2* __restrict__ pts2,
+	float* __restrict__ pts3d, long long n) {
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	reconstruct_pair(v1, v2, pts1 + i, pts2 + i, pts3d + 3 * i);
+}
+
+// The POI2DS record of POI i in frame f (reference examples/test_3d_dic_epipolar_sift.cpp:193-202, :233-245, :280-290,
+// :303-317), one thread per (frame, POI): x, y of the view-1 seed; r2, t1, t2 = location + (u, v) of the stereo record and of
+// both registrations, stored before the reconstruction clamps its copies; the three ZNCCs as they are (failure codes too);
+// ref_coor = reconstruct((x, y), r2), tar_coor = reconstruct(t1, t2); u, v, w = tar_coor - ref_coor; strain and subset
+// radius 0.  Records: stereo and seeds1 n POI2D, out1 / out2 n_frames x n POI2D and out2ds n_frames x n POI2DS, frame-major.
+__global__ void __launch_bounds__(256) stereo_poi2ds_kernel(StereoView v1, StereoView v2, const float* __restrict__ stereo,
+	const float* __restrict__ seeds1, const float* __restrict__ out1, const float* __restrict__ out2, float* __restrict__ out2ds, long long n,
+	long long total) {
+	const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= total) return;
+	const long long i = t % n;
+	const float* s = stereo + i * OCB_POI2D_FLOATS;
+	const float* a = out1 + t * OCB_POI2D_FLOATS;
+	const float* b = out2 + t * OCB_POI2D_FLOATS;
+	const float x = seeds1[i * OCB_POI2D_FLOATS], y = seeds1[i * OCB_POI2D_FLOATS + 1];
+	// POI2D: x 0, y 1, u 2, v 8, zncc 16
+	const float2 r2 = make_float2(__fadd_rn(s[0], s[2]), __fadd_rn(s[1], s[8]));
+	const float2 t1 = make_float2(__fadd_rn(a[0], a[2]), __fadd_rn(a[1], a[8]));
+	const float2 t2 = make_float2(__fadd_rn(b[0], b[2]), __fadd_rn(b[1], b[8]));
+	float2 c[4] = { make_float2(x, y), r2, t1, t2 };
+	float ref[3], tar[3];
+	reconstruct_pair(v1, v2, &c[0], &c[1], ref);
+	reconstruct_pair(v1, v2, &c[2], &c[3], tar);
+	float* o = out2ds + t * OCB_POI2DS_FLOATS;
+	o[0] = x;
+	o[1] = y;
+	for (int k = 0; k < 3; k++) o[2 + k] = __fsub_rn(tar[k], ref[k]);
+	o[5] = s[16];
+	o[6] = a[16];
+	o[7] = b[16];
+	o[8] = r2.x;
+	o[9] = r2.y;
+	o[10] = t1.x;
+	o[11] = t1.y;
+	o[12] = t2.x;
+	o[13] = t2.y;
+	for (int k = 0; k < 3; k++) {
+		o[14 + k] = ref[k];
+		o[17 + k] = tar[k];
+	}
+	for (int k = 20; k < OCB_POI2DS_FLOATS; k++) o[k] = 0.f;
+}
+
 static unsigned int blocks_for(long long n) { return (unsigned int)((n + 255) / 256); }
 
 void calib_map_launch(const float* intrinsics, int height, int width, float convergence, int iteration, float* d_map_x, float* d_map_y,
@@ -243,9 +292,7 @@ void calib_undistort_launch(const float* d_map_x, const float* d_map_y, int heig
 		(float2*)d_pts, (float2*)d_out, (long long)n);
 }
 
-void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
-	cudaStream_t stream) {
-	StereoView v[2];
+static void stereo_views(const StereoCam& c1, const StereoCam& c2, StereoView* v) {
 	const StereoCam* c[2] = { &c1, &c2 };
 	for (int k = 0; k < 2; k++) {
 		v[k].map_x = c[k]->map_x;
@@ -255,7 +302,21 @@ void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* 
 		v[k].I = load_intrinsics(c[k]->intrinsics);
 		for (int j = 0; j < 12; j++) v[k].P[j] = c[k]->projection[j];
 	}
+}
+
+void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
+	cudaStream_t stream) {
+	StereoView v[2];
+	stereo_views(c1, c2, v);
 	stereo_reconstruct_kernel<<<blocks_for((long long)n), 256, 0, stream>>>(v[0], v[1], (float2*)d_pts1, (float2*)d_pts2, d_pts3d, (long long)n);
+}
+
+void stereo_poi2ds_launch(const StereoCam& c1, const StereoCam& c2, const float* d_stereo, const float* d_seeds1, const float* d_out1,
+	const float* d_out2, float* d_out2ds, size_t n, int n_frames, cudaStream_t stream) {
+	StereoView v[2];
+	stereo_views(c1, c2, v);
+	const long long total = (long long)n * n_frames;
+	stereo_poi2ds_kernel<<<blocks_for(total), 256, 0, stream>>>(v[0], v[1], d_stereo, d_seeds1, d_out1, d_out2, d_out2ds, (long long)n, total);
 }
 
 } // namespace ocb

@@ -132,6 +132,128 @@ def speckle_series_3d(dim_x, dim_y, dim_z, n_frames, rho=2.0, seed=REF_SEED, dev
     return volume(0.0), np.stack([volume((f + 1) / n_frames) for f in range(n_frames)])
 
 
+def _rotation(rv):
+    """Rotation matrix of a rotation vector (angle-axis), float64."""
+    rv = np.asarray(rv, np.float64)
+    th = np.linalg.norm(rv)
+    if th == 0:
+        return np.eye(3)
+    k = rv / th
+    kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    return np.eye(3) + np.sin(th) * kx + (1 - np.cos(th)) * kx @ kx
+
+
+def _render_plane(shape, hom, to_px, centres, amps, rho, half, device=None):
+    """Gaussian speckles on a plane seen through a homography: pixel (c, r) shows material point hom @ (c, r, 1) (dehomogenised),
+    and I = sum_k a_k exp(-|m - c_k|^2 / rho^2) over the material centres c_k [K, 2] (x, y).  to_px maps material points to
+    pixels (the inverse of hom); each speckle is evaluated on the pixels within +-half of its image."""
+    if device is not None:
+        import torch
+        xp, f = torch, lambda a: torch.as_tensor(np.asarray(a, np.float64), device=device)
+    else:
+        xp, f = np, lambda a: np.asarray(a, np.float64)
+    h, w = shape
+    H, G, c, a = f(hom), f(to_px), f(centres), f(amps)
+    q = c @ G[:, :2].T + G[:, 2]
+    base = xp.floor(q[:, :2] / q[:, 2:3])
+    img = xp.zeros(h * w, dtype=base.dtype) if device is None else torch.zeros(h * w, dtype=torch.float64, device=device)
+    inv = 1.0 / (rho * rho)
+    for dy in range(-half, half + 1):
+        for dx in range(-half, half + 1):
+            px, py = base[:, 0] + dx, base[:, 1] + dy
+            ok = (px >= 0) & (px < w) & (py >= 0) & (py < h)
+            px, py, ck, ak = px[ok], py[ok], c[ok], a[ok]
+            m = px[:, None] * H[:, 0] + py[:, None] * H[:, 1] + H[:, 2]
+            d2 = (m[:, 0] / m[:, 2] - ck[:, 0]) ** 2 + (m[:, 1] / m[:, 2] - ck[:, 1]) ** 2
+            idx = py * w + px
+            if device is None:
+                np.add.at(img, idx.astype(np.int64), ak * np.exp(-d2 * inv))
+            else:
+                img.index_add_(0, idx.to(torch.int64), ak * torch.exp(-d2 * inv))
+    img = img.reshape(h, w)
+    return img.cpu().numpy() if device is not None else img
+
+
+# Stereo rig of speckle_stereo_series: two pinhole cameras (no lens distortion) 600 mm from a planar specimen, the second one
+# 120 mm to the side and turned towards the specimen's centre; 1 px is about 0.2 mm on the specimen.
+STEREO_Z0, STEREO_BASELINE, STEREO_F = 600.0, 120.0, 3000.0
+# displacement of the specimen point (X, Y, Z0) in the last frame, X and Y in mm from the specimen's centre:
+# (ex X + tx, ey Y + ty, tz + gx X) -- a stretch in the plane, a rigid translation and an out-of-plane w with a tilt
+STEREO_FIELD = dict(ex=4e-3, ey=-2.5e-3, tx=0.8, ty=-0.5, tz=3.0, gx=0.01)
+
+
+def stereo_rig(width, height):
+    """(intrinsics [2, 13], extrinsics [2, 6]) of the speckle_stereo_series cameras, in the order Calibration takes them:
+    fx fy fs cx cy k1..k6 p1 p2 and tx ty tz rx ry rz (world -> camera: R X + t)."""
+    phi = np.arctan2(STEREO_BASELINE, STEREO_Z0)
+    r2 = _rotation([0.0, phi, 0.0])
+    t2 = -r2 @ np.array([STEREO_BASELINE, 0.0, 0.0])
+    intr = np.zeros((2, 13), np.float32)
+    intr[:, 0:5] = [STEREO_F, STEREO_F, 0.0, 0.5 * width, 0.5 * height]
+    extr = np.array([[0, 0, 0, 0, 0, 0], [t2[0], t2[1], t2[2], 0.0, phi, 0.0]], np.float32)
+    return intr, extr
+
+
+def speckle_stereo_series(width, height, n_frames, points=None, rho=2.0, seed=REF_SEED, device=None, background=BACKGROUND):
+    """A stereo load series of a planar speckled specimen seen by the two cameras of stereo_rig.
+
+    Frame f moves every specimen point by (f + 1) / n_frames of STEREO_FIELD, an affine 3D displacement, so the deformed specimen
+    is still a plane.  Each pixel is rendered by intersecting its ray with that plane, mapping the hit back to material
+    coordinates and evaluating the Gaussian speckle texture (speckle radius rho px at the specimen's centre) there; images are
+    8-bit valued float32 like speckle_pair_2d's.
+
+    Returns a dict: ref1, r2 (height, width), tars1, tars2 (n_frames, height, width), intrinsics, extrinsics (stereo_rig), and
+    for points (n, 2) of the view-1 reference image: material (n, 3), the specimen point under each point; displaced
+    (n_frames, n, 3), its position in every frame; r2_true (n, 2), its projection into the view-2 reference image; t1_true,
+    t2_true (n_frames, n, 2), its projections into both views of every frame (float64)."""
+    intr, extr = stereo_rig(width, height)
+    K = np.array([[STEREO_F, 0, 0.5 * width], [0, STEREO_F, 0.5 * height], [0, 0, 1]])
+    cams = [(np.eye(3), np.zeros(3)), (_rotation(extr[1, 3:6].astype(np.float64)), extr[1, 0:3].astype(np.float64))]
+    fd = STEREO_FIELD
+
+    def plane(s):  # the specimen in a frame with load s: P(X, Y) = o + X a + Y b
+        return (np.array([s * fd["tx"], s * fd["ty"], STEREO_Z0 + s * fd["tz"]]), np.array([1 + s * fd["ex"], 0, s * fd["gx"]]),
+                np.array([0, 1 + s * fd["ey"], 0]))
+
+    def to_px(cam, s):  # material (X, Y, 1) -> homogeneous pixel
+        R, t = cams[cam]
+        o, a, b = plane(s)
+        return K @ np.stack([R @ a, R @ b, R @ o + t], 1)
+
+    pix = STEREO_Z0 / STEREO_F
+    rng = np.random.default_rng(seed)
+    hw, hh = 0.75 * width * pix + 8, 0.75 * height * pix + 8  # the specimen outgrows both views in every frame
+    n = int(0.5 * (2 * hw) * (2 * hh) / (np.pi * (rho * pix) ** 2))
+    centres = np.stack([rng.uniform(-hw, hw, n), rng.uniform(-hh, hh, n)], 1)
+    amps = rng.uniform(0.4, 1.0, n)
+    half = int(np.ceil(3.5 * rho * 1.15)) + 1
+
+    def image(cam, s):
+        G = to_px(cam, s)
+        im = _render_plane((height, width), np.linalg.inv(G), G, centres, amps, rho * pix, half, device)
+        return np.round(np.clip(background + (255.0 - background) * im, 0, 255)).astype(np.float32)
+
+    loads = [(f + 1) / n_frames for f in range(n_frames)]
+    out = dict(ref1=image(0, 0.0), r2=image(1, 0.0), tars1=np.stack([image(0, s) for s in loads]),
+               tars2=np.stack([image(1, s) for s in loads]), intrinsics=intr, extrinsics=extr)
+    if points is not None:
+        p = np.asarray(points, np.float64).reshape(-1, 2)
+        m = np.c_[p, np.ones(len(p))] @ np.linalg.inv(to_px(0, 0.0)).T
+        m = m[:, :2] / m[:, 2:3]
+
+        def proj(cam, s):
+            q = np.c_[m, np.ones(len(m))] @ to_px(cam, s).T
+            return q[:, :2] / q[:, 2:3]
+
+        def pos(s):
+            o, a, b = plane(s)
+            return o + m[:, 0:1] * a + m[:, 1:2] * b
+
+        out.update(material=pos(0.0), displaced=np.stack([pos(s) for s in loads]), r2_true=proj(1, 0.0),
+                   t1_true=np.stack([proj(0, s) for s in loads]), t2_true=np.stack([proj(1, s) for s in loads]))
+    return out
+
+
 def grid_2d(x0, y0, nx, ny, sx, sy):
     """POI grid, row-major over y then x like the reference examples (test_2d_dic_fftcc_icgn1.cpp:57-66)."""
     ys, xs = np.meshgrid(y0 + sy * np.arange(ny), x0 + sx * np.arange(nx), indexing="ij")
