@@ -426,6 +426,9 @@ __global__ void __launch_bounds__(256) fftcc3d_kernel(Image3D img, float* __rest
 		}
 		block_argmax(bv, bi, red);
 		if (threadIdx.x == 0) {
+			// a window of constant grey: the reference's surface is zero everywhere, index 0 wins and ZNCC is 0 / 0 (see
+			// fftcc3d_w32.cu; the packed transform leaves rounding noise there instead)
+			if (na == 0.f || nb == 0.f) { bv = 0.f; bi = 0; }
 			int du = bi % sx, dv = (bi / sx) % sy, dw = bi / slice;
 			if (du > rx) du -= sx;
 			if (dv > ry) dv -= sy;
@@ -460,33 +463,17 @@ int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, 
 	return *err == cudaSuccess ? 0 : -2;
 }
 
-size_t fftcc3d_smem_bytes(int rx, int ry, int rz) {
-	const size_t slice = (size_t)4 * rx * ry, rowpair = (size_t)2 * (2 * rz) * (2 * rx);
-	const size_t nbuf = slice > rowpair ? slice : rowpair;
-	return 2 * nbuf * sizeof(float2) + (size_t)(2 * rx + 2 * ry + 2 * rz) * sizeof(float2) + 64 * sizeof(float);
-}
-
-int fftcc3d_grid(int rx, int ry, int rz, int sm_count) {
-	const size_t smem = fftcc3d_smem_bytes(rx, ry, rz);
-	int per_sm = (int)((228 * 1024) / (smem + 1024));
-	if (per_sm > 2) per_sm = 2;
-	if (per_sm < 1) per_sm = 1;
-	return sm_count * per_sm;
-}
-
-int fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const FftAxis& ax, const FftAxis& ay,
-	const FftAxis& az, const float2* tw_x, const float2* tw_y, const float2* tw_z, float2* scratch, int grid,
-	cudaStream_t stream, cudaError_t* err) {
+int fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const Fftcc3dPlan& plan, const float2* tw_x,
+	const float2* tw_y, const float2* tw_z, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err) {
 	Fft3DParams fp;
-	fp.ax = ax; fp.ay = ay; fp.az = az;
+	fp.ax = plan.ax; fp.ay = plan.ay; fp.az = plan.az;
 	fp.tw_x = tw_x; fp.tw_y = tw_y; fp.tw_z = tw_z;
 	fp.scratch = scratch;
-	const size_t smem = fftcc3d_smem_bytes(rx, ry, rz);
-	*err = cudaFuncSetAttribute(fftcc3d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	*err = cudaFuncSetAttribute(fftcc3d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
 	if (*err != cudaSuccess) return -2;
 	if ((long long)grid > (long long)n) grid = (int)n;
 	if (grid < 1) grid = 1;
-	fftcc3d_kernel<<<grid, 256, smem, stream>>>(img, d_pois, (int)n, rx, ry, rz, fp);
+	fftcc3d_kernel<<<grid, 256, plan.smem, stream>>>(img, d_pois, (int)n, rx, ry, rz, fp);
 	*err = cudaGetLastError();
 	return *err == cudaSuccess ? 0 : -2;
 }

@@ -21,17 +21,14 @@
 
 namespace ocb {
 
-constexpr int F3R_THREADS = 128;
-
 template <int N>
 struct Fft3RegLayout {
 	static constexpr int G = F3R_THREADS / N; // slices per round
 	static constexpr int PITCH = N + 1;
 	static constexpr int TILE = N * PITCH;
 	static constexpr size_t SMEM = (size_t)2 * G * TILE * sizeof(float);
+	static_assert(SMEM == fftcc3d_reg_smem_bytes(N), "the launch plan sizes the shared memory with fftcc3d_reg_smem_bytes");
 };
-
-__host__ __device__ constexpr int fft3reg_min_ctas(int n) { return n <= 24 ? 4 : (n <= 48 ? 3 : 2); }
 
 __device__ __forceinline__ void f3r_argmax_merge(float& bv, int& bi, float v, int i) {
 	if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
@@ -240,6 +237,9 @@ __global__ void __launch_bounds__(F3R_THREADS, fft3reg_min_ctas(N)) fftcc3d_reg_
 			for (int i = 1; i < F3R_THREADS / 32; i++) f3r_argmax_merge(fv, fi, red[i], ((int*)red)[32 + i]);
 			float tna = 0.f, tnb = 0.f;
 			for (int i = 0; i < F3R_THREADS / 32; i++) { tna += red[64 + i]; tnb += red[96 + i]; }
+			// a window of constant grey: the reference's surface is zero everywhere, index 0 wins and ZNCC is 0 / 0 (see
+			// fftcc3d_w32.cu; the packed transform leaves rounding noise there instead)
+			if (tna == 0.f || tnb == 0.f) { fv = 0.f; fi = 0; }
 			int du = fi % N, dv = (fi / N) % N, dw = fi / NN;
 			if (du > R) du -= N;
 			if (dv > R) dv -= N;
@@ -256,52 +256,21 @@ __global__ void __launch_bounds__(F3R_THREADS, fft3reg_min_ctas(N)) fftcc3d_reg_
 }
 
 template <int N>
-static int fftcc3d_reg_grid_n(int sm_count) {
-	int per_sm = (int)((228 * 1024) / (Fft3RegLayout<N>::SMEM + 2048));
-	const int cap = fft3reg_min_ctas(N);
-	if (per_sm > cap) per_sm = cap;
-	if (per_sm < 1) per_sm = 1;
-	return sm_count * per_sm;
-}
-
-template <int N>
-static int fftcc3d_reg_launch_n(const Image3D& img, float* d_pois, size_t n, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err) {
-	typedef Fft3RegLayout<N> L;
-	*err = cudaFuncSetAttribute(fftcc3d_reg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::SMEM);
+static int fftcc3d_reg_launch_n(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
+	cudaError_t* err) {
+	*err = cudaFuncSetAttribute(fftcc3d_reg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
 	if (*err != cudaSuccess) return -2;
 	if ((long long)grid > (long long)n) grid = (int)n;
 	if (grid < 1) grid = 1;
-	fftcc3d_reg_kernel<N><<<grid, F3R_THREADS, L::SMEM, stream>>>(img, d_pois, (int)n, scratch);
+	fftcc3d_reg_kernel<N><<<grid, F3R_THREADS, plan.smem, stream>>>(img, d_pois, (int)n, scratch);
 	*err = cudaGetLastError();
 	return *err == cudaSuccess ? 0 : -2;
 }
 
-#define OCB_F3R_SIZES(X) X(8) X(10) X(12) X(16) X(18) X(20) X(24) X(30) X(36) X(40) X(48) X(50) X(54) X(60) X(64)
-
-// true when a register kernel exists for the cubic window of 2r points
-bool fftcc3d_reg_supported(int r) {
-	switch (2 * r) {
-#define X(n) case n:
-		OCB_F3R_SIZES(X)
-#undef X
-		return true;
-	default: return false;
-	}
-}
-
-// CTAs to launch (= scratch slots of 2 (2r)^3 complex each)
-int fftcc3d_reg_grid(int r, int sm_count) {
-	switch (2 * r) {
-#define X(n) case n: return fftcc3d_reg_grid_n<n>(sm_count);
-		OCB_F3R_SIZES(X)
-#undef X
-	default: return 0;
-	}
-}
-
-int fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, int r, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err) {
-	switch (2 * r) {
-#define X(n) case n: return fftcc3d_reg_launch_n<n>(img, d_pois, n_poi, scratch, grid, stream, err);
+int fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
+	cudaError_t* err) {
+	switch (plan.n) {
+#define X(n) case n: return fftcc3d_reg_launch_n<n>(img, d_pois, n_poi, plan, scratch, grid, stream, err);
 		OCB_F3R_SIZES(X)
 #undef X
 	default: *err = cudaErrorInvalidValue; return -2;

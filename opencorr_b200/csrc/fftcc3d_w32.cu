@@ -27,13 +27,10 @@
 
 namespace ocb {
 
-constexpr int F3_WARPS = 8;
-#ifndef FFTCC3D_W32_CTAS_PER_SM
-#define FFTCC3D_W32_CTAS_PER_SM 2
-#endif
 constexpr int F3_PITCH = 33;
 constexpr int F3_BOX_W = 36;              // TMA box: 32 columns + up to 3 of alignment slack
 constexpr int F3_TILE = 32 * F3_BOX_W;    // floats per tile: a TMA box (36 x 32) or a padded transpose tile (32 x 33)
+static_assert((size_t)2 * F3_WARPS * F3_TILE * sizeof(float) == FFTCC3D_W32_SMEM, "the launch plan sizes the shared memory with FFTCC3D_W32_SMEM");
 
 __device__ __forceinline__ void argmax_merge3(float& bv, int& bi, float v, int i) {
 	if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
@@ -260,6 +257,10 @@ __global__ void __launch_bounds__(F3_WARPS * 32, 2) fftcc3d_w32_kernel(Image3D i
 			for (int i = 1; i < F3_WARPS; i++) argmax_merge3(fv, fi, red[i], ((int*)red)[32 + i]);
 			float tna = 0.f, tnb = 0.f;
 			for (int i = 0; i < F3_WARPS; i++) { tna += red[64 + i]; tnb += red[96 + i]; }
+			// A window of constant grey is zero once its mean is taken off.  The reference transforms the two windows separately
+			// (src/oc_fftcc.cpp:378-379), so its surface is then zero everywhere: index 0 wins and ZNCC is 0 / 0.  The packed
+			// transform only cancels Z(k) + conj Z(-k) up to rounding, which would leave noise to pick the displacement.
+			if (tna == 0.f || tnb == 0.f) { fv = 0.f; fi = 0; }
 			int du = fi & 31, dv = (fi >> 5) & 31, dw = fi >> 10;
 			if (du > R) du -= NW;
 			if (dv > R) dv -= NW;
@@ -275,12 +276,11 @@ __global__ void __launch_bounds__(F3_WARPS * 32, 2) fftcc3d_w32_kernel(Image3D i
 	}
 }
 
-int fftcc3d_w32_grid(int sm_count) { return sm_count * FFTCC3D_W32_CTAS_PER_SM; }
-
-int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err) {
+int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
+	cudaError_t* err) {
 	if ((long long)grid > (long long)n) grid = (int)n;
 	if (grid < 1) grid = 1;
-	const size_t smem = (size_t)2 * F3_WARPS * F3_TILE * sizeof(float);
+	const size_t smem = plan.smem;
 	CUtensorMap tm_ref, tm_tar;
 	memset(&tm_ref, 0, sizeof(tm_ref));
 	memset(&tm_tar, 0, sizeof(tm_tar));

@@ -877,14 +877,8 @@ int ocb_set_images_3d(ocb_ctx* ctx, const float* ref, const float* tar, int dim_
 // ---- FFT-CC ----------------------------------------------------------------------------------
 // Which FFT-CC kernel runs: W32 is the register-FFT kernel specialised for the 32-point window (r = 16 on every axis), REG the
 // register FFT codelets for square / cubic windows of N = 2^a 3^b 5^c <= 64 points, GENERIC the shared-memory kernel for any
-// window whose prime factors are <= 31.  OCB_FFTCC2D_GENERIC / OCB_FFTCC3D_GENERIC select GENERIC for every window; the 2D
-// choice is ocb::fftcc2d_plan (ocb_kernels.h).
-enum class FftPath { W32, REG, GENERIC };
-static FftPath fftcc3d_path(int rx, int ry, int rz) {
-	if (getenv("OCB_FFTCC3D_GENERIC")) return FftPath::GENERIC;
-	if (rx == 16 && ry == 16 && rz == 16) return FftPath::W32;
-	return rx == ry && ry == rz && ocb::fftcc3d_reg_supported(rx) ? FftPath::REG : FftPath::GENERIC;
-}
+// window whose prime factors are <= 31.  OCB_FFTCC2D_GENERIC / OCB_FFTCC3D_GENERIC select GENERIC for every window; the choice
+// is ocb::fftcc2d_plan / ocb::fftcc3d_plan (ocb_kernels.h).
 
 // The kernel that takes a (2rx x 2ry) window, or OCB_ERR_UNSUPPORTED with the reason none does.
 static int fftcc2d_plan_or_error(ocb_ctx* ctx, int rx, int ry, ocb::Fftcc2dPlan* plan) {
@@ -937,54 +931,34 @@ int ocb_fftcc2d(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry) {
 
 // The kernel that takes a (2rx x 2ry x 2rz) window, with its grid and scratch per CTA, or OCB_ERR_UNSUPPORTED with the reason none
 // does (a window of < 2^31 points).
-struct Fftcc3dLaunch {
-	FftPath path;
-	ocb::FftAxis ax, ay, az;
-	int grid;
-	size_t cta_scratch; // float2 scratch elements per CTA
-};
-static int fftcc3d_plan_or_error(ocb_ctx* ctx, int rx, int ry, int rz, Fftcc3dLaunch* L) {
-	L->path = fftcc3d_path(rx, ry, rz);
-	if (L->path == FftPath::W32) {
-		L->grid = ocb::fftcc3d_w32_grid(ctx->sm_count);
-		L->cta_scratch = 32768;
-	} else if (L->path == FftPath::REG) {
-		L->grid = ocb::fftcc3d_reg_grid(rx, ctx->sm_count);
-		L->cta_scratch = (size_t)2 * 8 * rx * ry * rz; // two scratch volumes of (2r)^3 complex
-	} else {
-		if (!ocb::fft_plan_axis(2 * rx, &L->ax) || !ocb::fft_plan_axis(2 * ry, &L->ay) || !ocb::fft_plan_axis(2 * rz, &L->az))
-			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window size has a prime factor > 31");
-		if (ocb::fftcc3d_smem_bytes(rx, ry, rz) > ctx->smem_optin)
-			return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window needs %zu B of shared memory (> %zu)", ocb::fftcc3d_smem_bytes(rx, ry, rz),
-				ctx->smem_optin);
-		L->grid = ocb::fftcc3d_grid(rx, ry, rz, ctx->sm_count);
-		L->cta_scratch = (size_t)8 * rx * ry * rz;
-	}
-	return OCB_OK;
+static int fftcc3d_plan_or_error(ocb_ctx* ctx, int rx, int ry, int rz, ocb::Fftcc3dPlan* plan) {
+	if (ocb::fftcc3d_plan(rx, ry, rz, getenv("OCB_FFTCC3D_GENERIC") != nullptr, ctx->smem_optin, ctx->sm_count, plan)) return OCB_OK;
+	if (plan->reject == ocb::Fftcc3dReject::PRIME_FACTOR) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window size has a prime factor > 31");
+	return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window needs %zu B of shared memory (> %zu)", plan->smem, ctx->smem_optin);
 }
 
 // FFT-CC of the n device records q (1 <= n < 2^31) against img.ref / img.tar, on ctx's device (current) and stream, with
 // ctx->fft_scratch.  The pair calls pass their volume pair, the re-seeding series call one frame of the series.
 static int fftcc3d_run(ocb_ctx* ctx, const ocb::Image3D& img, float* q, size_t n, int rx, int ry, int rz) {
-	Fftcc3dLaunch L;
+	ocb::Fftcc3dPlan plan;
 	int rc;
-	if ((rc = fftcc3d_plan_or_error(ctx, rx, ry, rz, &L))) return rc;
+	if ((rc = fftcc3d_plan_or_error(ctx, rx, ry, rz, &plan))) return rc;
 	const float2 *twx = nullptr, *twy = nullptr, *twz = nullptr;
-	if (L.path == FftPath::GENERIC
+	if (plan.path == ocb::Fftcc3dPath::GENERIC
 		&& ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy)) || (rc = get_twiddles(ctx, 2 * rz, &twz))))
 		return rc;
-	int grid = L.grid;
+	int grid = plan.ctas;
 	if ((size_t)grid > n) grid = (int)n;
-	if ((rc = grow(ctx, ctx->fft_scratch, (size_t)grid * L.cta_scratch * sizeof(float2)))) return rc;
+	if ((rc = grow(ctx, ctx->fft_scratch, (size_t)grid * plan.cta_scratch * sizeof(float2)))) return rc;
 	float2* const scratch = ctx->fft_scratch.as<float2>();
 	cudaError_t err;
 	int failed;
-	if (L.path == FftPath::W32)
-		failed = ocb::fftcc3d_w32_launch(img, q, n, scratch, grid, ctx->stream, &err);
-	else if (L.path == FftPath::REG)
-		failed = ocb::fftcc3d_reg_launch(img, q, n, rx, scratch, grid, ctx->stream, &err);
+	if (plan.path == ocb::Fftcc3dPath::W32)
+		failed = ocb::fftcc3d_w32_launch(img, q, n, plan, scratch, grid, ctx->stream, &err);
+	else if (plan.path == ocb::Fftcc3dPath::REG)
+		failed = ocb::fftcc3d_reg_launch(img, q, n, plan, scratch, grid, ctx->stream, &err);
 	else
-		failed = ocb::fftcc3d_launch(img, q, n, rx, ry, rz, L.ax, L.ay, L.az, twx, twy, twz, scratch, grid, ctx->stream, &err);
+		failed = ocb::fftcc3d_launch(img, q, n, rx, ry, rz, plan, twx, twy, twz, scratch, grid, ctx->stream, &err);
 	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc3d launch failed: %s", cudaGetErrorString(err));
 	ctx->launches++;
 	return OCB_OK;
@@ -1108,8 +1082,8 @@ static int reseed_check(ocb_ctx* ctx, const char* what, int dim, const SeriesRes
 		return fftcc2d_plan_or_error(ctx, rs.fft_r[0], rs.fft_r[1], &plan);
 	}
 	if ((size_t)8 * rs.fft_r[0] * rs.fft_r[1] * rs.fft_r[2] > 0x7fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window too large");
-	Fftcc3dLaunch L;
-	return fftcc3d_plan_or_error(ctx, rs.fft_r[0], rs.fft_r[1], rs.fft_r[2], &L);
+	ocb::Fftcc3dPlan plan;
+	return fftcc3d_plan_or_error(ctx, rs.fft_r[0], rs.fft_r[1], rs.fft_r[2], &plan);
 }
 
 // Device workspace of a re-seeding call over n POIs and `frames` frames (ctx->reseed_ws): each POI's first lost frame, the

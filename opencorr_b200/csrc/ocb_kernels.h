@@ -253,18 +253,104 @@ int fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int sm_count
 // fftcc2d_reg.cu (square windows of 2^a 3^b 5^c <= 64 points, one thread per row, register FFT codelets)
 int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int sm_count, cudaStream_t stream,
 	cudaError_t* err);
+// FFTCC3D: which of the three kernels a window takes, and what that kernel needs
+constexpr int F3_WARPS = 8;        // fftcc3d_w32.cu: warps of the one-POI CTA
+// fftcc3d_w32.cu: resident CTAs per SM (DESIGN.md section 5).  The launch plan sizes the grid with it in ocb_api.cu, so an A/B
+// build that overrides it compiles both fftcc3d_w32.cu and ocb_api.cu with the flag.
+#ifndef FFTCC3D_W32_CTAS_PER_SM
+#define FFTCC3D_W32_CTAS_PER_SM 2
+#endif
+// fftcc3d_w32.cu: two tiles per warp, each a TMA box (36 x 32 floats) or a padded transpose tile (32 x 33)
+constexpr size_t FFTCC3D_W32_SMEM = (size_t)2 * F3_WARPS * 32 * 36 * sizeof(float);
+constexpr int F3R_THREADS = 128;   // fftcc3d_reg.cu: one thread per 1D transform, 128 / N z-slices per round
+// fftcc3d_reg.cu, window of n^3 points: two padded tiles (pitch n + 1) per slice of a round
+__host__ __device__ constexpr size_t fftcc3d_reg_smem_bytes(int n) { return (size_t)2 * (F3R_THREADS / n) * n * (n + 1) * sizeof(float); }
+// resident CTAs the register budget of fftcc3d_reg_kernel<N> is sized for
+__host__ __device__ constexpr int fft3reg_min_ctas(int n) { return n <= 24 ? 4 : (n <= 48 ? 3 : 2); }
+#define OCB_F3R_SIZES(X) X(8) X(10) X(12) X(16) X(18) X(20) X(24) X(30) X(36) X(40) X(48) X(50) X(54) X(60) X(64)
+// true when a register kernel exists for the cubic window of 2r points
+inline bool fftcc3d_reg_supported(int r) {
+	switch (2 * r) {
+#define X(n) case n:
+		OCB_F3R_SIZES(X)
+#undef X
+		return true;
+	default: return false;
+	}
+}
+// fftcc.cu: two ping-pong buffers (a slice or a (ky, -ky) row pair of z-x planes), the twiddle tables of the three axes, 64
+// floats of reduction scratch
+inline size_t fftcc3d_smem_bytes(int rx, int ry, int rz) {
+	const size_t slice = (size_t)4 * rx * ry, rowpair = (size_t)2 * (2 * rz) * (2 * rx);
+	const size_t nbuf = slice > rowpair ? slice : rowpair;
+	return 2 * nbuf * sizeof(float2) + (size_t)(2 * rx + 2 * ry + 2 * rz) * sizeof(float2) + 64 * sizeof(float);
+}
+
+// W32 is the register-FFT kernel specialised for the 32^3 window (r = 16 on every axis), REG the register FFT codelets for cubic
+// windows of N = 2^a 3^b 5^c <= 64 points, GENERIC the shared-memory Stockham kernel for any window whose prime factors are <= 31.
+// Every kernel runs one POI per CTA at a time in a persistent grid, with a scratch volume per CTA in global memory.
+enum class Fftcc3dPath { W32, REG, GENERIC };
+enum class Fftcc3dReject { NONE, PRIME_FACTOR, SHARED_MEMORY };
+struct Fftcc3dPlan {
+	Fftcc3dPath path;
+	int n;                // REG: points per axis, N = 2r
+	int slices_per_round; // REG: z-slices transformed at once, G = 128 / N
+	int idle_threads;     // REG: threads without a slice, 128 - G N
+	FftAxis ax, ay, az;   // GENERIC: the Stockham stages of the 2rx-, 2ry- and 2rz-point transforms
+	size_t smem;          // dynamic shared memory per CTA
+	int ctas;             // CTAs of a full launch (a queue of n POIs launches min(n, ctas))
+	size_t cta_scratch;   // float2 scratch elements per CTA
+	Fftcc3dReject reject; // why the plan is refused (GENERIC only)
+};
+
+// false when no kernel takes the (2rx x 2ry x 2rz) window: a prime factor above 31, or more shared memory than smem_optin (the
+// device's opt-in limit per block).  force_generic sends every window to the GENERIC kernel.  rx, ry, rz >= 1.
+inline bool fftcc3d_plan(int rx, int ry, int rz, bool force_generic, size_t smem_optin, int sm_count, Fftcc3dPlan* p) {
+	p->reject = Fftcc3dReject::NONE;
+	p->n = p->slices_per_round = p->idle_threads = 0;
+	p->ax.n = p->ay.n = p->az.n = p->ax.nstage = p->ay.nstage = p->az.nstage = 0;
+	if (!force_generic && rx == 16 && ry == 16 && rz == 16) {
+		p->path = Fftcc3dPath::W32;
+		p->smem = FFTCC3D_W32_SMEM;
+		p->ctas = sm_count * FFTCC3D_W32_CTAS_PER_SM;
+		p->cta_scratch = (size_t)32 * 32 * 32;
+		return true;
+	}
+	if (!force_generic && rx == ry && ry == rz && fftcc3d_reg_supported(rx)) {
+		const int N = 2 * rx;
+		p->path = Fftcc3dPath::REG;
+		p->n = N;
+		p->slices_per_round = F3R_THREADS / N;
+		p->idle_threads = F3R_THREADS - p->slices_per_round * N;
+		p->smem = fftcc3d_reg_smem_bytes(N);
+		int per_sm = (int)((228 * 1024) / (p->smem + 2048));
+		if (per_sm > fft3reg_min_ctas(N)) per_sm = fft3reg_min_ctas(N);
+		if (per_sm < 1) per_sm = 1;
+		p->ctas = sm_count * per_sm;
+		p->cta_scratch = (size_t)2 * N * N * N; // two scratch volumes of N^3 complex
+		return true;
+	}
+	p->path = Fftcc3dPath::GENERIC;
+	p->smem = fftcc3d_smem_bytes(rx, ry, rz);
+	int per_sm = (int)((228 * 1024) / (p->smem + 1024));
+	if (per_sm > 2) per_sm = 2;
+	if (per_sm < 1) per_sm = 1;
+	p->ctas = sm_count * per_sm;
+	p->cta_scratch = (size_t)8 * rx * ry * rz;
+	if (!fft_plan_axis(2 * rx, &p->ax) || !fft_plan_axis(2 * ry, &p->ay) || !fft_plan_axis(2 * rz, &p->az)) p->reject = Fftcc3dReject::PRIME_FACTOR;
+	else if (p->smem > smem_optin) p->reject = Fftcc3dReject::SHARED_MEMORY;
+	return p->reject == Fftcc3dReject::NONE;
+}
+
 // fftcc3d_reg.cu (cubic windows of 2^a 3^b 5^c <= 64 points, one thread per 1D transform, register FFT codelets)
-bool fftcc3d_reg_supported(int r);
-int fftcc3d_reg_grid(int r, int sm_count);
-int fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, int r, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err);
-size_t fftcc3d_smem_bytes(int rx, int ry, int rz);
-int fftcc3d_grid(int rx, int ry, int rz, int sm_count);
-int fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const FftAxis& ax, const FftAxis& ay,
-	const FftAxis& az, const float2* tw_x, const float2* tw_y, const float2* tw_z, float2* scratch, int grid, cudaStream_t stream,
+int fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
 	cudaError_t* err);
+// fftcc.cu
+int fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const Fftcc3dPlan& plan, const float2* tw_x,
+	const float2* tw_y, const float2* tw_z, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err);
 // fftcc3d_w32.cu (32^3 window, register FFTs)
-int fftcc3d_w32_grid(int sm_count);
-int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err);
+int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
+	cudaError_t* err);
 // icgn3d.cu
 constexpr int ICGN3D_MAX_WARPS = 16; // CTAs run 8 warps (two CTAs per SM) or, when only one slab-carrying CTA fits, 16
 constexpr int NP3 = 12;

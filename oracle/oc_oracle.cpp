@@ -901,6 +901,8 @@ void fftcc3d_poi(const Ctx3D& c, float* poi, int rx, int ry, int rz, const FFT<T
 	size_t size = (size_t)sx * sy * sz;
 	float px = poi[P3_X], py = poi[P3_Y], pz = poi[P3_Z];
 	float u0 = poi[P3_DEF + 0], v0 = poi[P3_DEF + 4], w0 = poi[P3_DEF + 8];
+	// a NaN position or guess is refused, as the kernels do, before it reaches an (int) conversion
+	if (is_nan(px) || is_nan(py) || is_nan(pz) || is_nan(u0) || is_nan(v0) || is_nan(w0)) return;
 	{
 		int x0 = (int)(px - rx), y0 = (int)(py - ry), z0 = (int)(pz - rz);
 		int x1 = (int)(px + sx - 1 - rx), y1 = (int)(py + sy - 1 - ry), z1 = (int)(pz + sz - 1 - rz);
@@ -959,6 +961,11 @@ void fftcc3d_poi(const Ctx3D& c, float* poi, int rx, int ry, int rz, const FFT<T
 				cc[((size_t)kz * sy + ky) * sx + kx] = cpx(A.real() * B.real() + A.imag() * B.imag(), A.real() * B.imag() - A.imag() * B.real());
 			}
 	fft3(cc, true);
+	// A window of constant grey is zero after the mean is taken off, and the reference, which transforms the two windows
+	// separately (:378-379), then gets a surface that is zero everywhere: index 0 wins and ZNCC is 0 / 0.  The packed transform
+	// above only gives Z(k) + conj Z(-k) = 0 up to rounding.
+	if (ref_norm == 0 || tar_norm == 0)
+		for (size_t i = 0; i < size; i++) cc[i] = cpx(0, 0);
 	T max_zncc = (T)-2;
 	size_t idx = 0;
 	for (size_t i = 0; i < size; i++) {
