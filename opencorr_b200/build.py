@@ -48,7 +48,7 @@ def build(force=False, verbose=False, variant=None, variant_flags=(), variant_so
     under lib/obj/ so that only stale sources are recompiled.
 
     variant: build lib/variants/<variant>.so instead (A/B experiments, selected at run time with OCB_LIB_PATH): the
-    sources named in variant_sources are compiled with variant_flags added (e.g. -DFFTCC3D_W32_CTAS_PER_SM=1), the rest is linked
+    sources named in variant_sources are compiled with variant_flags added (e.g. -DICGN3D_PAIRS=0), the rest is linked
     from the regular objects."""
     if variant is None and not force and not is_stale():
         return LIB_PATH

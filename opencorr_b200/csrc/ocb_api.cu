@@ -880,6 +880,13 @@ int ocb_set_images_3d(ocb_ctx* ctx, const float* ref, const float* tar, int dim_
 // window whose prime factors are <= 31.  OCB_FFTCC2D_GENERIC / OCB_FFTCC3D_GENERIC select GENERIC for every window; the choice
 // is ocb::fftcc2d_plan / ocb::fftcc3d_plan (ocb_kernels.h).
 
+// CTAs of a launch over n POIs (n >= 1): enough for the queue at pois_per_cta POIs per CTA, at most the plan's full launch
+static int fftcc_grid(size_t n, int pois_per_cta, int ctas) {
+	const size_t need = (n + pois_per_cta - 1) / pois_per_cta;
+	const int grid = need < (size_t)ctas ? (int)need : ctas;
+	return grid < 1 ? 1 : grid;
+}
+
 // The kernel that takes a (2rx x 2ry) window, or OCB_ERR_UNSUPPORTED with the reason none does.
 static int fftcc2d_plan_or_error(ocb_ctx* ctx, int rx, int ry, ocb::Fftcc2dPlan* plan) {
 	if (ocb::fftcc2d_plan(rx, ry, getenv("OCB_FFTCC2D_GENERIC") != nullptr, ctx->smem_optin, plan)) return OCB_OK;
@@ -896,15 +903,16 @@ static int fftcc2d_run(ocb_ctx* ctx, const ocb::Image2D& img, float* q, size_t n
 	int failed;
 	ocb::Fftcc2dPlan plan;
 	if (const int rc = fftcc2d_plan_or_error(ctx, rx, ry, &plan)) return rc;
+	const int grid = fftcc_grid(n, plan.pois_per_cta, ctx->sm_count * plan.ctas_per_sm);
 	if (plan.path == ocb::Fftcc2dPath::W32) {
-		failed = ocb::fftcc2d_w32_launch(img, q, n, ctx->sm_count, ctx->stream, &err);
+		failed = ocb::fftcc2d_w32_launch(img, q, n, grid, ctx->stream, &err);
 	} else if (plan.path == ocb::Fftcc2dPath::REG) { // one thread per row
-		failed = ocb::fftcc2d_reg_launch(img, q, n, rx, plan, ctx->sm_count, ctx->stream, &err);
+		failed = ocb::fftcc2d_reg_launch(img, q, n, rx, plan, grid, ctx->stream, &err);
 	} else {
 		const float2 *twx, *twy;
 		int rc;
 		if ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy))) return rc;
-		failed = ocb::fftcc2d_launch(img, q, n, rx, ry, plan, twx, twy, ctx->sm_count, ctx->stream, &err);
+		failed = ocb::fftcc2d_launch(img, q, n, rx, ry, plan, twx, twy, grid, ctx->stream, &err);
 	}
 	if (failed) return set_error(ctx, OCB_ERR_CUDA, "fftcc2d launch failed: %s", cudaGetErrorString(err));
 	ctx->launches++;
@@ -930,8 +938,9 @@ int ocb_fftcc2d(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry) {
 }
 
 // The kernel that takes a (2rx x 2ry x 2rz) window, with its grid and scratch per CTA, or OCB_ERR_UNSUPPORTED with the reason none
-// does (a window of < 2^31 points).
+// does.  The kernels index the window with int: it has fewer than 2^31 points.
 static int fftcc3d_plan_or_error(ocb_ctx* ctx, int rx, int ry, int rz, ocb::Fftcc3dPlan* plan) {
+	if ((size_t)8 * rx * ry * rz > 0x7fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window too large");
 	if (ocb::fftcc3d_plan(rx, ry, rz, getenv("OCB_FFTCC3D_GENERIC") != nullptr, ctx->smem_optin, ctx->sm_count, plan)) return OCB_OK;
 	if (plan->reject == ocb::Fftcc3dReject::PRIME_FACTOR) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window size has a prime factor > 31");
 	return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window needs %zu B of shared memory (> %zu)", plan->smem, ctx->smem_optin);
@@ -947,8 +956,7 @@ static int fftcc3d_run(ocb_ctx* ctx, const ocb::Image3D& img, float* q, size_t n
 	if (plan.path == ocb::Fftcc3dPath::GENERIC
 		&& ((rc = get_twiddles(ctx, 2 * rx, &twx)) || (rc = get_twiddles(ctx, 2 * ry, &twy)) || (rc = get_twiddles(ctx, 2 * rz, &twz))))
 		return rc;
-	int grid = plan.ctas;
-	if ((size_t)grid > n) grid = (int)n;
+	const int grid = fftcc_grid(n, 1, plan.ctas);
 	if ((rc = grow(ctx, ctx->fft_scratch, (size_t)grid * plan.cta_scratch * sizeof(float2)))) return rc;
 	float2* const scratch = ctx->fft_scratch.as<float2>();
 	cudaError_t err;
@@ -970,7 +978,6 @@ int ocb_fftcc3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int r
 	if (!ctx->img3.ref) return set_error(ctx, OCB_ERR_STATE, "fftcc3d: images not set");
 	if (n == 0) return OCB_OK;
 	if (n > 0x7fffffffull) return set_error(ctx, OCB_ERR_ARG, "fftcc3d: too many POIs in one call");
-	if ((size_t)8 * rx * ry * rz > 0x7fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window too large");
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
 	return fftcc3d_run(ctx, ctx->img3, (float*)d_poi3d, n, rx, ry, rz);
 }
@@ -1081,7 +1088,6 @@ static int reseed_check(ocb_ctx* ctx, const char* what, int dim, const SeriesRes
 		ocb::Fftcc2dPlan plan;
 		return fftcc2d_plan_or_error(ctx, rs.fft_r[0], rs.fft_r[1], &plan);
 	}
-	if ((size_t)8 * rs.fft_r[0] * rs.fft_r[1] * rs.fft_r[2] > 0x7fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "fftcc3d: window too large");
 	ocb::Fftcc3dPlan plan;
 	return fftcc3d_plan_or_error(ctx, rs.fft_r[0], rs.fft_r[1], rs.fft_r[2], &plan);
 }

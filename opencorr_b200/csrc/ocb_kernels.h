@@ -194,13 +194,23 @@ constexpr int FFTREG_THREADS = 128; // fftcc2d_reg.cu: one thread per window row
 __host__ __device__ constexpr size_t fftcc2d_reg_smem_bytes(int n) {
 	return ((size_t)2 * (FFTREG_THREADS / n) * n * (n + 1) + 4 * FFTREG_THREADS) * sizeof(float);
 }
-// true when a register kernel exists for the square window of 2r points
-inline bool fftcc2d_reg_supported(int r) {
+// Window sizes N (points per axis) that fftcc2d_reg.cu and fftcc3d_reg.cu instantiate (fft_codelet.cuh: N = 2^a 3^b 5^c <= 64;
+// N = 32 goes to the W32 kernels)
+#define OCB_FFT_REG_SIZES(X) X(8) X(10) X(12) X(16) X(18) X(20) X(24) X(30) X(36) X(40) X(48) X(50) X(54) X(60) X(64)
+// true when a register kernel exists for windows of 2r points per axis
+inline bool fft_reg_supported(int r) {
 	switch (2 * r) {
-	case 8: case 10: case 12: case 16: case 18: case 20: case 24: case 30: case 36: case 40: case 48: case 50: case 54: case 60: case 64: return true;
+#define X(n) case n:
+		OCB_FFT_REG_SIZES(X)
+#undef X
+		return true;
 	default: return false;
 	}
 }
+// resident CTAs the register budget of fftcc2d_reg_kernel<N> and fftcc3d_reg_kernel<N> is sized for (2 N floats of transform data
+// per thread + temporaries)
+__host__ __device__ constexpr int fft_reg_min_ctas(int n) { return n <= 24 ? 4 : (n <= 48 ? 3 : 2); }
+
 // fftcc.cu: two ping-pong windows of complex points, the twiddle tables of both axes, 64 floats of reduction scratch
 inline size_t fftcc2d_smem_bytes(int rx, int ry) {
 	const size_t M = (size_t)4 * rx * ry;
@@ -217,8 +227,15 @@ struct Fftcc2dPlan {
 	FftAxis ax, ay;       // GENERIC: the Stockham stages of the 2rx- and 2ry-point transforms
 	size_t smem;          // dynamic shared memory per CTA (W32: none, its tiles are static)
 	int pois_per_cta;     // POIs a CTA carries at a time
+	int ctas_per_sm;      // CTAs per SM of a full launch: a queue of n POIs launches min(ceil(n / pois_per_cta), SMs x ctas_per_sm)
 	Fftcc2dReject reject; // why the plan is refused (GENERIC only)
 };
+
+// resident CTAs per SM that smem bytes of shared memory per CTA allow (228 KB per SM, 1 KB of it reserved per CTA), between 1 and cap
+inline int fftcc_ctas_per_sm(size_t smem, int cap) {
+	const int k = (int)((228 * 1024) / (smem + 1024));
+	return k > cap ? cap : (k < 1 ? 1 : k);
+}
 
 // false when no kernel takes the (2rx x 2ry) window: a prime factor above 31, or more shared memory than smem_optin (the
 // device's opt-in limit per block).  force_generic sends every window to the GENERIC kernel.  rx, ry >= 1.
@@ -229,17 +246,20 @@ inline bool fftcc2d_plan(int rx, int ry, bool force_generic, size_t smem_optin, 
 	if (!force_generic && rx == 16 && ry == 16) {
 		p->path = Fftcc2dPath::W32;
 		p->pois_per_cta = FFTW32_WARPS;
+		p->ctas_per_sm = 16;
 		return true;
 	}
-	if (!force_generic && rx == ry && fftcc2d_reg_supported(rx)) {
+	if (!force_generic && rx == ry && fft_reg_supported(rx)) {
 		p->path = Fftcc2dPath::REG;
 		p->pois_per_cta = FFTREG_THREADS / (2 * rx);
 		p->smem = fftcc2d_reg_smem_bytes(2 * rx);
+		p->ctas_per_sm = fftcc_ctas_per_sm(p->smem, 8);
 		return true;
 	}
 	p->path = Fftcc2dPath::GENERIC;
 	p->pois_per_cta = 1;
 	p->smem = fftcc2d_smem_bytes(rx, ry);
+	p->ctas_per_sm = fftcc_ctas_per_sm(p->smem, 16) * 2;
 	if (!fft_plan_axis(2 * rx, &p->ax) || !fft_plan_axis(2 * ry, &p->ay)) p->reject = Fftcc2dReject::PRIME_FACTOR;
 	else if (p->smem > smem_optin) p->reject = Fftcc2dReject::SHARED_MEMORY;
 	return p->reject == Fftcc2dReject::NONE;
@@ -247,37 +267,18 @@ inline bool fftcc2d_plan(int rx, int ry, bool force_generic, size_t smem_optin, 
 
 // fftcc.cu
 int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const Fftcc2dPlan& plan, const float2* tw_x,
-	const float2* tw_y, int sm_count, cudaStream_t stream, cudaError_t* err);
+	const float2* tw_y, int grid, cudaStream_t stream, cudaError_t* err);
 // fftcc2d_w32.cu (32x32 window, one warp per POI, register FFT)
-int fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int sm_count, cudaStream_t stream, cudaError_t* err);
+int fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int grid, cudaStream_t stream, cudaError_t* err);
 // fftcc2d_reg.cu (square windows of 2^a 3^b 5^c <= 64 points, one thread per row, register FFT codelets)
-int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int sm_count, cudaStream_t stream,
-	cudaError_t* err);
+int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int grid, cudaStream_t stream, cudaError_t* err);
 // FFTCC3D: which of the three kernels a window takes, and what that kernel needs
 constexpr int F3_WARPS = 8;        // fftcc3d_w32.cu: warps of the one-POI CTA
-// fftcc3d_w32.cu: resident CTAs per SM (DESIGN.md section 5).  The launch plan sizes the grid with it in ocb_api.cu, so an A/B
-// build that overrides it compiles both fftcc3d_w32.cu and ocb_api.cu with the flag.
-#ifndef FFTCC3D_W32_CTAS_PER_SM
-#define FFTCC3D_W32_CTAS_PER_SM 2
-#endif
 // fftcc3d_w32.cu: two tiles per warp, each a TMA box (36 x 32 floats) or a padded transpose tile (32 x 33)
 constexpr size_t FFTCC3D_W32_SMEM = (size_t)2 * F3_WARPS * 32 * 36 * sizeof(float);
 constexpr int F3R_THREADS = 128;   // fftcc3d_reg.cu: one thread per 1D transform, 128 / N z-slices per round
 // fftcc3d_reg.cu, window of n^3 points: two padded tiles (pitch n + 1) per slice of a round
 __host__ __device__ constexpr size_t fftcc3d_reg_smem_bytes(int n) { return (size_t)2 * (F3R_THREADS / n) * n * (n + 1) * sizeof(float); }
-// resident CTAs the register budget of fftcc3d_reg_kernel<N> is sized for
-__host__ __device__ constexpr int fft3reg_min_ctas(int n) { return n <= 24 ? 4 : (n <= 48 ? 3 : 2); }
-#define OCB_F3R_SIZES(X) X(8) X(10) X(12) X(16) X(18) X(20) X(24) X(30) X(36) X(40) X(48) X(50) X(54) X(60) X(64)
-// true when a register kernel exists for the cubic window of 2r points
-inline bool fftcc3d_reg_supported(int r) {
-	switch (2 * r) {
-#define X(n) case n:
-		OCB_F3R_SIZES(X)
-#undef X
-		return true;
-	default: return false;
-	}
-}
 // fftcc.cu: two ping-pong buffers (a slice or a (ky, -ky) row pair of z-x planes), the twiddle tables of the three axes, 64
 // floats of reduction scratch
 inline size_t fftcc3d_smem_bytes(int rx, int ry, int rz) {
@@ -298,7 +299,7 @@ struct Fftcc3dPlan {
 	int idle_threads;     // REG: threads without a slice, 128 - G N
 	FftAxis ax, ay, az;   // GENERIC: the Stockham stages of the 2rx-, 2ry- and 2rz-point transforms
 	size_t smem;          // dynamic shared memory per CTA
-	int ctas;             // CTAs of a full launch (a queue of n POIs launches min(n, ctas))
+	int ctas;             // CTAs of a full launch (a queue of n POIs launches min(n, ctas): one POI per CTA at a time)
 	size_t cta_scratch;   // float2 scratch elements per CTA
 	Fftcc3dReject reject; // why the plan is refused (GENERIC only)
 };
@@ -312,30 +313,24 @@ inline bool fftcc3d_plan(int rx, int ry, int rz, bool force_generic, size_t smem
 	if (!force_generic && rx == 16 && ry == 16 && rz == 16) {
 		p->path = Fftcc3dPath::W32;
 		p->smem = FFTCC3D_W32_SMEM;
-		p->ctas = sm_count * FFTCC3D_W32_CTAS_PER_SM;
+		p->ctas = sm_count * 2; // two resident CTAs per SM (DESIGN.md section 5)
 		p->cta_scratch = (size_t)32 * 32 * 32;
 		return true;
 	}
-	if (!force_generic && rx == ry && ry == rz && fftcc3d_reg_supported(rx)) {
+	if (!force_generic && rx == ry && ry == rz && fft_reg_supported(rx)) {
 		const int N = 2 * rx;
 		p->path = Fftcc3dPath::REG;
 		p->n = N;
 		p->slices_per_round = F3R_THREADS / N;
 		p->idle_threads = F3R_THREADS - p->slices_per_round * N;
 		p->smem = fftcc3d_reg_smem_bytes(N);
-		int per_sm = (int)((228 * 1024) / (p->smem + 2048));
-		if (per_sm > fft3reg_min_ctas(N)) per_sm = fft3reg_min_ctas(N);
-		if (per_sm < 1) per_sm = 1;
-		p->ctas = sm_count * per_sm;
+		p->ctas = sm_count * fftcc_ctas_per_sm(p->smem + 1024, fft_reg_min_ctas(N)); // + 1 KB covering its static shared memory
 		p->cta_scratch = (size_t)2 * N * N * N; // two scratch volumes of N^3 complex
 		return true;
 	}
 	p->path = Fftcc3dPath::GENERIC;
 	p->smem = fftcc3d_smem_bytes(rx, ry, rz);
-	int per_sm = (int)((228 * 1024) / (p->smem + 1024));
-	if (per_sm > 2) per_sm = 2;
-	if (per_sm < 1) per_sm = 1;
-	p->ctas = sm_count * per_sm;
+	p->ctas = sm_count * fftcc_ctas_per_sm(p->smem, 2);
 	p->cta_scratch = (size_t)8 * rx * ry * rz;
 	if (!fft_plan_axis(2 * rx, &p->ax) || !fft_plan_axis(2 * ry, &p->ay) || !fft_plan_axis(2 * rz, &p->az)) p->reject = Fftcc3dReject::PRIME_FACTOR;
 	else if (p->smem > smem_optin) p->reject = Fftcc3dReject::SHARED_MEMORY;
