@@ -1,5 +1,6 @@
-// fft32.cuh -- 32-point complex FFTs held entirely in registers (fully unrolled radix-2, compile-time
-// twiddles), shared by the 32x32 and 32x32x32 FFT-CC kernels.
+// fft32.cuh -- 32- and 16-point complex FFTs held entirely in registers (fully unrolled radix-2, compile-time
+// twiddles), shared by the 32x32 and 32x32x32 FFT-CC kernels, and the split that inverts a 32-point spectrum whose
+// output is real as one 16-point transform.
 #pragma once
 #include "ocb_common.cuh"
 
@@ -48,12 +49,13 @@ __device__ __forceinline__ void mul_tw32(float xr, float xi, int k, float& yr, f
 	}
 }
 
-// One radix-2 stage with butterflies `HALF` apart.  HALF is a template argument so that every loop below has a
-// compile-time trip count and is unrolled completely (re/im then stay in registers instead of local memory).
-template <bool INV, int HALF>
-__device__ __forceinline__ void fft32_dif_stage(float* re, float* im) {
+// One radix-2 stage of an N-point transform (N = 16 or 32) with butterflies `HALF` apart: twiddle W_{2 HALF}^k =
+// W_32^{16 k / HALF}.  HALF is a template argument so that every loop below has a compile-time trip count and is unrolled
+// completely (re/im then stay in registers instead of local memory).
+template <int N, bool INV, int HALF>
+__device__ __forceinline__ void fft_dif_stage(float* re, float* im) {
 #pragma unroll
-	for (int base = 0; base < 32; base += 2 * HALF) {
+	for (int base = 0; base < N; base += 2 * HALF) {
 #pragma unroll
 		for (int k = 0; k < HALF; k++) {
 			const int i = base + k, j = i + HALF;
@@ -65,10 +67,10 @@ __device__ __forceinline__ void fft32_dif_stage(float* re, float* im) {
 	}
 }
 
-template <bool INV, int HALF>
-__device__ __forceinline__ void fft32_dit_stage(float* re, float* im) {
+template <int N, bool INV, int HALF>
+__device__ __forceinline__ void fft_dit_stage(float* re, float* im) {
 #pragma unroll
-	for (int base = 0; base < 32; base += 2 * HALF) {
+	for (int base = 0; base < N; base += 2 * HALF) {
 #pragma unroll
 		for (int k = 0; k < HALF; k++) {
 			const int i = base + k, j = i + HALF;
@@ -86,21 +88,65 @@ __device__ __forceinline__ void fft32_dit_stage(float* re, float* im) {
 // radix-2 decimation in frequency: natural order in, bit-reversed order out
 template <bool INV>
 __device__ __forceinline__ void fft32_dif(float* re, float* im) {
-	fft32_dif_stage<INV, 16>(re, im);
-	fft32_dif_stage<INV, 8>(re, im);
-	fft32_dif_stage<INV, 4>(re, im);
-	fft32_dif_stage<INV, 2>(re, im);
-	fft32_dif_stage<INV, 1>(re, im);
+	fft_dif_stage<32, INV, 16>(re, im);
+	fft_dif_stage<32, INV, 8>(re, im);
+	fft_dif_stage<32, INV, 4>(re, im);
+	fft_dif_stage<32, INV, 2>(re, im);
+	fft_dif_stage<32, INV, 1>(re, im);
 }
 
 // radix-2 decimation in time: bit-reversed order in, natural order out
 template <bool INV>
 __device__ __forceinline__ void fft32_dit(float* re, float* im) {
-	fft32_dit_stage<INV, 1>(re, im);
-	fft32_dit_stage<INV, 2>(re, im);
-	fft32_dit_stage<INV, 4>(re, im);
-	fft32_dit_stage<INV, 8>(re, im);
-	fft32_dit_stage<INV, 16>(re, im);
+	fft_dit_stage<32, INV, 1>(re, im);
+	fft_dit_stage<32, INV, 2>(re, im);
+	fft_dit_stage<32, INV, 4>(re, im);
+	fft_dit_stage<32, INV, 8>(re, im);
+	fft_dit_stage<32, INV, 16>(re, im);
+}
+
+// 16 points in re[0..15], im[0..15]; natural order in, bit-reversed order out (register j holds bin brev5(2 j) = brev4(j))
+template <bool INV>
+__device__ __forceinline__ void fft16_dif(float* re, float* im) {
+	fft_dif_stage<16, INV, 8>(re, im);
+	fft_dif_stage<16, INV, 4>(re, im);
+	fft_dif_stage<16, INV, 2>(re, im);
+	fft_dif_stage<16, INV, 1>(re, im);
+}
+
+// 16 points in re[0..15], im[0..15]; bit-reversed order in, natural order out
+template <bool INV>
+__device__ __forceinline__ void fft16_dit(float* re, float* im) {
+	fft_dit_stage<16, INV, 1>(re, im);
+	fft_dit_stage<16, INV, 2>(re, im);
+	fft_dit_stage<16, INV, 4>(re, im);
+	fft_dit_stage<16, INV, 8>(re, im);
+}
+
+// Inverse 32-point transform of a spectrum C whose output c(x) is known to be real (bit-reversed order in: register i holds
+// C(brev5(i))), first half.  Splitting the output into even and odd x, c(2n) = IDFT16(E)(n) and c(2n+1) = IDFT16(O)(n) with
+//   E(k) = C(k) + C(k + 16),  O(k) = W^k (C(k) - C(k + 16)),  W = exp(+2 pi i / 32),
+// and since both are real, one 16-point inverse of Z = E + i O gives z(n) = c(2n) + i c(2n+1).  The pair (k, k + 16) sits in
+// registers (2j, 2j+1) with k = brev4(j); Z(k) is left in register j, bit-reversed order out: fft16_dit<true> finishes the
+// transform in natural order.  Linear in C, so the same split applies to each row of a 2D spectrum whose 2D inverse is real.
+__device__ __forceinline__ void ifft32_real_split(float* re, float* im) {
+#pragma unroll
+	for (int j = 0; j < 16; j++) {
+		const int k = brev5(2 * j);
+		const float ar = re[2 * j], ai = im[2 * j], br = re[2 * j + 1], bi = im[2 * j + 1];
+		if (k == 0) { // i O = i D
+			re[j] = (ar + br) - (ai - bi);
+			im[j] = (ai + bi) + (ar - br);
+		} else if (k == 8) { // i O = i i D = -D: Z = E - D = 2 C(24)
+			re[j] = br + br;
+			im[j] = bi + bi;
+		} else { // i W^k D = (-dr s - di c) + i (dr c - di s)
+			const float er = ar + br, ei = ai + bi, dr = ar - br, di = ai - bi;
+			const float c = tw32_cos(k), s = tw32_sin(k);
+			re[j] = fmaf(-dr, s, fmaf(-di, c, er));
+			im[j] = fmaf(dr, c, fmaf(-di, s, ei));
+		}
+	}
 }
 
 } // namespace ocb

@@ -38,6 +38,16 @@ __device__ __forceinline__ void cross_spectrum(float& re, float& im, float nr, f
 	re = Ar * Br + Ai * Bi;
 	im = Ar * Bi - Ai * Br;
 }
+// 4 C(k), the same operations without the four halvings: every value is exactly 4 times cross_spectrum's (scaling by a power
+// of two commutes with rounding), and so is every value of a transform of it.  A kernel that uses it scans the surface from
+// -8 and hands a quarter of the peak to the result, and so returns cross_spectrum's records bit for bit.
+__device__ __forceinline__ void cross_spectrum4(float& re, float& im, float nr, float ni) {
+	const float Ar = re + nr, Ai = im - ni;
+	const float dr = re - nr, di = im + ni;
+	const float Br = di, Bi = -dr;
+	re = Ar * Br + Ai * Bi;
+	im = Ar * Bi - Ai * Br;
+}
 
 // First-maximum argmax: the reference scans the surface in linear order from -2.f with a strict '>' (src/oc_fftcc.cpp:246-255),
 // so of equal values the lowest index wins.  Partial results merge in any order.
