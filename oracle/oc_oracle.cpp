@@ -1239,25 +1239,41 @@ void lsq_qr(std::vector<T>& a, std::vector<T>& b, int m, T x[NB][C]) {
 	}
 }
 
+// only < 0: Strain::compute(queue), every POI whose ZNCC passes the threshold.  only >= 0: Strain::compute(POI*, queue)
+// (:158-237, :373-474) on POI `only` alone, whatever its own ZNCC.  POIs with a non-finite position are neither fitted
+// nor anyone's neighbour (a kd-tree cannot place them).
 template <class T, int MODE>
-void run_strain(float* pois, long n, float radius, int k_min, float zncc_threshold, int approximation, int threads) {
+void run_strain(float* pois, long n, float radius, int k_min, float zncc_threshold, int approximation, int threads, long only = -1) {
 	typedef StrainLayout<MODE> L;
 	constexpr int NF = L::NF, D = L::SD, FD = L::FD, NE = FD == 2 ? 3 : 6; // D: search dimensions
+	auto finite = [&](const float* p) { for (int d = 0; d < D; d++) if (!std::isfinite(p[d])) return false; return true; };
 	// uniform grid over the POI positions, cell edge = radius
 	float lo[3] = { 0, 0, 0 }, hi[3] = { 0, 0, 0 };
 	for (int d = 0; d < D; d++) { lo[d] = 1e30f; hi[d] = -1e30f; }
 	for (long i = 0; i < n; i++)
-		for (int d = 0; d < D; d++) { lo[d] = std::min(lo[d], pois[i * NF + d]); hi[d] = std::max(hi[d], pois[i * NF + d]); }
+		if (finite(pois + i * NF))
+			for (int d = 0; d < D; d++) { lo[d] = std::min(lo[d], pois[i * NF + d]); hi[d] = std::max(hi[d], pois[i * NF + d]); }
+	if (lo[0] > hi[0]) return; // no POI with a finite position
 	const float cell = radius > 0 ? radius : 1.f;
 	long nc[3] = { 1, 1, 1 };
 	for (int d = 0; d < D; d++) nc[d] = (long)std::floor((hi[d] - lo[d]) / cell) + 1;
 	auto cell_of = [&](const float* p, long* c) { for (int d = 0; d < 3; d++) c[d] = d < D ? (long)std::floor((p[d] - lo[d]) / cell) : 0; };
 	std::vector<long> start((size_t)(nc[0] * nc[1] * nc[2]) + 1, 0), order(n);
-	for (long i = 0; i < n; i++) { long c[3]; cell_of(pois + i * NF, c); start[(c[2] * nc[1] + c[1]) * nc[0] + c[0] + 1]++; }
+	for (long i = 0; i < n; i++) {
+		if (!finite(pois + i * NF)) continue;
+		long c[3];
+		cell_of(pois + i * NF, c);
+		start[(c[2] * nc[1] + c[1]) * nc[0] + c[0] + 1]++;
+	}
 	for (size_t k = 1; k < start.size(); k++) start[k] += start[k - 1];
 	{
 		std::vector<long> fill(start.begin(), start.end() - 1);
-		for (long i = 0; i < n; i++) { long c[3]; cell_of(pois + i * NF, c); order[fill[(c[2] * nc[1] + c[1]) * nc[0] + c[0]]++] = i; }
+		for (long i = 0; i < n; i++) {
+			if (!finite(pois + i * NF)) continue;
+			long c[3];
+			cell_of(pois + i * NF, c);
+			order[fill[(c[2] * nc[1] + c[1]) * nc[0] + c[0]]++] = i;
+		}
 	}
 	std::vector<float> out((size_t)n * NE);
 	std::vector<char> done(n, 0);
@@ -1270,7 +1286,10 @@ void run_strain(float* pois, long n, float radius, int k_min, float zncc_thresho
 #pragma omp for schedule(dynamic, 64)
 		for (long i = 0; i < n; i++) {
 			const float* p = pois + i * NF;
-			if (!strain_good<MODE>(p, zncc_threshold)) continue; // :244-248 / :362-368
+			if (!finite(p)) continue;
+			if (only >= 0) {
+				if (i != only) continue;
+			} else if (!strain_good<MODE>(p, zncc_threshold)) continue; // :244-248 / :362-368
 			long c[3];
 			cell_of(p, c);
 			fit.clear();
@@ -1295,11 +1314,12 @@ void run_strain(float* pois, long n, float radius, int k_min, float zncc_thresho
 				cand.clear();
 				for (long j = 0; j < n; j++) {
 					const float* q = pois + j * NF;
+					if (!finite(q)) continue;
 					float d2 = 0.f;
 					for (int d = 0; d < D; d++) { float df = p[d] - q[d]; d2 += df * df; }
 					cand.push_back(std::make_pair(d2, j));
 				}
-				long k = std::min((long)k_min, n);
+				long k = std::min((long)k_min, (long)cand.size());
 				std::partial_sort(cand.begin(), cand.begin() + k, cand.end());
 				for (long t = 0; t < k; t++)
 					if (strain_good<MODE>(pois + cand[t].second * NF, zncc_threshold)) fit.push_back(cand[t].second);
@@ -1565,21 +1585,27 @@ int oco_epipolar_search(void* h, float* pois, long n, const float* fundamental, 
 	return 0;
 }
 // Strain::prepare + Strain::compute(queue) on POI2D (dim 2) / POI3D (dim 3) records, src/oc_strain.cpp:100-111,239-250,476-487.
-// approximation: 1 Cauchy, 2 Green (setApproximation); zncc_threshold default 0.9 (:38).
-int oco_strain(float* pois, long n, int dim, float radius, int min_neighbors, float zncc_threshold, int approximation, int threads, int exact) {
+// approximation: 1 Cauchy, 2 Green (setApproximation); zncc_threshold default 0.9 (:38).  only >= 0: Strain::compute(POI*, queue)
+// on that POI alone (-1 when only >= n).
+int oco_strain_single(float* pois, long n, int dim, long only, float radius, int min_neighbors, float zncc_threshold, int approximation, int threads,
+	int exact) {
 	if (dim != 2 && dim != 3 && dim != 23) return -1; // 23: POI2DS records (28 floats), the stereo-DIC variant
+	if (only >= n) return -1;
 	if (threads < 1) threads = 1;
 	if (dim == 2) {
-		if (exact) run_strain<double, 2>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads);
-		else run_strain<float, 2>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads);
+		if (exact) run_strain<double, 2>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads, only);
+		else run_strain<float, 2>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads, only);
 	} else if (dim == 3) {
-		if (exact) run_strain<double, 3>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads);
-		else run_strain<float, 3>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads);
+		if (exact) run_strain<double, 3>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads, only);
+		else run_strain<float, 3>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads, only);
 	} else {
-		if (exact) run_strain<double, 23>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads);
-		else run_strain<float, 23>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads);
+		if (exact) run_strain<double, 23>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads, only);
+		else run_strain<float, 23>(pois, n, radius, min_neighbors, zncc_threshold, approximation, threads, only);
 	}
 	return 0;
+}
+int oco_strain(float* pois, long n, int dim, float radius, int min_neighbors, float zncc_threshold, int approximation, int threads, int exact) {
+	return oco_strain_single(pois, n, dim, -1, radius, min_neighbors, zncc_threshold, approximation, threads, exact);
 }
 void oco_set_legacy_no_minus4(int on) { g_legacy_no_m4 = on != 0; }
 int oco_max_threads(void) { return omp_get_num_procs(); }

@@ -72,6 +72,9 @@ def lib():
         L.oco_strain.restype = ctypes.c_int
         L.oco_strain.argtypes = [_f32p, ctypes.c_long, ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_float,
                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
+        L.oco_strain_single.restype = ctypes.c_int
+        L.oco_strain_single.argtypes = [_f32p, ctypes.c_long, ctypes.c_int, ctypes.c_long, ctypes.c_float, ctypes.c_int,
+                                        ctypes.c_float, ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.oco_max_threads.restype = ctypes.c_int
         _lib = L
     return _lib
@@ -94,13 +97,16 @@ def max_threads():
     return int(lib().oco_max_threads())
 
 
-def strain(pois, radius, min_neighbors, zncc_threshold=0.9, approximation=1, threads=0, exact=False):
+def strain(pois, radius, min_neighbors, zncc_threshold=0.9, approximation=1, threads=0, exact=False, only=None):
     """Strain::prepare + Strain::compute(queue) (reference src/oc_strain.cpp) on a POI2D [n,25] / POI3D [n,31] /
-    POI2DS [n,28] array."""
+    POI2DS [n,28] array.  only=i: Strain::compute(&pois[i], queue) instead, POI i alone whatever its own ZNCC."""
     assert pois.dtype == np.float32 and pois.flags.c_contiguous and pois.shape[1] in (25, 31, 28)
     dim = {25: 2, 31: 3, 28: 23}[pois.shape[1]]  # 28 floats: POI2DS records (stereo DIC)
     threads = threads if threads > 0 else max(1, max_threads() - 1)
-    rc = lib().oco_strain(_p(pois), pois.shape[0], dim, radius, min_neighbors, zncc_threshold, approximation, threads, int(exact))
+    if only is not None:
+        assert 0 <= only < pois.shape[0]
+    rc = lib().oco_strain_single(_p(pois), pois.shape[0], dim, -1 if only is None else int(only), radius, min_neighbors, zncc_threshold,
+                                 approximation, threads, int(exact))
     assert rc == 0
     return pois
 
