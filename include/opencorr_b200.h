@@ -103,7 +103,8 @@ int ocb_sync(ocb_ctx* ctx);
 long long ocb_launch_count(const ocb_ctx* ctx);
 
 /* ---- images: DIC::setImages / DVC::setImages (src/oc_dic.cpp:22-26,44-48) ----------------- */
-/* Host buffers; copied to the device (H2D on the context's stream). */
+/* Host buffers; copied to the device (H2D on the context's stream).  A call refused by its argument checks changes nothing; one
+ * that fails later (OCB_ERR_CUDA) leaves no images on the device where it failed, never a view of freed memory. */
 int ocb_set_images_2d(ocb_ctx* ctx, const float* ref, const float* tar, int width, int height, int col_major);
 int ocb_set_images_3d(ocb_ctx* ctx, const float* ref, const float* tar, int dim_x, int dim_y, int dim_z);
 /* 8-bit host images (what cv::imread(..., IMREAD_GRAYSCALE) hands the reference before cv2eigen turns
@@ -160,6 +161,7 @@ int ocb_icgn2d_ex_dev(ocb_ctx* ctx, int order, void* d_poi2d, size_t n, int rx, 
  *      reference subset of each POI (gradients, Hessian) is built once for the whole series.
  * The series is context state of its own: the pair calls (ocb_set_images_2d*, ocb_icgn2d*) neither see nor disturb it.
  * tars: n_frames row-major images, frame-major.  On a group context the first member holds the series and runs the calls.
+ * A setter refused by its argument checks changes nothing; one that fails later (OCB_ERR_CUDA) leaves no series set.
  * order = 1 (ICGN2D1) or 2 (ICGN2D2).  seeds: n POI2D records; out: n_frames x n POI2D records, frame-major (out[f n + i]),
  *   not overlapping seeds.  A long series runs in chunks: the last frame's slice of out seeds the next chunk.
  * The host variants copy (ocb_icgn2d_series blocks until out is filled); the _dev variants take BORROWED device pointers and
@@ -179,6 +181,7 @@ int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_
  * The series is context state of its own: the pair calls (ocb_set_images_3d*, ocb_icgn3d_prepare, ocb_icgn3d1*) neither see
  *   nor disturb it.  tars: n_frames [z][y][x] volumes, frame-major.  On a group context the first member holds the series and
  *   runs the calls.  ocb_set_series_3d_u8 keeps the stack as bytes on the device (1 B per voxel and frame).
+ * A setter refused by its argument checks changes nothing; one that fails later (OCB_ERR_CUDA) leaves no series set.
  * seeds: n POI3D records; out: n_frames x n POI3D records, frame-major (out[f n + i]), not overlapping seeds.  A long series
  *   runs in chunks: the last frame's slice of out seeds the next chunk.
  * Device footprint beyond the stack: about 28 B per voxel (reference, packed gradients, coefficients, scratch) and 420 B per
@@ -305,6 +308,7 @@ int ocb_stereo_reconstruct_dev(ocb_ctx* ctx, const ocb_calib* calib1, const floa
  *   not part of it: the r1 -> r2 match is an input (from the pair calls: ocb_set_images_2d(r1, r2), ocb_icgn2d_prepare,
  *   ocb_epipolar_search2d, ocb_icgn2d2).  The state is the context's own: the pair calls and ocb_set_series_2d* neither see nor
  *   change it, and it changes neither.  On a group context the first member holds it and runs the calls.
+ * A setter refused by its argument checks changes nothing; one that fails later (OCB_ERR_CUDA) leaves no stereo series set.
  * Inputs: stereo, n POI2D records of the r1 -> r2 match; seeds1 / seeds2, n POI2D frame-0 guesses of view 1 / view 2; order1,
  *   order2 = 1 (ICGN2D1) or 2 (ICGN2D2); rx, ry, conv, stop shared by both views; the cameras as ocb_stereo_reconstruct takes them.
  * For every frame f:
@@ -318,8 +322,8 @@ int ocb_stereo_reconstruct_dev(ocb_ctx* ctx, const ocb_calib* calib1, const floa
  * out1, out2: n_frames x n POI2D records, out2ds: n_frames x n POI2DS records, frame-major, overlapping no input.  A long series
  *   runs in chunks: the last frame's slices of out1 and out2 seed the next chunk.
  * The host variants copy (ocb_stereo_series blocks until the outputs are filled); the _dev variants take BORROWED device images,
- *   records and outputs (the camera arrays stay host pointers) and only enqueue.  Errors are detected before any work and write
- *   nothing to any output: OCB_ERR_STATE without a stereo series, OCB_ERR_ARG for a bad order, NULL pointers, sizes or a calibration
+ *   records and outputs (the camera arrays stay host pointers) and only enqueue.  Errors are detected before any kernel runs and
+ *   write nothing to any output: OCB_ERR_STATE without a stereo series, OCB_ERR_ARG for a bad order, NULL pointers, sizes or a calibration
  *   handle of another context, OCB_ERR_UNSUPPORTED for radii the pair calls reject. */
 int ocb_set_stereo_series_2d(ocb_ctx* ctx, const float* ref1, const float* tars1, const float* tars2, int n_frames, int width, int height);
 int ocb_set_stereo_series_2d_dev(ocb_ctx* ctx, const float* d_ref1, const float* d_tars1, const float* d_tars2, int n_frames, int width, int height);

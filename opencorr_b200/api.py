@@ -93,6 +93,7 @@ class Engine:
         if not self._ctx:
             raise _capi.OpenCorrB200Error(_capi.OCB_ERR_CUDA, _capi.last_error(None))
         self._keep = []  # host arrays referenced by the last upload
+        self._frames = {}  # frame count of each series set on this context: "2d", "3d", "stereo"
         self.image_token = 0  # bumped by every set_images_*: lets an operator see that another one replaced its images
 
     @property
@@ -211,21 +212,21 @@ class Engine:
         f, h, w = tars.shape
         self._ck(self._lib.ocb_set_series_2d(self._ctx, _vp(ref), _vp(tars), f, w, h))
         self._ck(self._lib.ocb_sync(self._ctx))
-        self._n_frames = f
+        self._frames["2d"] = f
 
     def icgn2d_series(self, order, seeds, rx, ry, conv, stop):
         """ICGN2D1 (order 1) / ICGN2D2 (order 2) over the series set by set_series_2d, frame f seeded by frame f - 1's records
         (frame 0 by `seeds`, [n, 25]).  Returns the records of every frame, float32 (F, n, 25); seeds are not changed."""
         _check_queue(seeds, POI2D_FLOATS)
-        n_frames = self._series_frames()
-        out = np.empty((n_frames, seeds.shape[0], POI2D_FLOATS), np.float32)
+        out = np.empty((self._series_frames("2d", "icgn2d_series"), seeds.shape[0], POI2D_FLOATS), np.float32)
         self._ck(self._lib.ocb_icgn2d_series(self._ctx, int(order), _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop))
         return out
 
-    def _series_frames(self):
-        if getattr(self, "_n_frames", None) is None:
-            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn2d_series: no series set")
-        return self._n_frames
+    def _series_frames(self, kind, call):
+        """The frame count of the series of this kind; without one, the error the C call would return."""
+        if kind not in self._frames:
+            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, call + ": no series set")
+        return self._frames[kind]
 
     def set_series_3d(self, ref, tars):
         """A volume series for icgn3d_series: ref (Z, Y, X) and tars (F, Z, Y, X).  uint8 volumes stay 8-bit on the device (one
@@ -242,15 +243,13 @@ class Engine:
             tars = np.ascontiguousarray(tars, dtype=np.float32)
             self._ck(self._lib.ocb_set_series_3d(self._ctx, _vp(ref), _vp(tars), f, dx, dy, dz))
         self._ck(self._lib.ocb_sync(self._ctx))
-        self._n_frames_3d = f
+        self._frames["3d"] = f
 
     def icgn3d_series(self, seeds, rx, ry, rz, conv, stop):
         """ICGN3D1 over the series set by set_series_3d, frame f seeded by frame f - 1's records (frame 0 by `seeds`, [n, 31]).
         Returns the records of every frame, float32 (F, n, 31); seeds are not changed."""
         _check_queue(seeds, POI3D_FLOATS)
-        if getattr(self, "_n_frames_3d", None) is None:
-            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn3d_series: no series set")
-        out = np.empty((self._n_frames_3d, seeds.shape[0], POI3D_FLOATS), np.float32)
+        out = np.empty((self._series_frames("3d", "icgn3d_series"), seeds.shape[0], POI3D_FLOATS), np.float32)
         self._ck(self._lib.ocb_icgn3d_series(self._ctx, _vp(seeds), _vp(out), seeds.shape[0], rx, ry, rz, conv, stop))
         return out
 
@@ -259,7 +258,7 @@ class Engine:
         its latest good translation and registered again in frame f by FFTCC2D (radii fft_rx, fft_ry) and IC-GN.  Returns
         (records float32 (F, n, 25), reseeded int64 (F,): the POIs re-seeded in each frame)."""
         _check_queue(seeds, POI2D_FLOATS)
-        n_frames = self._series_frames()
+        n_frames = self._series_frames("2d", "icgn2d_series_reseed")
         out = np.empty((n_frames, seeds.shape[0], POI2D_FLOATS), np.float32)
         counts = np.zeros(n_frames, np.uint64)
         self._ck(self._lib.ocb_icgn2d_series_reseed(self._ctx, int(order), _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop, int(fft_rx),
@@ -270,10 +269,9 @@ class Engine:
         """icgn3d_series that re-seeds lost POIs with FFTCC3D (radii fft_rx, fft_ry, fft_rz) in the frame where they are lost (see
         icgn2d_series_reseed).  Returns (records float32 (F, n, 31), reseeded int64 (F,))."""
         _check_queue(seeds, POI3D_FLOATS)
-        if getattr(self, "_n_frames_3d", None) is None:
-            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn3d_series_reseed: no series set")
-        out = np.empty((self._n_frames_3d, seeds.shape[0], POI3D_FLOATS), np.float32)
-        counts = np.zeros(self._n_frames_3d, np.uint64)
+        n_frames = self._series_frames("3d", "icgn3d_series_reseed")
+        out = np.empty((n_frames, seeds.shape[0], POI3D_FLOATS), np.float32)
+        counts = np.zeros(n_frames, np.uint64)
         self._ck(self._lib.ocb_icgn3d_series_reseed(self._ctx, _vp(seeds), _vp(out), seeds.shape[0], rx, ry, rz, conv, stop, int(fft_rx), int(fft_ry),
                                                     int(fft_rz), float(zncc_min), _vp(counts)))
         return out, counts.astype(np.int64)
@@ -289,12 +287,7 @@ class Engine:
         f, h, w = tars1.shape
         self._ck(self._lib.ocb_set_stereo_series_2d(self._ctx, _vp(ref1), _vp(tars1), _vp(tars2), f, w, h))
         self._ck(self._lib.ocb_sync(self._ctx))
-        self._n_frames_stereo = f
-
-    def _stereo_frames(self):
-        if getattr(self, "_n_frames_stereo", None) is None:
-            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "stereo_series: no stereo series set")
-        return self._n_frames_stereo
+        self._frames["stereo"] = f
 
     def stereo_series(self, rig, stereo, seeds1, seeds2, order1, order2, rx, ry, conv, stop):
         """Both views of every frame of the series set by set_stereo_series, registered against reference view 1 and
@@ -310,7 +303,7 @@ class Engine:
             raise ValueError("stereo, seeds1 and seeds2 must hold the same number of POIs")
         rig._engine()
         h1, i1, p1, h2, i2, p2 = rig._cameras()
-        f = self._stereo_frames()
+        f = self._series_frames("stereo", "stereo_series")
         out1 = np.empty((f, n, POI2D_FLOATS), np.float32)
         out2 = np.empty((f, n, POI2D_FLOATS), np.float32)
         out2ds = np.empty((f, n, POI2DS_FLOATS), np.float32)
@@ -374,7 +367,7 @@ class Engine:
     def set_series_2d_dev(self, d_ref, d_tars, n_frames, width, height):
         """Device pointers: ref (height x width) and the frame-major stack of n_frames targets; borrowed, not copied."""
         self._ck(self._lib.ocb_set_series_2d_dev(self._ctx, int(d_ref), int(d_tars), n_frames, width, height))
-        self._n_frames = int(n_frames)
+        self._frames["2d"] = int(n_frames)
 
     def icgn2d_series_dev(self, order, d_seeds, d_out, n, rx, ry, conv, stop):
         """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
@@ -382,7 +375,7 @@ class Engine:
 
     def icgn2d_series_reseed_dev(self, order, d_seeds, d_out, n, rx, ry, conv, stop, fft_rx, fft_ry, zncc_min):
         """icgn2d_series_reseed on device pointers; synchronises the stream.  Returns reseeded, int64 (F,)."""
-        counts = np.zeros(self._series_frames(), np.uint64)
+        counts = np.zeros(self._series_frames("2d", "icgn2d_series_reseed"), np.uint64)
         self._ck(self._lib.ocb_icgn2d_series_reseed_dev(self._ctx, int(order), int(d_seeds), int(d_out), n, rx, ry, conv, stop, int(fft_rx), int(fft_ry),
                                                         float(zncc_min), _vp(counts)))
         return counts.astype(np.int64)
@@ -393,7 +386,7 @@ class Engine:
     def set_series_3d_dev(self, d_ref, d_tars, n_frames, dim_x, dim_y, dim_z):
         """Device pointers: the float32 reference volume and the frame-major stack of n_frames targets; borrowed, not copied."""
         self._ck(self._lib.ocb_set_series_3d_dev(self._ctx, int(d_ref), int(d_tars), n_frames, dim_x, dim_y, dim_z))
-        self._n_frames_3d = int(n_frames)
+        self._frames["3d"] = int(n_frames)
 
     def icgn3d_series_dev(self, d_seeds, d_out, n, rx, ry, rz, conv, stop):
         """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
@@ -401,9 +394,7 @@ class Engine:
 
     def icgn3d_series_reseed_dev(self, d_seeds, d_out, n, rx, ry, rz, conv, stop, fft_rx, fft_ry, fft_rz, zncc_min):
         """icgn3d_series_reseed on device pointers; synchronises the stream.  Returns reseeded, int64 (F,)."""
-        if getattr(self, "_n_frames_3d", None) is None:
-            raise _capi.OpenCorrB200Error(_capi.OCB_ERR_STATE, "icgn3d_series_reseed: no series set")
-        counts = np.zeros(self._n_frames_3d, np.uint64)
+        counts = np.zeros(self._series_frames("3d", "icgn3d_series_reseed"), np.uint64)
         self._ck(self._lib.ocb_icgn3d_series_reseed_dev(self._ctx, int(d_seeds), int(d_out), n, rx, ry, rz, conv, stop, int(fft_rx), int(fft_ry),
                                                         int(fft_rz), float(zncc_min), _vp(counts)))
         return counts.astype(np.int64)
@@ -412,7 +403,7 @@ class Engine:
         """Device pointers: reference view 1 (height x width) and the frame-major stacks of view 1 and view 2 (n_frames images
         each); borrowed, not copied."""
         self._ck(self._lib.ocb_set_stereo_series_2d_dev(self._ctx, int(d_ref1), int(d_tars1), int(d_tars2), n_frames, width, height))
-        self._n_frames_stereo = int(n_frames)
+        self._frames["stereo"] = int(n_frames)
 
     def stereo_series_dev(self, rig, d_stereo, d_seeds1, d_seeds2, d_out1, d_out2, d_out2ds, n, order1, order2, rx, ry, conv, stop):
         """stereo_series on device pointers: n records each of stereo, seeds1, seeds2 in; n_frames x n POI2D records into d_out1

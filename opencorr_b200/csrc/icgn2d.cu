@@ -1165,6 +1165,16 @@ static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rc) {
 
 size_t icgn2d_slab_bytes(int rx, int ry) { return (size_t)icgn2d_slab_floats(rx, ry, false, 1) * sizeof(float); }
 
+// icgn2d_plan with the warps per POI the environment may force
+static bool icgn2d_plan_env(size_t n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, Icgn2dPlan* p) {
+	const char* e = getenv("OCB_ICGN2D_WPP"); // tuning knob: 1 or 2 forces the warps per POI
+	return icgn2d_plan(n, np, rx, ry, lm, sm_count, smem_optin, e ? atoi(e) : 0, p);
+}
+bool icgn2d_fits(size_t n, int np, int rx, int ry, int sm_count, size_t smem_optin) {
+	Icgn2dPlan plan;
+	return icgn2d_plan_env(n, np, rx, ry, false, sm_count, smem_optin, &plan);
+}
+
 // What a launch over n POIs runs with (icgn2d_plan) and the work-queue head it uses.  A series call takes the pair call's
 // geometry for the same n, so that a frame splits its sums between warps exactly as a pair call does.  The warps per POI are
 // those of a launch over plan_n POIs (plan_n = n but for a re-seeded sub-queue); the grid never exceeds n.
@@ -1174,8 +1184,7 @@ struct Icgn2dGeometry {
 };
 static int icgn2d_geometry(size_t n, size_t plan_n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, int* d_counter,
 	cudaStream_t stream, Icgn2dGeometry* g, cudaError_t* err) {
-	const char* e = getenv("OCB_ICGN2D_WPP"); // tuning knob: 1 or 2 forces the warps per POI
-	if (!icgn2d_plan(plan_n, np, rx, ry, lm, sm_count, smem_optin, e ? atoi(e) : 0, &g->plan)) return -1;
+	if (!icgn2d_plan_env(plan_n, np, rx, ry, lm, sm_count, smem_optin, &g->plan)) return -1;
 	if ((size_t)g->plan.grid > n) g->plan.grid = n > 0 ? (int)n : 1;
 	if (g->plan.wpp != 1) {
 		*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);

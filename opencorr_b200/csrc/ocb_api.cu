@@ -11,6 +11,7 @@
 #include <atomic>
 #include <condition_variable>
 #include <functional>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -117,6 +118,20 @@ struct DevBuf {
 	template <class T> T* as() const { return (T*)p; }
 };
 
+// One series (ocb_set_series_2d*, ocb_set_series_3d*, ocb_set_stereo_series_2d*): a float reference against the frame-major
+// stacks tars[0] and (stereo) tars[1], `frames` frames of w x h x d pixels (d = 1: images) starting `pitch` bytes apart (a float
+// stack: one frame of floats; the 8-bit volume stack: the frame's bytes rounded up to 16).  The host setters upload into `own`
+// ({reference, stack 0, stack 1}), the _dev setters borrow.  No reference: no series.
+struct SeriesStore {
+	DevBuf own[3];
+	const float* ref = nullptr;
+	const void* tars[2] = { nullptr, nullptr };
+	size_t pitch = 0;
+	int frames = 0;
+	int w = 0, h = 0, d = 0;
+	ocb::Image2D view2(int k) const { return ocb::Image2D{ ref, (const float*)tars[k], w, h }; }
+};
+
 struct ocb_ctx {
 	// GROUP context: non-empty `members` (single-device contexts owned by the group); none of the per-device fields below
 	// is used.  Host-buffer entry points shard their POI queue over the members; *_dev entry points are refused.
@@ -140,15 +155,9 @@ struct ocb_ctx {
 	bool prepared2 = false;
 	bool prepared_nr2 = false;
 
-	// 2D image series (ocb_set_series_2d*): its own state, untouched by the pair calls.  series.tar is the frame-major stack.
-	DevBuf own_series[2]; // {ref, stack} uploaded from the host
-	ocb::Image2D series{ nullptr, nullptr, 0, 0 };
-	int series_frames = 0;
-	// stereo image series (ocb_set_stereo_series_2d*): its own state, untouched by the pair calls and the 2D series.  stereo1 /
-	// stereo2 share the reference view-1 image; their .tar are the frame-major stacks of view 1 and view 2.
-	DevBuf own_stereo[3]; // {ref1, view-1 stack, view-2 stack} uploaded from the host
-	ocb::Image2D stereo1{ nullptr, nullptr, 0, 0 }, stereo2{ nullptr, nullptr, 0, 0 };
-	int stereo_frames = 0;
+	// the image, volume and stereo series: each its own state, untouched by the pair calls and by the other two.  The stereo
+	// series holds reference view 1 and the stacks of view 1 and view 2.
+	SeriesStore series2d, series3d, stereo;
 
 	// 3D images + tables
 	DevBuf own3[2]; // {ref, tar} uploaded from the host
@@ -158,14 +167,8 @@ struct ocb_ctx {
 	ocb::Image3D img3{ nullptr, nullptr, nullptr, nullptr, 0, 0, 0 };
 	bool prepared3 = false;
 
-	// 3D volume series (ocb_set_series_3d*): its own state and buffers, untouched by the pair calls.  series3.ref is the
-	// reference, series3_tars the frame-major stack (floats, or bytes with frames series3_u8_pitch bytes apart).
-	DevBuf own_series3[2]; // {ref, stack} uploaded from the host
+	// the volume series' work buffers: packed gradients, coefficients, scratch volume, per-POI setup cache
 	DevBuf series3_rg, series3_coef, series3_tmp, series3_cache;
-	ocb::Image3D series3{ nullptr, nullptr, nullptr, nullptr, 0, 0, 0 };
-	const void* series3_tars = nullptr;
-	size_t series3_u8_pitch = 0; // 0: a float stack
-	int series3_frames = 0;
 	// series calls that re-seed lost POIs: lost-frame/index/histogram/anchor workspace, the rebuilt sub-queue and (2D) the
 	// sub-queue's continuation over the later frames
 	DevBuf reseed_ws, reseed_sub, reseed_cont;
@@ -230,7 +233,8 @@ static int ensure_device(ocb_ctx* ctx) {
 
 // Make b hold at least `bytes` (on ctx's device, which must be current).  It only grows, and its contents are not kept across
 // a growth.  Work already enqueued on ctx->stream may still use the old allocation, so the stream is drained before it is
-// released.  If the allocation fails, b is left empty and the next call tries again.
+// released.  If the allocation fails, b is left empty and the next call tries again; the failure is cleared from the runtime's
+// last error, which the next launch's check would otherwise report.
 static int grow(ocb_ctx* ctx, DevBuf& b, size_t bytes) {
 	if (bytes <= b.bytes) return OCB_OK;
 	if (b.p) {
@@ -239,7 +243,12 @@ static int grow(ocb_ctx* ctx, DevBuf& b, size_t bytes) {
 		b.p = nullptr;
 		b.bytes = 0;
 	}
-	OCB_CUDA(ctx, cudaMalloc(&b.p, bytes));
+	const cudaError_t e = cudaMalloc(&b.p, bytes);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		b.p = nullptr;
+		return set_error(ctx, OCB_ERR_CUDA, "cudaMalloc(&b.p, bytes) failed: %s", cudaGetErrorString(e));
+	}
 	b.bytes = bytes;
 	return OCB_OK;
 }
@@ -382,6 +391,27 @@ static int run_host_queue(ocb_ctx* ctx, const char* what, void* host, size_t n, 
 // ---- GROUP contexts: one process, several devices -------------------------------------------------------------------
 static inline bool is_group(const ocb_ctx* ctx) { return ctx && !ctx->members.empty(); }
 
+// The single-device context that holds the state of the calls a group does not shard (the series, SIFT3D, the calibration maps):
+// the group's first member, or ctx itself.
+static ocb_ctx* exec_member(ocb_ctx* ctx) { return is_group(ctx) ? ctx->members[0] : ctx; }
+
+// A failure on the executing member of a group is reported on the group as well.
+static int relay_error(ocb_ctx* ctx, const ocb_ctx* exec, int rc) {
+	if (rc != OCB_OK && ctx != exec) {
+		ctx->last_error = exec->last_error;
+		g_last_error = ctx->last_error;
+	}
+	return rc;
+}
+
+// f(x) on the executing member x of ctx, its failure relayed to ctx
+template <class F>
+static int on_exec(ocb_ctx* ctx, F f) {
+	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
+	ocb_ctx* const x = exec_member(ctx);
+	return relay_error(ctx, x, f(x));
+}
+
 // Run f(member, index) on the first `used` members concurrently (member 0 on the calling thread); first failure wins.
 // (member, on its own thread) order the member's stream after every peer's image pushes, once per upload
 static int member_settle(ocb_ctx* m) {
@@ -493,9 +523,22 @@ static ocb_ctx* create_group(const int* devices, int n) {
 	return g;
 }
 
-// Image pair buffers of a single-device context (dim 2 or 3), each grown to `elems` floats
+// Forget the image pair of dimension dim (2 or 3) and what was prepared on it, before its buffers are replaced: an upload that
+// fails leaves no images rather than a view of freed memory.
+static void clear_pair(ocb_ctx* ctx, int dim) {
+	if (dim == 2) {
+		ctx->img2 = ocb::Image2D{ nullptr, nullptr, 0, 0 };
+		ctx->bands_fresh = ctx->prepared2 = ctx->prepared_nr2 = false;
+	} else {
+		ctx->img3 = ocb::Image3D{ nullptr, nullptr, nullptr, nullptr, 0, 0, 0 };
+		ctx->prepared3 = false;
+	}
+}
+
+// Image pair buffers of a single-device context (dim 2 or 3), each grown to `elems` floats; the pair is cleared first
 static DevBuf* own_pair(ocb_ctx* ctx, int dim) { return dim == 2 ? ctx->own2 : ctx->own3; }
 static int ensure_pair(ocb_ctx* ctx, int dim, size_t elems) {
+	clear_pair(ctx, dim);
 	DevBuf* pair = own_pair(ctx, dim);
 	const int rc = grow(ctx, pair[0], elems * sizeof(float));
 	return rc ? rc : grow(ctx, pair[1], elems * sizeof(float));
@@ -508,6 +551,7 @@ static int ensure_pair(ocb_ctx* ctx, int dim, size_t elems) {
 static int group_distribute_pair(ocb_ctx* g, const float* ref, const float* tar, size_t elems, int dim) {
 	const int G = (int)g->members.size();
 	int rc = OCB_OK;
+	for (ocb_ctx* m : g->members) clear_pair(m, dim); // a failure on any member leaves the group without images
 	for (ocb_ctx* m : g->members) { // buffers first: a peer may push into them as soon as the exchange starts
 		if (ensure_device(m)) return OCB_ERR_CUDA;
 		rc = ensure_pair(m, dim, elems);
@@ -542,6 +586,107 @@ static int group_distribute_pair(ocb_ctx* g, const float* ref, const float* tar,
 	// its next job, on its own thread (member_settle)
 	for (ocb_ctx* m : g->members) m->need_peer_wait = true;
 	return OCB_OK;
+}
+
+// ---- series: the state and host staging shared by the image, volume and stereo series ---------------------------------
+// Point s at a series (the _dev setters borrow the caller's device memory): see SeriesStore; tar1 is null but for the stereo series
+static void series_borrow(SeriesStore& s, const float* ref, const void* tar0, const void* tar1, size_t pitch, int frames, int w, int h, int d) {
+	s.ref = ref;
+	s.tars[0] = tar0;
+	s.tars[1] = tar1;
+	s.pitch = pitch;
+	s.frames = frames;
+	s.w = w;
+	s.h = h;
+	s.d = d;
+}
+static void series_clear(SeriesStore& s) { series_borrow(s, nullptr, nullptr, nullptr, 0, 0, 0, 0, 0); }
+
+// The host setters' upload, on the executing member x after their argument checks: s.own grows to a reference of w x h x d floats
+// and n_stacks stacks of `frames` frames `pitch` bytes apart, the reference (unless ref is null: the caller fills own[0]) and
+// every frame (frame_bytes each) are copied in, and s points at them.  s is cleared before any buffer is replaced, so a failure
+// leaves no series, never a view of freed memory.
+static int series_upload(ocb_ctx* x, SeriesStore& s, const float* ref, const void* const* stacks, int n_stacks, size_t frame_bytes, size_t pitch,
+	int frames, int w, int h, int d) {
+	if (ensure_device(x)) return OCB_ERR_CUDA;
+	series_clear(s);
+	const size_t ref_bytes = (size_t)w * h * d * sizeof(float);
+	int rc = grow(x, s.own[0], ref_bytes);
+	for (int k = 0; k < n_stacks && rc == OCB_OK; k++) rc = grow(x, s.own[1 + k], (size_t)frames * pitch);
+	if (rc) return rc;
+	if (ref) OCB_CUDA(x, cudaMemcpyAsync(s.own[0].p, ref, ref_bytes, cudaMemcpyHostToDevice, x->stream));
+	for (int k = 0; k < n_stacks; k++) {
+		char* const dst = s.own[1 + k].as<char>();
+		const char* const src = (const char*)stacks[k];
+		if (pitch == frame_bytes)
+			OCB_CUDA(x, cudaMemcpyAsync(dst, src, (size_t)frames * pitch, cudaMemcpyHostToDevice, x->stream));
+		else
+			for (int f = 0; f < frames; f++)
+				OCB_CUDA(x, cudaMemcpyAsync(dst + (size_t)f * pitch, src + (size_t)f * frame_bytes, frame_bytes, cudaMemcpyHostToDevice, x->stream));
+	}
+	series_borrow(s, s.own[0].as<float>(), s.own[1].p, n_stacks > 1 ? s.own[2].p : nullptr, pitch, frames, w, h, d);
+	return OCB_OK;
+}
+
+// A call over n POIs is refused when the kernels could not index its POIs with int or a byte count of its frames x n records of
+// rec bytes (per POI and frame, every output together) would not fit in a size_t; a host call (`staged`) also stages its inputs,
+// at most one frame's worth.
+static int series_size_check(ocb_ctx* x, const char* what, size_t n, int frames, size_t rec, bool staged) {
+	if (n > 0x7fffffffull || (size_t)frames + (staged ? 1 : 0) > SIZE_MAX / (n * rec))
+		return set_error(x, OCB_ERR_ARG, "%s: too many POIs in one call", what);
+	return OCB_OK;
+}
+
+// A series call with host buffers, on the executing member x of ctx: the n records of in_floats floats of every input are
+// staged on the device, dev(x, d_in, d_out) runs the call's _dev body on them, the frames x n records (frame-major) of every
+// output {pointer, floats per record} come back, and the call returns after one synchronisation.  With n == 0, dev runs on null
+// pointers for its argument checks only.  A failure writes nothing to the outputs and is reported on ctx too.
+template <class F>
+static int series_host(ocb_ctx* ctx, const char* what, SeriesStore ocb_ctx::*which, size_t n, std::initializer_list<const void*> in, size_t in_floats,
+	std::initializer_list<std::pair<void*, size_t>> out, F dev) {
+	return on_exec(ctx, [&](ocb_ctx* x) -> int {
+		const float* d_in[3] = {};
+		float* d_out[3] = {};
+		size_t rec_floats = 0;
+		bool ptrs = true;
+		for (const void* h : in) ptrs = ptrs && h;
+		for (const auto& o : out) {
+			ptrs = ptrs && o.first;
+			rec_floats += o.second;
+		}
+		if (!ptrs && n) return set_error(x, OCB_ERR_ARG, "%s: bad arguments", what);
+		const SeriesStore& s = x->*which;
+		if (!s.ref) return set_error(x, OCB_ERR_STATE, "%s: no series set", what);
+		if (n == 0) return dev(x, d_in, d_out);
+		int rc;
+		if ((rc = series_size_check(x, what, n, s.frames, rec_floats * sizeof(float), true))) return rc;
+		if (ensure_device(x)) return OCB_ERR_CUDA;
+		const size_t frames = (size_t)s.frames;
+		if ((rc = grow(x, x->d_poi, (in.size() * in_floats + frames * rec_floats) * n * sizeof(float)))) return rc;
+		float* p = x->d_poi.as<float>(); // the inputs, then the outputs, back to back
+		for (size_t k = 0; k < in.size(); p += n * in_floats, k++) {
+			d_in[k] = p;
+			OCB_CUDA(x, cudaMemcpyAsync(p, in.begin()[k], n * in_floats * sizeof(float), cudaMemcpyHostToDevice, x->stream));
+		}
+		for (size_t k = 0; k < out.size(); p += frames * n * out.begin()[k].second, k++) d_out[k] = p;
+		if ((rc = dev(x, d_in, d_out))) return rc;
+		for (size_t k = 0; k < out.size(); k++)
+			OCB_CUDA(x, cudaMemcpyAsync(out.begin()[k].first, d_out[k], frames * n * out.begin()[k].second * sizeof(float), cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
+		return OCB_OK;
+	});
+}
+
+// The re-seeding entry points: call(counts) counts into a zeroed vector with one entry per frame of the series `which` of ctx's
+// executing member, and the counts go to `reseeded` only when it succeeds.  A device-pointer call (`dev`) is synchronised first.
+template <class F>
+static int series_reseed(ocb_ctx* ctx, SeriesStore ocb_ctx::*which, bool dev, size_t n, size_t* reseeded, F call) {
+	const SeriesStore* s = ctx ? &(exec_member(ctx)->*which) : nullptr;
+	std::vector<size_t> counts(s && s->ref ? s->frames : 0, 0);
+	const int rc = call(counts.data());
+	if (rc == OCB_OK && dev && n) OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	if (rc == OCB_OK && reseeded) memcpy(reseeded, counts.data(), counts.size() * sizeof(size_t));
+	return rc;
 }
 
 extern "C" {
@@ -1039,34 +1184,22 @@ int ocb_icgn2d_ex_dev(ocb_ctx* ctx, int order, void* d_poi2d, size_t n, int rx, 
 
 // ---- image series: one reference, n_frames targets, each frame seeded by the previous one ------------------------------
 // On a group context the first member holds the series and runs it.
-static int relay_error(ocb_ctx* ctx, const ocb_ctx* exec, int rc);
-static ocb_ctx* series_exec(ocb_ctx* ctx) { return is_group(ctx) ? ctx->members[0] : ctx; }
 
 int ocb_set_series_2d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars, int n_frames, int width, int height) {
 	OCB_NO_GROUP(ctx, "set_series_2d_dev");
 	if (!ctx || !d_ref || !d_tars || n_frames < 1 || width < 5 || height < 5) return set_error(ctx, OCB_ERR_ARG, "set_series_2d: bad arguments");
-	ctx->series = ocb::Image2D{ d_ref, d_tars, width, height };
-	ctx->series_frames = n_frames;
+	series_borrow(ctx->series2d, d_ref, d_tars, nullptr, (size_t)width * height * sizeof(float), n_frames, width, height, 1);
 	return OCB_OK;
 }
 
 int ocb_set_series_2d(ocb_ctx* ctx, const float* ref, const float* tars, int n_frames, int width, int height) {
-	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	ocb_ctx* x = series_exec(ctx);
-	const int rc = [&]() -> int {
+	return on_exec(ctx, [&](ocb_ctx* x) {
 		if (!ref || !tars || n_frames < 1 || width < 5 || height < 5) return set_error(x, OCB_ERR_ARG, "set_series_2d: bad arguments");
-		const size_t elems = (size_t)width * height;
-		if ((size_t)n_frames > SIZE_MAX / sizeof(float) / elems) return set_error(x, OCB_ERR_ARG, "set_series_2d: series too large");
-		if (ensure_device(x)) return OCB_ERR_CUDA;
-		int r;
-		if ((r = grow(x, x->own_series[0], elems * sizeof(float))) || (r = grow(x, x->own_series[1], (size_t)n_frames * elems * sizeof(float)))) return r;
-		OCB_CUDA(x, cudaMemcpyAsync(x->own_series[0].p, ref, elems * sizeof(float), cudaMemcpyHostToDevice, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(x->own_series[1].p, tars, (size_t)n_frames * elems * sizeof(float), cudaMemcpyHostToDevice, x->stream));
-		x->series = ocb::Image2D{ x->own_series[0].as<float>(), x->own_series[1].as<float>(), width, height };
-		x->series_frames = n_frames;
-		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+		const size_t frame = (size_t)width * height * sizeof(float);
+		if ((size_t)n_frames > SIZE_MAX / frame) return set_error(x, OCB_ERR_ARG, "set_series_2d: series too large");
+		const void* stack[1] = { tars };
+		return series_upload(x, x->series2d, ref, stack, 1, frame, frame, n_frames, width, height, 1);
+	});
 }
 
 // What a series call that re-seeds lost POIs adds to the plain series (a null SeriesReseed: the plain series).  POI i is lost in
@@ -1203,42 +1336,20 @@ static int icgn2d_series_dev(ocb_ctx* ctx, const char* what, int order, const vo
 	float stop, const SeriesReseed* rs) {
 	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
 	if (order != 1 && order != 2) return set_error(ctx, OCB_ERR_ARG, "%s: order must be 1 or 2", what);
-	if (!ctx->series.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
+	const SeriesStore& s = ctx->series2d;
+	if (!s.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
 	int rc;
 	if (rs && (rc = reseed_check(ctx, what, 2, *rs))) return rc;
 	if (n == 0) return OCB_OK;
-	if (n > 0x7fffffffull || (size_t)ctx->series_frames > SIZE_MAX / (n * OCB_POI2D_FLOATS * sizeof(float)))
-		return set_error(ctx, OCB_ERR_ARG, "%s: too many POIs in one call", what);
+	if ((rc = series_size_check(ctx, what, n, s.frames, OCB_POI2D_FLOATS * sizeof(float), false))) return rc;
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	return icgn2d_series_run(ctx, order == 1 ? 6 : 12, ctx->series, ctx->series_frames, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv, stop,
-		rs);
+	return icgn2d_series_run(ctx, order == 1 ? 6 : 12, s.view2(0), s.frames, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv, stop, rs);
 }
 
-// Host seeds and output, on the series' executing member: seeds in, the series, every frame's records out
 static int icgn2d_series_host(ocb_ctx* ctx, const char* what, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop,
 	const SeriesReseed* rs) {
-	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	ocb_ctx* x = series_exec(ctx);
-	const int rc = [&]() -> int {
-		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "%s: bad arguments", what);
-		if (!x->series.ref) return set_error(x, OCB_ERR_STATE, "%s: no series set", what);
-		if (n == 0) return icgn2d_series_dev(x, what, order, nullptr, nullptr, 0, rx, ry, conv, stop, rs); // argument checks only
-		const size_t rec = OCB_POI2D_FLOATS * sizeof(float);
-		if (n > 0x7fffffffull || (size_t)x->series_frames + 1 > SIZE_MAX / (n * rec))
-			return set_error(x, OCB_ERR_ARG, "%s: too many POIs in one call", what);
-		if (ensure_device(x)) return OCB_ERR_CUDA;
-		const size_t out_bytes = (size_t)x->series_frames * n * rec;
-		int r;
-		if ((r = grow(x, x->d_poi, n * rec + out_bytes))) return r;
-		float* const d_seeds = x->d_poi.as<float>();
-		float* const d_out = d_seeds + n * OCB_POI2D_FLOATS;
-		OCB_CUDA(x, cudaMemcpyAsync(d_seeds, seeds, n * rec, cudaMemcpyHostToDevice, x->stream));
-		if ((r = icgn2d_series_dev(x, what, order, d_seeds, d_out, n, rx, ry, conv, stop, rs))) return r;
-		OCB_CUDA(x, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, x->stream));
-		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
-		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+	return series_host(ctx, what, &ocb_ctx::series2d, n, { seeds }, OCB_POI2D_FLOATS, { { out, OCB_POI2D_FLOATS } },
+		[&](ocb_ctx* x, const float* const* d_in, float* const* d_out) { return icgn2d_series_dev(x, what, order, d_in[0], d_out[0], n, rx, ry, conv, stop, rs); });
 }
 
 int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop) {
@@ -1250,28 +1361,21 @@ int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, siz
 	return icgn2d_series_host(ctx, "icgn2d_series", order, seeds, out, n, rx, ry, conv, stop, nullptr);
 }
 
-// The re-seeding calls count into a zeroed vector and copy it to `reseeded` only when the call succeeds.
-static int series_reseed_counts(int rc, const std::vector<size_t>& counts, size_t* reseeded) {
-	if (rc == OCB_OK && reseeded) memcpy(reseeded, counts.data(), counts.size() * sizeof(size_t));
-	return rc;
-}
-
 int ocb_icgn2d_series_reseed_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
 	int fft_rx, int fft_ry, float zncc_min, size_t* reseeded) {
 	OCB_NO_GROUP(ctx, "icgn2d_series_reseed_dev");
-	std::vector<size_t> counts(ctx && ctx->series.ref ? ctx->series_frames : 0, 0);
-	SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts.data() };
-	int rc = icgn2d_series_dev(ctx, "icgn2d_series_reseed", order, d_seeds, d_out, n, rx, ry, conv, stop, &rs);
-	if (rc == OCB_OK && n) OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	return series_reseed_counts(rc, counts, reseeded);
+	return series_reseed(ctx, &ocb_ctx::series2d, true, n, reseeded, [&](size_t* counts) {
+		const SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts };
+		return icgn2d_series_dev(ctx, "icgn2d_series_reseed", order, d_seeds, d_out, n, rx, ry, conv, stop, &rs);
+	});
 }
 
 int ocb_icgn2d_series_reseed(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, int fft_rx,
 	int fft_ry, float zncc_min, size_t* reseeded) {
-	const ocb_ctx* x = ctx ? series_exec(ctx) : nullptr;
-	std::vector<size_t> counts(x && x->series.ref ? x->series_frames : 0, 0);
-	SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts.data() };
-	return series_reseed_counts(icgn2d_series_host(ctx, "icgn2d_series_reseed", order, seeds, out, n, rx, ry, conv, stop, &rs), counts, reseeded);
+	return series_reseed(ctx, &ocb_ctx::series2d, false, n, reseeded, [&](size_t* counts) {
+		const SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts };
+		return icgn2d_series_host(ctx, "icgn2d_series_reseed", order, seeds, out, n, rx, ry, conv, stop, &rs);
+	});
 }
 
 // one launch over a host queue (all POIs share the radius), optional host offsets
@@ -1546,65 +1650,46 @@ static size_t series3_elems(int n_frames, int dim_x, int dim_y, int dim_z, size_
 	return elems > SIZE_MAX / voxel / (size_t)n_frames ? 0 : elems;
 }
 
-static void series3_set(ocb_ctx* x, const float* ref, const void* tars, size_t u8_pitch, int n_frames, int dim_x, int dim_y, int dim_z) {
-	x->series3 = ocb::Image3D{ ref, nullptr, nullptr, nullptr, dim_x, dim_y, dim_z };
-	x->series3_tars = tars;
-	x->series3_u8_pitch = u8_pitch;
-	x->series3_frames = n_frames;
-}
-
 int ocb_set_series_3d_dev(ocb_ctx* ctx, const float* d_ref, const float* d_tars, int n_frames, int dim_x, int dim_y, int dim_z) {
 	OCB_NO_GROUP(ctx, "set_series_3d_dev");
-	if (!ctx || !d_ref || !d_tars || !series3_elems(n_frames, dim_x, dim_y, dim_z, sizeof(float)))
+	const size_t elems = series3_elems(n_frames, dim_x, dim_y, dim_z, sizeof(float));
+	if (!ctx || !d_ref || !d_tars || !elems)
 		return set_error(ctx, OCB_ERR_ARG, "set_series_3d: bad arguments (each dimension must be >= 15, n_frames >= 1)");
-	series3_set(ctx, d_ref, d_tars, 0, n_frames, dim_x, dim_y, dim_z);
+	series_borrow(ctx->series3d, d_ref, d_tars, nullptr, elems * sizeof(float), n_frames, dim_x, dim_y, dim_z);
 	return OCB_OK;
 }
 
 int ocb_set_series_3d(ocb_ctx* ctx, const float* ref, const float* tars, int n_frames, int dim_x, int dim_y, int dim_z) {
-	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	ocb_ctx* x = series_exec(ctx);
-	const int rc = [&]() -> int {
+	return on_exec(ctx, [&](ocb_ctx* x) {
 		const size_t elems = series3_elems(n_frames, dim_x, dim_y, dim_z, sizeof(float));
 		if (!ref || !tars || !elems) return set_error(x, OCB_ERR_ARG, "set_series_3d: bad arguments (each dimension must be >= 15, n_frames >= 1)");
-		if (ensure_device(x)) return OCB_ERR_CUDA;
-		const size_t bytes = elems * sizeof(float);
-		int r;
-		if ((r = grow(x, x->own_series3[0], bytes)) || (r = grow(x, x->own_series3[1], (size_t)n_frames * bytes))) return r;
-		OCB_CUDA(x, cudaMemcpyAsync(x->own_series3[0].p, ref, bytes, cudaMemcpyHostToDevice, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(x->own_series3[1].p, tars, (size_t)n_frames * bytes, cudaMemcpyHostToDevice, x->stream));
-		series3_set(x, x->own_series3[0].as<float>(), x->own_series3[1].p, 0, n_frames, dim_x, dim_y, dim_z);
-		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+		const void* stack[1] = { tars };
+		return series_upload(x, x->series3d, ref, stack, 1, elems * sizeof(float), elems * sizeof(float), n_frames, dim_x, dim_y, dim_z);
+	});
+}
+
+// the reference of an 8-bit volume series crosses PCIe as bytes too, staged in the series' scratch volume and widened into the
+// reference buffer
+static int widen_series3_ref(ocb_ctx* x, const unsigned char* ref, size_t elems) {
+	if (const int rc = grow(x, x->series3_tmp, elems * sizeof(float))) return rc;
+	OCB_CUDA(x, cudaMemcpyAsync(x->series3_tmp.p, ref, elems, cudaMemcpyHostToDevice, x->stream));
+	ocb::widen_u8_kernel<<<x->sm_count * 8, 256, 0, x->stream>>>(x->series3_tmp.as<unsigned char>(), x->series3d.own[0].as<float>(), elems);
+	x->launches++;
+	OCB_CUDA(x, cudaGetLastError());
+	return OCB_OK;
 }
 
 int ocb_set_series_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned char* tars, int n_frames, int dim_x, int dim_y, int dim_z) {
-	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	ocb_ctx* x = series_exec(ctx);
-	const int rc = [&]() -> int {
+	return on_exec(ctx, [&](ocb_ctx* x) {
 		// frames start on 16-byte boundaries: the widening kernel reads uchar4
 		const size_t elems = series3_elems(n_frames, dim_x, dim_y, dim_z, 16);
 		if (!ref || !tars || !elems)
 			return set_error(x, OCB_ERR_ARG, "set_series_3d_u8: bad arguments (each dimension must be >= 15, n_frames >= 1)");
-		if (ensure_device(x)) return OCB_ERR_CUDA;
-		const size_t pitch = (elems + 15) & ~(size_t)15;
-		int r;
-		// the reference crosses PCIe as bytes too, staged in the series' scratch volume and widened into the reference buffer
-		if ((r = grow(x, x->own_series3[0], elems * sizeof(float))) || (r = grow(x, x->series3_tmp, elems * sizeof(float)))
-			|| (r = grow(x, x->own_series3[1], (size_t)n_frames * pitch)))
-			return r;
-		unsigned char* const stack = x->own_series3[1].as<unsigned char>();
-		OCB_CUDA(x, cudaMemcpyAsync(x->series3_tmp.p, ref, elems, cudaMemcpyHostToDevice, x->stream));
-		ocb::widen_u8_kernel<<<x->sm_count * 8, 256, 0, x->stream>>>(x->series3_tmp.as<unsigned char>(), x->own_series3[0].as<float>(), elems);
-		x->launches++;
-		OCB_CUDA(x, cudaGetLastError());
-		for (int f = 0; f < n_frames; f++)
-			OCB_CUDA(x, cudaMemcpyAsync(stack + (size_t)f * pitch, tars + (size_t)f * elems, elems, cudaMemcpyHostToDevice, x->stream));
-		series3_set(x, x->own_series3[0].as<float>(), stack, pitch, n_frames, dim_x, dim_y, dim_z);
-		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+		const void* stack[1] = { tars };
+		int rc = series_upload(x, x->series3d, nullptr, stack, 1, elems, (elems + 15) & ~(size_t)15, n_frames, dim_x, dim_y, dim_z);
+		if (rc == OCB_OK && (rc = widen_series3_ref(x, ref, elems))) series_clear(x->series3d);
+		return rc;
+	});
 }
 
 // Checks and runs a volume series on a single-device context: device seeds and output; rs null for the plain series.  Per frame:
@@ -1613,21 +1698,22 @@ int ocb_set_series_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned 
 static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv,
 	float stop, const SeriesReseed* rs) {
 	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1 || rz < 1) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
-	if (!ctx->series3.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
+	const SeriesStore& s = ctx->series3d;
+	if (!s.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
 	int rc;
 	if (rs && (rc = reseed_check(ctx, what, 3, *rs))) return rc;
 	if (n == 0) return OCB_OK;
 	const size_t rec = OCB_POI3D_FLOATS * sizeof(float);
-	if (n > 0x7fffffffull || (size_t)ctx->series3_frames > SIZE_MAX / (n * rec))
-		return set_error(ctx, OCB_ERR_ARG, "%s: too many POIs in one call", what);
+	if ((rc = series_size_check(ctx, what, n, s.frames, rec, false))) return rc;
 	if ((size_t)(2 * rx + 1) * (2 * ry + 1) * (2 * rz + 1) > 0x3fffffffull) return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn3d1: subset too large");
 	ocb::Icgn3dPlan plan;
 	if (!ocb::icgn3d1_plan(rx, ry, rz, ctx->smem_optin, &plan))
 		return set_error(ctx, OCB_ERR_UNSUPPORTED, "icgn3d1: subset radius (%d,%d,%d) exceeds the shared-memory design limit", rx, ry, rz);
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	const int F = ctx->series3_frames;
-	const int dx = ctx->series3.dx, dy = ctx->series3.dy, dz = ctx->series3.dz;
+	const int F = s.frames;
+	const int dx = s.w, dy = s.h, dz = s.d;
 	const size_t elems = (size_t)dx * dy * dz;
+	const bool u8 = s.pitch < elems * sizeof(float); // an 8-bit stack, widened into the scratch volume frame by frame
 	if ((rc = grow(ctx, ctx->series3_rg, elems * sizeof(float4))) || (rc = grow(ctx, ctx->series3_coef, elems * sizeof(float)))
 		|| (rc = grow(ctx, ctx->series3_tmp, elems * sizeof(float))) || (rc = grow(ctx, ctx->series3_cache, n * ocb::ICGN3D_SETUP_FLOATS * sizeof(float))))
 		return rc;
@@ -1638,7 +1724,7 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 	float* const coef = ctx->series3_coef.as<float>();
 	float* const tmp = ctx->series3_tmp.as<float>();
 	float* const cache = ctx->series3_cache.as<float>();
-	const ocb::Image3D img{ ctx->series3.ref, nullptr, rg, coef, dx, dy, dz };
+	const ocb::Image3D img{ s.ref, nullptr, rg, coef, dx, dy, dz };
 	cudaError_t err = cudaSuccess;
 	auto icgn = [&](float* q, size_t m, int setup) {
 		const int r3 = ocb::icgn3d1_launch(img, q, m, rx, ry, rz, conv, stop, ctx->sm_count, ctx->smem_optin, ctx->d_counter + 1, ctx->stream, &err, setup,
@@ -1647,9 +1733,9 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 		ctx->launches++;
 		return (int)OCB_OK;
 	};
+	auto frame = [&](int f) { return (const char*)s.tars[0] + (size_t)f * s.pitch; };
 	auto widen = [&](int f) {
-		ocb::widen_u8_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const unsigned char*)ctx->series3_tars + (size_t)f * ctx->series3_u8_pitch, tmp,
-			elems);
+		ocb::widen_u8_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const unsigned char*)frame(f), tmp, elems);
 		ctx->launches++;
 	};
 	// the reference's products, once per call: packed gradients, then each POI's setup pass (records are not written).
@@ -1658,7 +1744,7 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 	// reaches frame f + 1's LOAD with a good record.  The setup state depends only on the reference, the coordinates and the
 	// radii, so the entries of the POIs the plain series stores are the same; a POI without one (coordinates outside the
 	// volume or NaN) is still rejected by every guard.
-	ocb::gradient3d_launch(ctx->series3.ref, rg, dx, dy, dz, ctx->sm_count, ctx->stream);
+	ocb::gradient3d_launch(s.ref, rg, dx, dy, dz, ctx->sm_count, ctx->stream);
 	ctx->launches++;
 	if (rs) {
 		OCB_RESEED(ctx, ocb::reseed_rebuild_launch(3, (const float*)d_seeds, nullptr, nullptr, n, 0.f, nullptr, sub, ctx->sm_count, ctx->stream));
@@ -1667,13 +1753,8 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 	if ((rc = icgn(rs ? sub : const_cast<float*>((const float*)d_seeds), n, ocb::ICGN3D_SETUP_STORE))) return rc;
 	for (int f = 0; f < F; f++) {
 		// TricubicBspline::prepare of frame f as in ocb_icgn3d_prepare: x -> coefficient, y -> scratch, z -> coefficient
-		const float* tar;
-		if (ctx->series3_u8_pitch) {
-			widen(f);
-			tar = tmp;
-		} else {
-			tar = (const float*)ctx->series3_tars + (size_t)f * elems;
-		}
+		if (u8) widen(f);
+		const float* const tar = u8 ? tmp : (const float*)frame(f);
 		ocb::prefilter3d_launch(tar, coef, dx, dy, dz, 0, ctx->sm_count, ctx->stream);
 		ocb::prefilter3d_launch(coef, tmp, dx, dy, dz, 1, ctx->sm_count, ctx->stream);
 		ocb::prefilter3d_launch(tmp, coef, dx, dy, dz, 2, ctx->sm_count, ctx->stream);
@@ -1689,8 +1770,8 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 		const size_t m = (size_t)w.h_hist[f];
 		if (!m) continue;
 		if ((rc = reseed_gather(ctx, 3, &w, (const float*)d_seeds, f ? prev : nullptr, n, f, m, rs->zncc_min, sub))) return rc;
-		if (ctx->series3_u8_pitch) widen(f); // the prefilter's y pass overwrote the widened frame
-		const ocb::Image3D raw{ ctx->series3.ref, ctx->series3_u8_pitch ? tmp : tar, rg, coef, dx, dy, dz };
+		if (u8) widen(f); // the prefilter's y pass overwrote the widened frame
+		const ocb::Image3D raw{ s.ref, tar, rg, coef, dx, dy, dz };
 		if ((rc = fftcc3d_run(ctx, raw, sub, m, rs->fft_r[0], rs->fft_r[1], rs->fft_r[2]))) return rc;
 		if ((rc = icgn(sub, m, ocb::ICGN3D_SETUP_COMPUTE))) return rc;
 		OCB_RESEED(ctx, ocb::reseed_scatter_launch(3, sub, m, 1, w.idx, (float*)d_out, n, f, ctx->sm_count, ctx->stream));
@@ -1701,28 +1782,8 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 
 static int icgn3d_series_host(ocb_ctx* ctx, const char* what, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop,
 	const SeriesReseed* rs) {
-	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	ocb_ctx* x = series_exec(ctx);
-	const int rc = [&]() -> int {
-		if ((!seeds || !out) && n) return set_error(x, OCB_ERR_ARG, "%s: bad arguments", what);
-		if (!x->series3.ref) return set_error(x, OCB_ERR_STATE, "%s: no series set", what);
-		if (n == 0) return icgn3d_series_dev(x, what, nullptr, nullptr, 0, rx, ry, rz, conv, stop, rs); // argument checks only
-		const size_t rec = OCB_POI3D_FLOATS * sizeof(float);
-		if (n > 0x7fffffffull || (size_t)x->series3_frames + 1 > SIZE_MAX / (n * rec))
-			return set_error(x, OCB_ERR_ARG, "%s: too many POIs in one call", what);
-		if (ensure_device(x)) return OCB_ERR_CUDA;
-		const size_t out_bytes = (size_t)x->series3_frames * n * rec;
-		int r;
-		if ((r = grow(x, x->d_poi, n * rec + out_bytes))) return r;
-		float* const d_seeds = x->d_poi.as<float>();
-		float* const d_out = d_seeds + n * OCB_POI3D_FLOATS;
-		OCB_CUDA(x, cudaMemcpyAsync(d_seeds, seeds, n * rec, cudaMemcpyHostToDevice, x->stream));
-		if ((r = icgn3d_series_dev(x, what, d_seeds, d_out, n, rx, ry, rz, conv, stop, rs))) return r;
-		OCB_CUDA(x, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, x->stream));
-		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
-		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+	return series_host(ctx, what, &ocb_ctx::series3d, n, { seeds }, OCB_POI3D_FLOATS, { { out, OCB_POI3D_FLOATS } },
+		[&](ocb_ctx* x, const float* const* d_in, float* const* d_out) { return icgn3d_series_dev(x, what, d_in[0], d_out[0], n, rx, ry, rz, conv, stop, rs); });
 }
 
 int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop) {
@@ -1737,19 +1798,18 @@ int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int 
 int ocb_icgn3d_series_reseed_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop, int fft_rx,
 	int fft_ry, int fft_rz, float zncc_min, size_t* reseeded) {
 	OCB_NO_GROUP(ctx, "icgn3d_series_reseed_dev");
-	std::vector<size_t> counts(ctx && ctx->series3.ref ? ctx->series3_frames : 0, 0);
-	SeriesReseed rs{ { fft_rx, fft_ry, fft_rz }, zncc_min, counts.data() };
-	int rc = icgn3d_series_dev(ctx, "icgn3d_series_reseed", d_seeds, d_out, n, rx, ry, rz, conv, stop, &rs);
-	if (rc == OCB_OK && n) OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	return series_reseed_counts(rc, counts, reseeded);
+	return series_reseed(ctx, &ocb_ctx::series3d, true, n, reseeded, [&](size_t* counts) {
+		const SeriesReseed rs{ { fft_rx, fft_ry, fft_rz }, zncc_min, counts };
+		return icgn3d_series_dev(ctx, "icgn3d_series_reseed", d_seeds, d_out, n, rx, ry, rz, conv, stop, &rs);
+	});
 }
 
 int ocb_icgn3d_series_reseed(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop, int fft_rx,
 	int fft_ry, int fft_rz, float zncc_min, size_t* reseeded) {
-	const ocb_ctx* x = ctx ? series_exec(ctx) : nullptr;
-	std::vector<size_t> counts(x && x->series3.ref ? x->series3_frames : 0, 0);
-	SeriesReseed rs{ { fft_rx, fft_ry, fft_rz }, zncc_min, counts.data() };
-	return series_reseed_counts(icgn3d_series_host(ctx, "icgn3d_series_reseed", seeds, out, n, rx, ry, rz, conv, stop, &rs), counts, reseeded);
+	return series_reseed(ctx, &ocb_ctx::series3d, false, n, reseeded, [&](size_t* counts) {
+		const SeriesReseed rs{ { fft_rx, fft_ry, fft_rz }, zncc_min, counts };
+		return icgn3d_series_host(ctx, "icgn3d_series_reseed", seeds, out, n, rx, ry, rz, conv, stop, &rs);
+	});
 }
 
 int ocb_get_tables_3d(ocb_ctx* ctx, float* gx, float* gy, float* gz, float* coefficient) {
@@ -1769,15 +1829,6 @@ int ocb_get_tables_3d(ocb_ctx* ctx, float* gx, float* gy, float* gz, float* coef
 }
 
 // ---- Stereo reconstruction: Calibration::prepare / undistort, Stereovision::reconstruct --------------------------------------
-// A failure on the executing member of a group is reported on the group as well.
-static int relay_error(ocb_ctx* ctx, const ocb_ctx* exec, int rc) {
-	if (rc != OCB_OK && ctx != exec) {
-		ctx->last_error = exec->last_error;
-		g_last_error = ctx->last_error;
-	}
-	return rc;
-}
-
 static int calib_check(ocb_ctx* ctx, const ocb_calib* c, const char* what) {
 	if (!c) return set_error(ctx, OCB_ERR_ARG, "%s: null calibration handle", what);
 	if (c->owner != ctx) return set_error(ctx, OCB_ERR_ARG, "%s: calibration handle belongs to another context", what);
@@ -1810,7 +1861,7 @@ int ocb_calib_prepare(ocb_ctx* ctx, const float* intrinsics, int height, int wid
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
 	if (!intrinsics || !out) return set_error(ctx, OCB_ERR_ARG, "calib_prepare: bad arguments");
 	if (height < 2 || width < 2) return set_error(ctx, OCB_ERR_ARG, "calib_prepare: image size %d x %d is below 2 x 2", width, height);
-	ocb_ctx* x = is_group(ctx) ? ctx->members[0] : ctx;
+	ocb_ctx* x = exec_member(ctx);
 	ocb_calib* c = new ocb_calib;
 	c->owner = ctx;
 	c->exec = x;
@@ -1934,77 +1985,55 @@ int ocb_stereo_reconstruct(ocb_ctx* ctx, const ocb_calib* calib1, const float* i
 
 // ---- Stereo series: both views of every frame registered against reference view 1, triangulated into POI2DS records ---------
 // On a group context the first member holds the series and runs the calls; the calibration maps of a group live there too.
-static void stereo_series_set(ocb_ctx* x, const float* ref1, const float* tars1, const float* tars2, int n_frames, int width, int height) {
-	x->stereo1 = ocb::Image2D{ ref1, tars1, width, height };
-	x->stereo2 = ocb::Image2D{ ref1, tars2, width, height };
-	x->stereo_frames = n_frames;
-}
-
 int ocb_set_stereo_series_2d_dev(ocb_ctx* ctx, const float* d_ref1, const float* d_tars1, const float* d_tars2, int n_frames, int width, int height) {
 	OCB_NO_GROUP(ctx, "set_stereo_series_2d_dev");
 	if (!ctx || !d_ref1 || !d_tars1 || !d_tars2 || n_frames < 1 || width < 5 || height < 5)
 		return set_error(ctx, OCB_ERR_ARG, "set_stereo_series_2d: bad arguments");
-	stereo_series_set(ctx, d_ref1, d_tars1, d_tars2, n_frames, width, height);
+	series_borrow(ctx->stereo, d_ref1, d_tars1, d_tars2, (size_t)width * height * sizeof(float), n_frames, width, height, 1);
 	return OCB_OK;
 }
 
 int ocb_set_stereo_series_2d(ocb_ctx* ctx, const float* ref1, const float* tars1, const float* tars2, int n_frames, int width, int height) {
-	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	ocb_ctx* x = series_exec(ctx);
-	const int rc = [&]() -> int {
+	return on_exec(ctx, [&](ocb_ctx* x) {
 		if (!ref1 || !tars1 || !tars2 || n_frames < 1 || width < 5 || height < 5) return set_error(x, OCB_ERR_ARG, "set_stereo_series_2d: bad arguments");
-		const size_t elems = (size_t)width * height;
-		if ((size_t)n_frames > SIZE_MAX / sizeof(float) / elems) return set_error(x, OCB_ERR_ARG, "set_stereo_series_2d: series too large");
-		if (ensure_device(x)) return OCB_ERR_CUDA;
-		stereo_series_set(x, nullptr, nullptr, nullptr, 0, 0, 0); // a failed growth below leaves no series rather than a stale one
-		const size_t frame = elems * sizeof(float), stack = (size_t)n_frames * frame;
-		int r;
-		if ((r = grow(x, x->own_stereo[0], frame)) || (r = grow(x, x->own_stereo[1], stack)) || (r = grow(x, x->own_stereo[2], stack))) return r;
-		OCB_CUDA(x, cudaMemcpyAsync(x->own_stereo[0].p, ref1, frame, cudaMemcpyHostToDevice, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(x->own_stereo[1].p, tars1, stack, cudaMemcpyHostToDevice, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(x->own_stereo[2].p, tars2, stack, cudaMemcpyHostToDevice, x->stream));
-		stereo_series_set(x, x->own_stereo[0].as<float>(), x->own_stereo[1].as<float>(), x->own_stereo[2].as<float>(), n_frames, width, height);
-		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+		const size_t frame = (size_t)width * height * sizeof(float);
+		if ((size_t)n_frames > SIZE_MAX / frame) return set_error(x, OCB_ERR_ARG, "set_stereo_series_2d: series too large");
+		const void* stacks[2] = { tars1, tars2 };
+		return series_upload(x, x->stereo, ref1, stacks, 2, frame, frame, n_frames, width, height, 1);
+	});
 }
 
 // The cameras, checked on the caller's context as ocb_stereo_reconstruct checks them
 static int stereo_series_cams(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrinsics1, const float* projection1, const ocb_calib* calib2,
-	const float* intrinsics2, const float* projection2) {
+	const float* intrinsics2, const float* projection2, ocb::StereoCam* s1, ocb::StereoCam* s2) {
 	int rc = calib_check(ctx, calib1, "stereo_series");
 	if (!rc) rc = calib_check(ctx, calib2, "stereo_series");
 	if (rc) return rc;
 	if (!intrinsics1 || !projection1 || !intrinsics2 || !projection2) return set_error(ctx, OCB_ERR_ARG, "stereo_series: bad arguments");
+	stereo_cams(calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, s1, s2);
 	return OCB_OK;
 }
 
-// Everything else, on the context x that holds the series, before any work: pointers, orders, the series, sizes and the radii
-// (both IC-GN plans, so that a radius one order rejects stops the call before the other view runs).
-static int stereo_series_check(ocb_ctx* x, bool pointers_ok, int order1, int order2, size_t n, int rx, int ry) {
-	if (!pointers_ok || rx < 1 || ry < 1) return set_error(x, OCB_ERR_ARG, "stereo_series: bad arguments");
-	if ((order1 != 1 && order1 != 2) || (order2 != 1 && order2 != 2)) return set_error(x, OCB_ERR_ARG, "stereo_series: order must be 1 or 2");
-	if (!x->stereo1.ref) return set_error(x, OCB_ERR_STATE, "stereo_series: no stereo series set");
-	if (n == 0) return OCB_OK;
-	const size_t rec = (2 * OCB_POI2D_FLOATS + OCB_POI2DS_FLOATS) * sizeof(float); // per frame and POI; the host call stages 3 n records more
-	if (n > 0x7fffffffull || (size_t)x->stereo_frames + 1 > SIZE_MAX / (n * rec)) return set_error(x, OCB_ERR_ARG, "stereo_series: too many POIs in one call");
-	const char* e = getenv("OCB_ICGN2D_WPP"); // as icgn2d_series_launch plans
-	for (const int order : { order1, order2 }) {
-		ocb::Icgn2dPlan plan;
-		if (!ocb::icgn2d_plan(n, order == 1 ? 6 : 12, rx, ry, false, x->sm_count, x->smem_optin, e ? atoi(e) : 0, &plan))
-			return set_error(x, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
-	}
-	return OCB_OK;
-}
-
-// The two registrations (each one 2D series launch) and the records, on x (device current), after the checks above
-static int stereo_series_run(ocb_ctx* x, const ocb::StereoCam& c1, const ocb::StereoCam& c2, int order1, int order2, const float* d_stereo,
+// Checks and runs a stereo series call on the context x that holds the series (device pointers), after the cameras' checks.  Every
+// check comes before any work: pointers, orders, the series, sizes and the radii (both IC-GN plans, so that a radius one order
+// rejects stops the call before the other view runs).  Then the two registrations (each one 2D series launch) and the records.
+static int stereo_series_dev(ocb_ctx* x, const ocb::StereoCam& c1, const ocb::StereoCam& c2, int order1, int order2, const float* d_stereo,
 	const float* d_seeds1, const float* d_seeds2, float* d_out1, float* d_out2, float* d_out2ds, size_t n, int rx, int ry, float conv, float stop) {
-	const int F = x->stereo_frames;
+	if (((!d_stereo || !d_seeds1 || !d_seeds2 || !d_out1 || !d_out2 || !d_out2ds) && n) || rx < 1 || ry < 1)
+		return set_error(x, OCB_ERR_ARG, "stereo_series: bad arguments");
+	if ((order1 != 1 && order1 != 2) || (order2 != 1 && order2 != 2)) return set_error(x, OCB_ERR_ARG, "stereo_series: order must be 1 or 2");
+	const SeriesStore& s = x->stereo;
+	if (!s.ref) return set_error(x, OCB_ERR_STATE, "stereo_series: no series set");
+	if (n == 0) return OCB_OK;
 	int rc;
-	if ((rc = icgn2d_series_run(x, order1 == 1 ? 6 : 12, x->stereo1, F, d_seeds1, d_out1, n, rx, ry, conv, stop, nullptr))) return rc;
-	if ((rc = icgn2d_series_run(x, order2 == 1 ? 6 : 12, x->stereo2, F, d_seeds2, d_out2, n, rx, ry, conv, stop, nullptr))) return rc;
-	ocb::stereo_poi2ds_launch(c1, c2, d_stereo, d_seeds1, d_out1, d_out2, d_out2ds, n, F, x->stream);
+	if ((rc = series_size_check(x, "stereo_series", n, s.frames, (2 * OCB_POI2D_FLOATS + OCB_POI2DS_FLOATS) * sizeof(float), false))) return rc;
+	const int np1 = order1 == 1 ? 6 : 12, np2 = order2 == 1 ? 6 : 12;
+	if (!ocb::icgn2d_fits(n, np1, rx, ry, x->sm_count, x->smem_optin) || !ocb::icgn2d_fits(n, np2, rx, ry, x->sm_count, x->smem_optin))
+		return set_error(x, OCB_ERR_UNSUPPORTED, "icgn2d: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
+	if (ensure_device(x)) return OCB_ERR_CUDA;
+	if ((rc = icgn2d_series_run(x, np1, s.view2(0), s.frames, d_seeds1, d_out1, n, rx, ry, conv, stop, nullptr))) return rc;
+	if ((rc = icgn2d_series_run(x, np2, s.view2(1), s.frames, d_seeds2, d_out2, n, rx, ry, conv, stop, nullptr))) return rc;
+	ocb::stereo_poi2ds_launch(c1, c2, d_stereo, d_seeds1, d_out1, d_out2, d_out2ds, n, s.frames, x->stream);
 	OCB_CUDA(x, cudaGetLastError());
 	x->launches++;
 	return OCB_OK;
@@ -2015,14 +2044,9 @@ int ocb_stereo_series_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* in
 	void* d_out1, void* d_out2, void* d_out2ds, size_t n, int rx, int ry, float conv, float stop) {
 	OCB_NO_GROUP(ctx, "stereo_series_dev");
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	int rc = stereo_series_cams(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2);
-	if (rc) return rc;
-	const bool ptrs = (d_stereo && d_seeds1 && d_seeds2 && d_out1 && d_out2 && d_out2ds) || n == 0;
-	if ((rc = stereo_series_check(ctx, ptrs, order1, order2, n, rx, ry)) || n == 0) return rc;
-	if (ensure_device(ctx)) return OCB_ERR_CUDA;
 	ocb::StereoCam s1, s2;
-	stereo_cams(calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2);
-	return stereo_series_run(ctx, s1, s2, order1, order2, (const float*)d_stereo, (const float*)d_seeds1, (const float*)d_seeds2, (float*)d_out1,
+	if (const int rc = stereo_series_cams(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2)) return rc;
+	return stereo_series_dev(ctx, s1, s2, order1, order2, (const float*)d_stereo, (const float*)d_seeds1, (const float*)d_seeds2, (float*)d_out1,
 		(float*)d_out2, (float*)d_out2ds, n, rx, ry, conv, stop);
 }
 
@@ -2030,46 +2054,20 @@ int ocb_stereo_series(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrin
 	const float* intrinsics2, const float* projection2, int order1, int order2, const void* stereo, const void* seeds1, const void* seeds2,
 	void* out1, void* out2, void* out2ds, size_t n, int rx, int ry, float conv, float stop) {
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	int rc = stereo_series_cams(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2);
-	if (rc) return rc;
-	ocb_ctx* x = series_exec(ctx);
-	rc = [&]() -> int {
-		const bool ptrs = (stereo && seeds1 && seeds2 && out1 && out2 && out2ds) || n == 0;
-		int r;
-		if ((r = stereo_series_check(x, ptrs, order1, order2, n, rx, ry)) || n == 0) return r;
-		if (ensure_device(x)) return OCB_ERR_CUDA;
-		const size_t rec = OCB_POI2D_FLOATS * sizeof(float), F = (size_t)x->stereo_frames;
-		const size_t out_bytes = F * n * rec, ds_bytes = F * n * OCB_POI2DS_FLOATS * sizeof(float);
-		if ((r = grow(x, x->d_poi, 3 * n * rec + 2 * out_bytes + ds_bytes))) return r;
-		float* const d_stereo = x->d_poi.as<float>();
-		float* const d_seeds1 = d_stereo + n * OCB_POI2D_FLOATS;
-		float* const d_seeds2 = d_seeds1 + n * OCB_POI2D_FLOATS;
-		float* const d_out1 = d_seeds2 + n * OCB_POI2D_FLOATS;
-		float* const d_out2 = d_out1 + F * n * OCB_POI2D_FLOATS;
-		float* const d_out2ds = d_out2 + F * n * OCB_POI2D_FLOATS;
-		OCB_CUDA(x, cudaMemcpyAsync(d_stereo, stereo, n * rec, cudaMemcpyHostToDevice, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(d_seeds1, seeds1, n * rec, cudaMemcpyHostToDevice, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(d_seeds2, seeds2, n * rec, cudaMemcpyHostToDevice, x->stream));
-		ocb::StereoCam s1, s2;
-		stereo_cams(calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2);
-		if ((r = stereo_series_run(x, s1, s2, order1, order2, d_stereo, d_seeds1, d_seeds2, d_out1, d_out2, d_out2ds, n, rx, ry, conv, stop))) return r;
-		OCB_CUDA(x, cudaMemcpyAsync(out1, d_out1, out_bytes, cudaMemcpyDeviceToHost, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(out2, d_out2, out_bytes, cudaMemcpyDeviceToHost, x->stream));
-		OCB_CUDA(x, cudaMemcpyAsync(out2ds, d_out2ds, ds_bytes, cudaMemcpyDeviceToHost, x->stream));
-		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
-		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+	ocb::StereoCam s1, s2;
+	if (const int rc = stereo_series_cams(ctx, calib1, intrinsics1, projection1, calib2, intrinsics2, projection2, &s1, &s2)) return rc;
+	return series_host(ctx, "stereo_series", &ocb_ctx::stereo, n, { stereo, seeds1, seeds2 }, OCB_POI2D_FLOATS,
+		{ { out1, OCB_POI2D_FLOATS }, { out2, OCB_POI2D_FLOATS }, { out2ds, OCB_POI2DS_FLOATS } },
+		[&](ocb_ctx* x, const float* const* d_in, float* const* d_out) {
+			return stereo_series_dev(x, s1, s2, order1, order2, d_in[0], d_in[1], d_in[2], d_out[0], d_out[1], d_out[2], n, rx, ry, conv, stop);
+		});
 }
 
 // ---- SIFT3D: SIFT3D::compute (src/oc_sift.cpp:234-293) --------------------------------------------------------------------
 // On a group context the first member runs it and keeps the results (one pair of volumes; see DESIGN.md section 6).
-static ocb_ctx* sift3d_exec(ocb_ctx* ctx) { return is_group(ctx) ? ctx->members[0] : ctx; }
-
 int ocb_sift3d(ocb_ctx* ctx, const float* config, const float* unit_xyz, float matching_ratio, size_t* n_matched, int* n_octave) {
 	if (!ctx || !config || !unit_xyz) return set_error(ctx, OCB_ERR_ARG, "sift3d: null argument");
-	ocb_ctx* x = sift3d_exec(ctx);
-	const int rc = [&]() -> int {
+	return on_exec(ctx, [&](ocb_ctx* x) -> int {
 		if (!x->img3.ref) return set_error(x, OCB_ERR_STATE, "sift3d: images not set");
 		for (int a = 0; a < 3; a++)
 			if (!(unit_xyz[a] > 0.f) || !std::isfinite(unit_xyz[a])) return set_error(x, OCB_ERR_ARG, "sift3d: physical units must be positive");
@@ -2083,13 +2081,12 @@ int ocb_sift3d(ocb_ctx* ctx, const float* config, const float* unit_xyz, float m
 		if (n_matched) *n_matched = ocb::sift3d_n_matched(x->sift3d);
 		if (n_octave) *n_octave = ocb::sift3d_n_octave(x->sift3d, 1);
 		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+	});
 }
 
 int ocb_sift3d_get_matches(ocb_ctx* ctx, float* ref_xyz, float* tar_xyz) {
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
-	ocb_ctx* x = sift3d_exec(ctx);
+	ocb_ctx* x = exec_member(ctx);
 	if (!x->sift3d) return relay_error(ctx, x, set_error(x, OCB_ERR_STATE, "sift3d_get_matches: ocb_sift3d has not run"));
 	ocb::sift3d_get_matches(x->sift3d, ref_xyz, tar_xyz);
 	return OCB_OK;
@@ -2097,21 +2094,19 @@ int ocb_sift3d_get_matches(ocb_ctx* ctx, float* ref_xyz, float* tar_xyz) {
 
 int ocb_sift3d_inspect(ocb_ctx* ctx, int image, size_t* counts, int* candidates, float* max_abs, float* keypoints, float* descriptors) {
 	if (!ctx || !counts || (image != 0 && image != 1)) return set_error(ctx, OCB_ERR_ARG, "sift3d_inspect: bad arguments");
-	ocb_ctx* x = sift3d_exec(ctx);
-	const int rc = [&]() -> int {
+	return on_exec(ctx, [&](ocb_ctx* x) -> int {
 		if (!x->sift3d) return set_error(x, OCB_ERR_STATE, "sift3d_inspect: ocb_sift3d has not run");
 		if (ensure_device(x)) return OCB_ERR_CUDA;
 		std::string err;
 		if (ocb::sift3d_inspect(x->sift3d, image, counts, candidates, max_abs, keypoints, descriptors, x->stream, &err))
 			return set_error(x, OCB_ERR_CUDA, "%s", err.c_str());
 		return OCB_OK;
-	}();
-	return relay_error(ctx, x, rc);
+	});
 }
 
 int ocb_sift3d_stage_times(ocb_ctx* ctx, float* ms) {
 	if (!ctx || !ms) return set_error(ctx, OCB_ERR_ARG, "sift3d_stage_times: bad arguments");
-	ocb_ctx* x = sift3d_exec(ctx);
+	ocb_ctx* x = exec_member(ctx);
 	if (!x->sift3d) return relay_error(ctx, x, set_error(x, OCB_ERR_STATE, "sift3d_stage_times: ocb_sift3d has not run"));
 	const float* t = ocb::sift3d_stage_ms(x->sift3d);
 	std::copy(t, t + ocb::SIFT3D_STAGES, ms);

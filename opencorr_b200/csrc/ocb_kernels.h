@@ -118,6 +118,9 @@ int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, i
 	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err,
 	size_t plan_n);
 size_t icgn2d_slab_bytes(int rx, int ry); // shared memory one POI needs (plain IC-GN, one warp per POI)
+// whether a plain IC-GN launch over n POIs (icgn2d_launch, icgn2d_series_launch) has a plan for radius (rx, ry): false where they
+// would return -1
+bool icgn2d_fits(size_t n, int np, int rx, int ry, int sm_count, size_t smem_optin);
 // one reference (img.ref) against the frame-major stack img.tar [n_frames][h][w]: n seeds in, n_frames x n records out (frame-major)
 int icgn2d_series_launch(int np, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
 	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err, size_t plan_n);
