@@ -94,7 +94,7 @@ __global__ void epipolar_select_kernel(float* __restrict__ pois, int poi0, int n
 	}
 }
 
-void epipolar_candidates_launch(const float* d_pois, size_t poi0, size_t n_poi, const float* fundamental, const float* parallax_x,
+cudaError_t epipolar_candidates_launch(const float* d_pois, size_t poi0, size_t n_poi, const float* fundamental, const float* parallax_x,
 	const float* parallax_y, int search_radius, int search_step, int rx, int ry, int w, int h, int slots, float* d_cand, int sm_count,
 	cudaStream_t stream) {
 	EpiParams p;
@@ -106,13 +106,15 @@ void epipolar_candidates_launch(const float* d_pois, size_t poi0, size_t n_poi, 
 	if (blocks > (long long)sm_count * 16) blocks = (long long)sm_count * 16;
 	if (blocks < 1) blocks = 1;
 	epipolar_candidates_kernel<<<(int)blocks, 256, 0, stream>>>(d_pois, (int)poi0, (int)n_poi, p, d_cand);
+	return cudaGetLastError();
 }
 
-void epipolar_select_launch(float* d_pois, size_t poi0, size_t n_poi, int slots, const float* d_cand, int sm_count, cudaStream_t stream) {
+cudaError_t epipolar_select_launch(float* d_pois, size_t poi0, size_t n_poi, int slots, const float* d_cand, int sm_count, cudaStream_t stream) {
 	long long blocks = ((long long)n_poi * 32 + 255) / 256;
 	if (blocks > (long long)sm_count * 16) blocks = (long long)sm_count * 16;
 	if (blocks < 1) blocks = 1;
 	epipolar_select_kernel<<<(int)blocks, 256, 0, stream>>>(d_pois, (int)poi0, (int)n_poi, slots, d_cand);
+	return cudaGetLastError();
 }
 
 } // namespace ocb

@@ -388,29 +388,20 @@ __global__ void __launch_bounds__(256) fftcc3d_kernel(Image3D img, float* __rest
 }
 
 // host side ------------------------------------------------------------------------------------
-int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const Fftcc2dPlan& plan, const float2* tw_x,
-	const float2* tw_y, int grid, cudaStream_t stream, cudaError_t* err) {
+cudaError_t fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const Fftcc2dPlan& plan, const float2* tw_x,
+	const float2* tw_y, int grid, cudaStream_t stream) {
 	Fft2DParams fp;
 	fp.ax = plan.ax; fp.ay = plan.ay; fp.tw_x = tw_x; fp.tw_y = tw_y;
-	const size_t smem = plan.smem;
-	*err = cudaFuncSetAttribute(fftcc2d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-	if (*err != cudaSuccess) return -2;
-	fftcc2d_kernel<<<grid, 128, smem, stream>>>(img, d_pois, (int)n, rx, ry, fp);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return launch_smem(fftcc2d_kernel, grid, 128, plan.smem, stream, img, d_pois, (int)n, rx, ry, fp);
 }
 
-int fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const Fftcc3dPlan& plan, const float2* tw_x,
-	const float2* tw_y, const float2* tw_z, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err) {
+cudaError_t fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const Fftcc3dPlan& plan, const float2* tw_x,
+	const float2* tw_y, const float2* tw_z, float2* scratch, int grid, cudaStream_t stream) {
 	Fft3DParams fp;
 	fp.ax = plan.ax; fp.ay = plan.ay; fp.az = plan.az;
 	fp.tw_x = tw_x; fp.tw_y = tw_y; fp.tw_z = tw_z;
 	fp.scratch = scratch;
-	*err = cudaFuncSetAttribute(fftcc3d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
-	if (*err != cudaSuccess) return -2;
-	fftcc3d_kernel<<<grid, 256, plan.smem, stream>>>(img, d_pois, (int)n, rx, ry, rz, fp);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return launch_smem(fftcc3d_kernel, grid, 256, plan.smem, stream, img, d_pois, (int)n, rx, ry, rz, fp);
 }
 
 } // namespace ocb

@@ -168,21 +168,12 @@ __global__ void __launch_bounds__(FFTREG_THREADS, fft_reg_min_ctas(N)) fftcc2d_r
 	}
 }
 
-template <int N>
-static int fftcc2d_reg_launch_n(const Image2D& img, float* d_pois, size_t n, const Fftcc2dPlan& plan, int grid, cudaStream_t stream, cudaError_t* err) {
-	*err = cudaFuncSetAttribute(fftcc2d_reg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
-	if (*err != cudaSuccess) return -2;
-	fftcc2d_reg_kernel<N><<<grid, FFTREG_THREADS, plan.smem, stream>>>(img, d_pois, (int)n);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
-}
-
-int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int grid, cudaStream_t stream, cudaError_t* err) {
+cudaError_t fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int grid, cudaStream_t stream) {
 	switch (2 * r) {
-#define X(N) case N: return fftcc2d_reg_launch_n<N>(img, d_pois, n, plan, grid, stream, err);
+#define X(N) case N: return launch_smem(fftcc2d_reg_kernel<N>, grid, FFTREG_THREADS, plan.smem, stream, img, d_pois, (int)n);
 		OCB_FFT_REG_SIZES(X)
 #undef X
-	default: *err = cudaErrorInvalidValue; return -2;
+	default: return cudaErrorInvalidValue;
 	}
 }
 

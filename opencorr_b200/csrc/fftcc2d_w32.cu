@@ -207,15 +207,14 @@ __global__ void __launch_bounds__(FFTW32_WARPS * 32) fftcc2d_w32_kernel(Image2D 
 	}
 }
 
-int fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int grid, cudaStream_t stream, cudaError_t* err) {
+cudaError_t fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int grid, cudaStream_t stream) {
 	CUtensorMap tm_ref, tm_tar;
 	memset(&tm_ref, 0, sizeof(tm_ref));
 	memset(&tm_tar, 0, sizeof(tm_tar));
 	const int dims[2] = { img.w, img.h }, box[2] = { FFTW32_BOX_W, 32 };
-	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_ref, img.ref, 2, dims, box) && tma_make_map(&tm_tar, img.tar, 2, dims, box);
+	const int use_tma = tma_enabled() && tma_make_map(&tm_ref, img.ref, 2, dims, box) && tma_make_map(&tm_tar, img.tar, 2, dims, box);
 	fftcc2d_w32_kernel<<<grid, FFTW32_WARPS * 32, 0, stream>>>(img, d_pois, (int)n, tm_ref, tm_tar, use_tma);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return cudaGetLastError();
 }
 
 } // namespace ocb

@@ -222,23 +222,13 @@ __global__ void __launch_bounds__(F3R_THREADS, fft_reg_min_ctas(N)) fftcc3d_reg_
 	}
 }
 
-template <int N>
-static int fftcc3d_reg_launch_n(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
-	cudaError_t* err) {
-	*err = cudaFuncSetAttribute(fftcc3d_reg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem);
-	if (*err != cudaSuccess) return -2;
-	fftcc3d_reg_kernel<N><<<grid, F3R_THREADS, plan.smem, stream>>>(img, d_pois, (int)n, scratch);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
-}
-
-int fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
-	cudaError_t* err) {
+cudaError_t fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, const Fftcc3dPlan& plan, float2* scratch, int grid,
+	cudaStream_t stream) {
 	switch (plan.n) {
-#define X(n) case n: return fftcc3d_reg_launch_n<n>(img, d_pois, n_poi, plan, scratch, grid, stream, err);
+#define X(N) case N: return launch_smem(fftcc3d_reg_kernel<N>, grid, F3R_THREADS, plan.smem, stream, img, d_pois, (int)n_poi, scratch);
 		OCB_FFT_REG_SIZES(X)
 #undef X
-	default: *err = cudaErrorInvalidValue; return -2;
+	default: return cudaErrorInvalidValue;
 	}
 }
 

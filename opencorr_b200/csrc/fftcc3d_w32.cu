@@ -241,19 +241,14 @@ __global__ void __launch_bounds__(F3_WARPS * 32, 2) fftcc3d_w32_kernel(Image3D i
 	}
 }
 
-int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
-	cudaError_t* err) {
-	const size_t smem = plan.smem;
+cudaError_t fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid,
+	cudaStream_t stream) {
 	CUtensorMap tm_ref, tm_tar;
 	memset(&tm_ref, 0, sizeof(tm_ref));
 	memset(&tm_tar, 0, sizeof(tm_tar));
 	const int dims[3] = { img.dx, img.dy, img.dz }, box[3] = { F3_BOX_W, 32, 1 };
-	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_ref, img.ref, 3, dims, box) && tma_make_map(&tm_tar, img.tar, 3, dims, box);
-	*err = cudaFuncSetAttribute(fftcc3d_w32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-	if (*err != cudaSuccess) return -2;
-	fftcc3d_w32_kernel<<<grid, F3_WARPS * 32, smem, stream>>>(img, d_pois, (int)n, scratch, tm_ref, tm_tar, use_tma);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	const int use_tma = tma_enabled() && tma_make_map(&tm_ref, img.ref, 3, dims, box) && tma_make_map(&tm_tar, img.tar, 3, dims, box);
+	return launch_smem(fftcc3d_w32_kernel, grid, F3_WARPS * 32, plan.smem, stream, img, d_pois, (int)n, scratch, tm_ref, tm_tar, use_tma);
 }
 
 } // namespace ocb

@@ -1145,9 +1145,6 @@ __global__ void __launch_bounds__(32 * WPP, icgn2d_min_ctas(NP, RC, WPP)) icgn2d
 }
 
 // host-side launch ---------------------------------------------------------------------------
-// Returns 0, -1 when one warp's slab does not fit in shared memory, -2 on a CUDA error.
-// d_counter: a work-queue head owned by the context (64 ints; see ocb_create: [k] is zeroed per launch, [32 + k] and [40 + k] are
-// the self-resetting head and departure count of the one-warp-per-POI kernels).
 typedef void (*Icgn2dKernel)(Image2D, float*, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int, const float*, float, float, float);
 typedef void (*Icgn2dSeriesKernel)(Image2D, const float*, float*, int, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int);
 
@@ -1163,78 +1160,45 @@ static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rc) {
 	return rc == 20 ? icgn2d_series_kernel<12, 20, WPP> : icgn2d_series_kernel<12, 0, WPP>;
 }
 
-size_t icgn2d_slab_bytes(int rx, int ry) { return (size_t)icgn2d_slab_floats(rx, ry, false, 1) * sizeof(float); }
-
-// icgn2d_plan with the warps per POI the environment may force
-static bool icgn2d_plan_env(size_t n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, Icgn2dPlan* p) {
-	const char* e = getenv("OCB_ICGN2D_WPP"); // tuning knob: 1 or 2 forces the warps per POI
-	return icgn2d_plan(n, np, rx, ry, lm, sm_count, smem_optin, e ? atoi(e) : 0, p);
-}
-bool icgn2d_fits(size_t n, int np, int rx, int ry, int sm_count, size_t smem_optin) {
-	Icgn2dPlan plan;
-	return icgn2d_plan_env(n, np, rx, ry, false, sm_count, smem_optin, &plan);
-}
-
-// What a launch over n POIs runs with (icgn2d_plan) and the work-queue head it uses.  A series call takes the pair call's
-// geometry for the same n, so that a frame splits its sums between warps exactly as a pair call does.  The warps per POI are
-// those of a launch over plan_n POIs (plan_n = n but for a re-seeded sub-queue); the grid never exceeds n.
-struct Icgn2dGeometry {
-	Icgn2dPlan plan;
-	int* counter;
-};
-static int icgn2d_geometry(size_t n, size_t plan_n, int np, int rx, int ry, bool lm, int sm_count, size_t smem_optin, int* d_counter,
-	cudaStream_t stream, Icgn2dGeometry* g, cudaError_t* err) {
-	if (!icgn2d_plan_env(plan_n, np, rx, ry, lm, sm_count, smem_optin, &g->plan)) return -1;
-	if ((size_t)g->plan.grid > n) g->plan.grid = n > 0 ? (int)n : 1;
-	if (g->plan.wpp != 1) {
-		*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
-		if (*err != cudaSuccess) return -2;
-	} else {
-		d_counter += 32; // the one-warp-per-POI kernels reset their queue head themselves: a set of heads nobody else touches
+// The work-queue head of a launch: [0] of the context's heads, zeroed here, for two warps per POI; [32] for the one-warp-per-POI
+// kernels, which reset their head themselves (a set of heads nobody else touches; [40] is their departure count).
+static cudaError_t icgn2d_counter(const Icgn2dPlan& p, int** d_counter, cudaStream_t stream) {
+	if (p.wpp == 1) {
+		*d_counter += 32;
+		return cudaSuccess;
 	}
-	g->counter = d_counter;
-	return 0;
+	return cudaMemsetAsync(*d_counter, 0, sizeof(int), stream);
 }
 
-int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
-	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err,
-	size_t plan_n) {
+cudaError_t icgn2d_launch(int np, const Icgn2dPlan& p, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop,
+	int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream) {
 	const bool lm = lm_damping != nullptr;
-	Icgn2dGeometry g;
-	if (const int rc = icgn2d_geometry(n, plan_n, np, rx, ry, lm, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
-	const Icgn2dPlan& p = g.plan;
+	cudaError_t e = icgn2d_counter(p, &d_counter, stream);
+	if (e != cudaSuccess) return e;
 	CUtensorMap tm_ref, tm_tar;
 	memset(&tm_ref, 0, sizeof(tm_ref));
 	memset(&tm_tar, 0, sizeof(tm_tar));
 	const int dims[2] = { img.w, img.h };
 	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[2] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry) };
-	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
+	const int use_tma = tma_enabled() && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
 	Icgn2dKernel kern = p.wpp == 2 ? icgn2d_pick<2>(np, p.rc, lm) : icgn2d_pick<1>(np, p.rc, lm);
-	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
-	if (*err != cudaSuccess) return -2;
-	kern<<<p.grid, p.wpp * 32, p.smem, stream>>>(img, d_pois, (int)n, rx, ry, conv, stop, g.counter, tm_ref, tm_tar, use_tma, d_center_offsets,
-		lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return launch_smem(kern, p.grid, p.wpp * 32, p.smem, stream, img, d_pois, (int)n, rx, ry, conv, stop, d_counter, tm_ref, tm_tar, use_tma,
+		d_center_offsets, lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
 }
 
-int icgn2d_series_launch(int np, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
-	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err, size_t plan_n) {
-	Icgn2dGeometry g;
-	if (const int rc = icgn2d_geometry(n, plan_n, np, rx, ry, false, sm_count, smem_optin, d_counter, stream, &g, err)) return rc;
-	const Icgn2dPlan& p = g.plan;
+cudaError_t icgn2d_series_launch(int np, const Icgn2dPlan& p, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n,
+	int rx, int ry, float conv, float stop, int* d_counter, cudaStream_t stream) {
+	cudaError_t e = icgn2d_counter(p, &d_counter, stream);
+	if (e != cudaSuccess) return e;
 	CUtensorMap tm_ref, tm_tars;
 	memset(&tm_ref, 0, sizeof(tm_ref));
 	memset(&tm_tars, 0, sizeof(tm_tars));
 	const int dims[3] = { img.w, img.h, n_frames };
 	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[3] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry), 1 };
-	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tars, img.tar, 3, dims, box_tar);
+	const int use_tma = tma_enabled() && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tars, img.tar, 3, dims, box_tar);
 	Icgn2dSeriesKernel kern = p.wpp == 2 ? icgn2d_series_pick<2>(np, p.rc) : icgn2d_series_pick<1>(np, p.rc);
-	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
-	if (*err != cudaSuccess) return -2;
-	kern<<<p.grid, p.wpp * 32, p.smem, stream>>>(img, d_seeds, d_out, n_frames, (int)n, rx, ry, conv, stop, g.counter, tm_ref, tm_tars, use_tma);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return launch_smem(kern, p.grid, p.wpp * 32, p.smem, stream, img, d_seeds, d_out, n_frames, (int)n, rx, ry, conv, stop, d_counter, tm_ref,
+		tm_tars, use_tma);
 }
 
 } // namespace ocb

@@ -73,11 +73,13 @@ __global__ void prefilter3d_kernel(const float* __restrict__ in, float* __restri
 	}
 }
 
-void gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s) {
+cudaError_t gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s) {
 	gradient3d_kernel<<<sm_count * 8, 256, 0, s>>>(ref, rg, dx, dy, dz);
+	return cudaGetLastError();
 }
-void prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s) {
+cudaError_t prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s) {
 	prefilter3d_kernel<<<sm_count * 8, 256, 0, s>>>(in, out, dx, dy, dz, axis);
+	return cudaGetLastError();
 }
 
 // ---- ICGN3D1::compute (NP3, NSETUP, Icgn3dShared, tile extents and launch plan: ocb_kernels.h) ---------------------------
@@ -754,32 +756,24 @@ static Icgn3dKernel icgn3d1_kernel_for(int setup) {
 	return icgn3d1_kernel<RC, THREADS>;
 }
 
-// Returns 0, -1 when even a one-layer slab does not fit in shared memory, -2 on a CUDA error.
-int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop, int sm_count, size_t smem_optin,
-	int* d_counter, cudaStream_t stream, cudaError_t* err, int setup, float* setup_cache) {
-	Icgn3dPlan plan;
-	if (!icgn3d1_plan(rx, ry, rz, smem_optin, &plan)) return -1;
+cudaError_t icgn3d1_launch(const Icgn3dPlan& plan, const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop,
+	int sm_count, int* d_counter, cudaStream_t stream, int setup, float* setup_cache) {
 	const int slab_k = plan.slab_k;
-	const size_t smem = plan.smem;
 	CUtensorMap tm;
 	memset(&tm, 0, sizeof(tm));
 	const int dims[3] = { img.dx, img.dy, img.dz };
 	const int box[3] = { icgn3d_tile_x(rx), icgn3d_tile_y(ry), icgn3d_tile_z(slab_k) };
-	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm, img.coef, 3, dims, box);
+	const int use_tma = tma_enabled() && tma_make_map(&tm, img.coef, 3, dims, box);
 	Icgn3dKernel kern;
-	const int threads = plan.threads;
 	if (plan.threads == 512) kern = plan.rc == 30 ? icgn3d1_kernel_for<30, 512>(setup) : icgn3d1_kernel_for<0, 512>(setup);
 	else kern = plan.rc == 16 ? icgn3d1_kernel_for<16, 256>(setup) : icgn3d1_kernel_for<0, 256>(setup);
-	*err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-	if (*err != cudaSuccess) return -2;
-	*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
-	if (*err != cudaSuccess) return -2;
+	const cudaError_t e = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
+	if (e != cudaSuccess) return e;
 	long long grid = (long long)sm_count * plan.ctas_per_sm;
 	if (grid > (long long)n) grid = (long long)n;
 	if (grid < 1) grid = 1;
-	kern<<<(int)grid, threads, smem, stream>>>(img, d_pois, (int)n, rx, ry, rz, conv, stop, slab_k, d_counter, tm, use_tma, setup_cache);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return launch_smem(kern, (int)grid, plan.threads, plan.smem, stream, img, d_pois, (int)n, rx, ry, rz, conv, stop, slab_k, d_counter, tm, use_tma,
+		setup_cache);
 }
 
 } // namespace ocb

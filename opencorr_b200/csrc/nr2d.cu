@@ -375,27 +375,20 @@ __global__ void __launch_bounds__(128) nr2d1_kernel(Image2D img, float* __restri
 	}
 }
 
-// Returns 0, -1 when one warp's slab does not fit in shared memory, -2 on a CUDA error.
-int nr2d1_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count, size_t smem_optin,
-	int* d_counter, cudaStream_t stream, cudaError_t* err) {
-	Nr2dPlan p;
-	if (!nr2d1_plan(rx, ry, smem_optin, &p)) return -1;
+cudaError_t nr2d1_launch(const Nr2dPlan& p, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
+	int* d_counter, cudaStream_t stream) {
 	CUtensorMap tm_tar;
 	memset(&tm_tar, 0, sizeof(tm_tar));
 	const int dims[2] = { img.w, img.h };
 	const int box_tar[2] = { nr2d_tar_w(rx), nr2d_tar_h(ry) };
-	const int use_tma = !getenv("OCB_NO_TMA") && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
-	*err = cudaFuncSetAttribute(nr2d1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
-	if (*err != cudaSuccess) return -2;
-	*err = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
-	if (*err != cudaSuccess) return -2;
+	const int use_tma = tma_enabled() && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
+	const cudaError_t e = cudaMemsetAsync(d_counter, 0, sizeof(int), stream);
+	if (e != cudaSuccess) return e;
 	long long blocks_needed = ((long long)n + p.warps_per_cta - 1) / p.warps_per_cta;
 	long long resident = (long long)sm_count * p.ctas_per_sm;
 	int grid = (int)(blocks_needed < resident ? blocks_needed : resident);
 	if (grid < 1) grid = 1;
-	nr2d1_kernel<<<grid, p.warps_per_cta * 32, p.smem, stream>>>(img, d_pois, (int)n, rx, ry, conv, stop, d_counter, tm_tar, use_tma);
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return launch_smem(nr2d1_kernel, grid, p.warps_per_cta * 32, p.smem, stream, img, d_pois, (int)n, rx, ry, conv, stop, d_counter, tm_tar, use_tma);
 }
 
 } // namespace ocb

@@ -10,6 +10,19 @@
 
 namespace ocb {
 
+// Every *_launch below enqueues its kernels on `stream` and returns the first CUDA error among its attribute set, work-counter
+// reset, copies and launches, or cudaSuccess.  It runs the plan it is given: whether a call is supported is decided by the
+// caller, which makes the plan (ocb_api.cu, *_plan_or_error).
+
+// kern<<<grid, block, smem, stream>>>(args...) with smem bytes of dynamic shared memory allowed first (beyond the default 48 KB)
+template <class K, class... A>
+inline cudaError_t launch_smem(K kern, int grid, int block, size_t smem, cudaStream_t stream, A... args) {
+	const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	if (e != cudaSuccess) return e;
+	kern<<<grid, block, smem, stream>>>(args...);
+	return cudaGetLastError();
+}
+
 // Factorisation of one FFT axis into Stockham stages (radix 4/2/3/5, generic odd radix <= 31).
 struct FftAxis {
 	int n;
@@ -112,20 +125,15 @@ inline bool icgn2d_plan(size_t n, int np, int rx, int ry, bool lm, int sm_count,
 	return true;
 }
 
-// plan_n: the queue length whose warps per POI the launch takes (icgn2d_plan); n for a plain call.  A re-seeded sub-queue passes
-// the length of the whole queue, so that its POIs split their sums as they do in the launch over all of them.
-int icgn2d_launch(int np, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
-	size_t smem_optin, int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream, cudaError_t* err,
-	size_t plan_n);
-size_t icgn2d_slab_bytes(int rx, int ry); // shared memory one POI needs (plain IC-GN, one warp per POI)
-// whether a plain IC-GN launch over n POIs (icgn2d_launch, icgn2d_series_launch) has a plan for radius (rx, ry): false where they
-// would return -1
-bool icgn2d_fits(size_t n, int np, int rx, int ry, int sm_count, size_t smem_optin);
+// plan: icgn2d_plan for the call's order, radii and IC-LM flag (lm_damping non-null), its grid at most n.  d_counter: the context's
+// work-queue heads (64 ints; see ocb_create).
+cudaError_t icgn2d_launch(int np, const Icgn2dPlan& plan, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop,
+	int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream);
 // one reference (img.ref) against the frame-major stack img.tar [n_frames][h][w]: n seeds in, n_frames x n records out (frame-major)
-int icgn2d_series_launch(int np, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry, float conv, float stop,
-	int sm_count, size_t smem_optin, int* d_counter, cudaStream_t stream, cudaError_t* err, size_t plan_n);
+cudaError_t icgn2d_series_launch(int np, const Icgn2dPlan& plan, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n,
+	int rx, int ry, float conv, float stop, int* d_counter, cudaStream_t stream);
 // series_reseed.cu: the lost-POI scan, compaction, rebuild and scatter of the re-seeding series calls (dim: 2 or 3; records
-// frame-major, out[f * n + i]).  Each returns the launch's CUDA error.
+// frame-major, out[f * n + i]).
 // scan: for the POIs idx[0..m) (0..m when idx is null), first[i] = the first frame in [f_begin, f_end) with !(zncc >= zncc_min), or
 // -1; hist[f] += the POIs whose first lost frame is f.
 cudaError_t reseed_scan_launch(int dim, const float* d_out, size_t n, int f_begin, int f_end, const int* d_idx, size_t m, float zncc_min, int* d_first,
@@ -178,18 +186,19 @@ inline bool nr2d1_plan(int rx, int ry, size_t smem_optin, Nr2dPlan* p) {
 	p->smem = per_warp * best_wpb;
 	return true;
 }
-int nr2d1_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count, size_t smem_optin,
-	int* d_counter, cudaStream_t stream, cudaError_t* err);
+cudaError_t nr2d1_launch(const Nr2dPlan& plan, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
+	int* d_counter, cudaStream_t stream);
 // epipolar.cu
 int epipolar_slots(int search_radius, int search_step);
-void epipolar_candidates_launch(const float* d_pois, size_t poi0, size_t n_poi, const float* fundamental, const float* parallax_x,
+cudaError_t epipolar_candidates_launch(const float* d_pois, size_t poi0, size_t n_poi, const float* fundamental, const float* parallax_x,
 	const float* parallax_y, int search_radius, int search_step, int rx, int ry, int w, int h, int slots, float* d_cand, int sm_count,
 	cudaStream_t stream);
-void epipolar_select_launch(float* d_pois, size_t poi0, size_t n_poi, int slots, const float* d_cand, int sm_count, cudaStream_t stream);
+cudaError_t epipolar_select_launch(float* d_pois, size_t poi0, size_t n_poi, int slots, const float* d_cand, int sm_count, cudaStream_t stream);
 // strain.cu
 size_t strain_workspace_bytes(size_t n);
-int strain_launch(int dim, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only, void* workspace,
-	int sm_count, cudaStream_t stream, cudaError_t* err, long long* launches);
+// *launches grows by the kernels it launched
+cudaError_t strain_launch(int dim, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only,
+	void* workspace, int sm_count, cudaStream_t stream, long long* launches);
 // FFTCC2D: which of the three kernels a window takes, and what that kernel needs
 constexpr int FFTW32_WARPS = 4;     // fftcc2d_w32.cu: one-POI warps per CTA
 constexpr int FFTREG_THREADS = 128; // fftcc2d_reg.cu: one thread per window row, 128 / N POIs per CTA
@@ -269,12 +278,12 @@ inline bool fftcc2d_plan(int rx, int ry, bool force_generic, size_t smem_optin, 
 }
 
 // fftcc.cu
-int fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const Fftcc2dPlan& plan, const float2* tw_x,
-	const float2* tw_y, int grid, cudaStream_t stream, cudaError_t* err);
+cudaError_t fftcc2d_launch(const Image2D& img, float* d_pois, size_t n, int rx, int ry, const Fftcc2dPlan& plan, const float2* tw_x,
+	const float2* tw_y, int grid, cudaStream_t stream);
 // fftcc2d_w32.cu (32x32 window, one warp per POI, register FFT)
-int fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int grid, cudaStream_t stream, cudaError_t* err);
+cudaError_t fftcc2d_w32_launch(const Image2D& img, float* d_pois, size_t n, int grid, cudaStream_t stream);
 // fftcc2d_reg.cu (square windows of 2^a 3^b 5^c <= 64 points, one thread per row, register FFT codelets)
-int fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int grid, cudaStream_t stream, cudaError_t* err);
+cudaError_t fftcc2d_reg_launch(const Image2D& img, float* d_pois, size_t n, int r, const Fftcc2dPlan& plan, int grid, cudaStream_t stream);
 // FFTCC3D: which of the three kernels a window takes, and what that kernel needs
 constexpr int F3_WARPS = 8;        // fftcc3d_w32.cu: warps of the one-POI CTA
 // fftcc3d_w32.cu: two tiles per warp, each a TMA box (36 x 32 floats) or a padded transpose tile (32 x 33)
@@ -341,14 +350,14 @@ inline bool fftcc3d_plan(int rx, int ry, int rz, bool force_generic, size_t smem
 }
 
 // fftcc3d_reg.cu (cubic windows of 2^a 3^b 5^c <= 64 points, one thread per 1D transform, register FFT codelets)
-int fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
-	cudaError_t* err);
+cudaError_t fftcc3d_reg_launch(const Image3D& img, float* d_pois, size_t n_poi, const Fftcc3dPlan& plan, float2* scratch, int grid,
+	cudaStream_t stream);
 // fftcc.cu
-int fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const Fftcc3dPlan& plan, const float2* tw_x,
-	const float2* tw_y, const float2* tw_z, float2* scratch, int grid, cudaStream_t stream, cudaError_t* err);
+cudaError_t fftcc3d_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, const Fftcc3dPlan& plan, const float2* tw_x,
+	const float2* tw_y, const float2* tw_z, float2* scratch, int grid, cudaStream_t stream);
 // fftcc3d_w32.cu (32^3 window, register FFTs)
-int fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid, cudaStream_t stream,
-	cudaError_t* err);
+cudaError_t fftcc3d_w32_launch(const Image3D& img, float* d_pois, size_t n, const Fftcc3dPlan& plan, float2* scratch, int grid,
+	cudaStream_t stream);
 // icgn3d.cu
 constexpr int ICGN3D_MAX_WARPS = 16; // CTAs run 8 warps (two CTAs per SM) or, when only one slab-carrying CTA fits, 16
 constexpr int NP3 = 12;
@@ -426,21 +435,21 @@ struct StereoCam {
 	const float* intrinsics; // host pointer, 13 floats
 	const float* projection; // host pointer, 3x4 row-major
 };
-void calib_map_launch(const float* intrinsics, int height, int width, float convergence, int iteration, float* d_map_x, float* d_map_y,
+cudaError_t calib_map_launch(const float* intrinsics, int height, int width, float convergence, int iteration, float* d_map_x, float* d_map_y,
 	cudaStream_t stream);
-void calib_undistort_launch(const float* d_map_x, const float* d_map_y, int height, int width, const float* intrinsics, float* d_pts, float* d_out,
+cudaError_t calib_undistort_launch(const float* d_map_x, const float* d_map_y, int height, int width, const float* intrinsics, float* d_pts, float* d_out,
 	size_t n, cudaStream_t stream);
-void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
+cudaError_t stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
 	cudaStream_t stream);
 // the POI2DS records of a stereo series (ocb_stereo_series): n_frames x n, frame-major, from the r1 -> r2 records d_stereo (n), the
 // view-1 seeds (n, for x and y) and the two registrations d_out1, d_out2 (n_frames x n POI2D each)
-void stereo_poi2ds_launch(const StereoCam& c1, const StereoCam& c2, const float* d_stereo, const float* d_seeds1, const float* d_out1,
+cudaError_t stereo_poi2ds_launch(const StereoCam& c1, const StereoCam& c2, const float* d_stereo, const float* d_seeds1, const float* d_out1,
 	const float* d_out2, float* d_out2ds, size_t n, int n_frames, cudaStream_t stream);
 
-void gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s);
-void prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s);
+cudaError_t gradient3d_launch(const float* ref, float4* rg, int dx, int dy, int dz, int sm_count, cudaStream_t s);
+cudaError_t prefilter3d_launch(const float* in, float* out, int dx, int dy, int dz, int axis, int sm_count, cudaStream_t s);
 // setup: an Icgn3dSetup; STORE and LOAD need setup_cache, n x ICGN3D_SETUP_FLOATS floats indexed by queue position
-int icgn3d1_launch(const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop, int sm_count, size_t smem_optin,
-	int* d_counter, cudaStream_t stream, cudaError_t* err, int setup = ICGN3D_SETUP_COMPUTE, float* setup_cache = nullptr);
+cudaError_t icgn3d1_launch(const Icgn3dPlan& plan, const Image3D& img, float* d_pois, size_t n, int rx, int ry, int rz, float conv, float stop,
+	int sm_count, int* d_counter, cudaStream_t stream, int setup = ICGN3D_SETUP_COMPUTE, float* setup_cache = nullptr);
 
 } // namespace ocb

@@ -6,6 +6,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdlib.h>
 
 namespace ocb {
 
@@ -61,6 +62,10 @@ inline EncodeTiledFn tma_encode_fn() {
 	}
 	return fn;
 }
+
+// false when OCB_NO_TMA is set: every launch then stages its tiles with ordinary loads.  Read at each launch, so that a
+// process can switch between the two load paths.
+inline bool tma_enabled() { return !getenv("OCB_NO_TMA"); }
 
 // Tensor map over a dense row-major f32 array of rank 2 or 3 (dims[0] = innermost) for box-shaped tile
 // loads.  Returns false when TMA cannot be used: pitch or base not 16-byte aligned, a box extent > 256,

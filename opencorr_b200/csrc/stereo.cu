@@ -280,16 +280,18 @@ __global__ void __launch_bounds__(256) stereo_poi2ds_kernel(StereoView v1, Stere
 
 static unsigned int blocks_for(long long n) { return (unsigned int)((n + 255) / 256); }
 
-void calib_map_launch(const float* intrinsics, int height, int width, float convergence, int iteration, float* d_map_x, float* d_map_y,
+cudaError_t calib_map_launch(const float* intrinsics, int height, int width, float convergence, int iteration, float* d_map_x, float* d_map_y,
 	cudaStream_t stream) {
 	calib_map_kernel<<<blocks_for((long long)height * width), 256, 0, stream>>>(load_intrinsics(intrinsics), height, width, convergence, iteration,
 		d_map_x, d_map_y);
+	return cudaGetLastError();
 }
 
-void calib_undistort_launch(const float* d_map_x, const float* d_map_y, int height, int width, const float* intrinsics, float* d_pts, float* d_out,
+cudaError_t calib_undistort_launch(const float* d_map_x, const float* d_map_y, int height, int width, const float* intrinsics, float* d_pts, float* d_out,
 	size_t n, cudaStream_t stream) {
 	calib_undistort_kernel<<<blocks_for((long long)n), 256, 0, stream>>>(d_map_x, d_map_y, height, width, load_intrinsics(intrinsics),
 		(float2*)d_pts, (float2*)d_out, (long long)n);
+	return cudaGetLastError();
 }
 
 static void stereo_views(const StereoCam& c1, const StereoCam& c2, StereoView* v) {
@@ -304,19 +306,21 @@ static void stereo_views(const StereoCam& c1, const StereoCam& c2, StereoView* v
 	}
 }
 
-void stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
+cudaError_t stereo_reconstruct_launch(const StereoCam& c1, const StereoCam& c2, float* d_pts1, float* d_pts2, float* d_pts3d, size_t n,
 	cudaStream_t stream) {
 	StereoView v[2];
 	stereo_views(c1, c2, v);
 	stereo_reconstruct_kernel<<<blocks_for((long long)n), 256, 0, stream>>>(v[0], v[1], (float2*)d_pts1, (float2*)d_pts2, d_pts3d, (long long)n);
+	return cudaGetLastError();
 }
 
-void stereo_poi2ds_launch(const StereoCam& c1, const StereoCam& c2, const float* d_stereo, const float* d_seeds1, const float* d_out1,
+cudaError_t stereo_poi2ds_launch(const StereoCam& c1, const StereoCam& c2, const float* d_stereo, const float* d_seeds1, const float* d_out1,
 	const float* d_out2, float* d_out2ds, size_t n, int n_frames, cudaStream_t stream) {
 	StereoView v[2];
 	stereo_views(c1, c2, v);
 	const long long total = (long long)n * n_frames;
 	stereo_poi2ds_kernel<<<blocks_for(total), 256, 0, stream>>>(v[0], v[1], d_stereo, d_seeds1, d_out1, d_out2, d_out2ds, (long long)n, total);
+	return cudaGetLastError();
 }
 
 } // namespace ocb

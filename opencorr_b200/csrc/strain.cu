@@ -389,10 +389,9 @@ size_t strain_workspace_bytes(size_t n) {
 	return 256 + 4 * align256(n * 4) + 3 * align256(n * 16) + align256(cub_bytes) + 256;
 }
 
-// Returns 0 on success, -2 on a CUDA error.  *launches is incremented by the number of kernels launched.
 // mode: 2 (POI2D records), 3 (POI3D), 23 (POI2DS)
-int strain_launch(int mode, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only, void* workspace,
-	int sm_count, cudaStream_t stream, cudaError_t* err, long long* launches) {
+cudaError_t strain_launch(int mode, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only,
+	void* workspace, int sm_count, cudaStream_t stream, long long* launches) {
 	char* ws = (char*)workspace;
 	unsigned int* d_bbox = (unsigned int*)ws; ws += 256;
 	unsigned int* keys_in = (unsigned int*)ws; ws += align256(n * 4);
@@ -412,16 +411,17 @@ int strain_launch(int mode, float* d_pois, size_t n, float radius, int k_min, fl
 	if (blocks > sm_count * 8) blocks = sm_count * 8;
 	if (blocks < 1) blocks = 1;
 
+	cudaError_t e;
 	const unsigned int init[6] = { 0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u };
-	if ((*err = cudaMemcpyAsync(d_bbox, init, sizeof(init), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return -2;
+	if ((e = cudaMemcpyAsync(d_bbox, init, sizeof(init), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
 	if (mode == 2) strain_bbox_kernel<2><<<blocks, threads, 0, stream>>>(d_pois, (int)n, d_bbox);
 	else if (mode == 3) strain_bbox_kernel<3><<<blocks, threads, 0, stream>>>(d_pois, (int)n, d_bbox);
 	else strain_bbox_kernel<23><<<blocks, threads, 0, stream>>>(d_pois, (int)n, d_bbox);
 	unsigned int hb[6];
-	if ((*err = cudaMemcpyAsync(hb, d_bbox, sizeof(hb), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return -2;
-	if ((*err = cudaStreamSynchronize(stream)) != cudaSuccess) return -2;
+	if ((e = cudaMemcpyAsync(hb, d_bbox, sizeof(hb), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+	if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
 	(*launches)++;
-	if (hb[0] == 0xffffffffu && hb[3] == 0u) return 0; // no POI with finite coordinates
+	if (hb[0] == 0xffffffffu && hb[3] == 0u) return cudaSuccess; // no POI with finite coordinates
 
 	StrainGrid g;
 	float extent = 0.f;
@@ -456,8 +456,8 @@ int strain_launch(int mode, float* d_pois, size_t n, float radius, int k_min, fl
 	else strain_keys_kernel<23><<<blocks, threads, 0, stream>>>(d_pois, (int)n, g, keys_in, vals_in);
 	int end_bit = 1;
 	while (end_bit < 32 && (g.n_cells >> end_bit) != 0) end_bit++;
-	if ((*err = cub::DeviceRadixSort::SortPairs(cub_temp, cub_bytes, keys_in, keys_out, vals_in, vals_out, (int)n, 0, end_bit, stream)) != cudaSuccess)
-		return -2;
+	if ((e = cub::DeviceRadixSort::SortPairs(cub_temp, cub_bytes, keys_in, keys_out, vals_in, vals_out, (int)n, 0, end_bit, stream)) != cudaSuccess)
+		return e;
 	if (mode == 2) strain_gather_kernel<2><<<blocks, threads, 0, stream>>>(d_pois, (int)n, vals_out, zncc_threshold, pos, disp, fpos);
 	else if (mode == 3) strain_gather_kernel<3><<<blocks, threads, 0, stream>>>(d_pois, (int)n, vals_out, zncc_threshold, pos, disp, fpos);
 	else strain_gather_kernel<23><<<blocks, threads, 0, stream>>>(d_pois, (int)n, vals_out, zncc_threshold, pos, disp, fpos);
@@ -466,11 +466,11 @@ int strain_launch(int mode, float* d_pois, size_t n, float radius, int k_min, fl
 	int n_valid = (int)n;
 	{
 		unsigned int last = 0;
-		if ((*err = cudaMemcpyAsync(&last, keys_out + (n - 1), sizeof(last), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return -2;
-		if ((*err = cudaStreamSynchronize(stream)) != cudaSuccess) return -2;
+		if ((e = cudaMemcpyAsync(&last, keys_out + (n - 1), sizeof(last), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+		if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
 		if (last == g.n_cells) { // rare: find the first sentinel on the host
 			std::vector<unsigned int> hk(n);
-			if ((*err = cudaMemcpy(hk.data(), keys_out, n * sizeof(unsigned int), cudaMemcpyDeviceToHost)) != cudaSuccess) return -2;
+			if ((e = cudaMemcpy(hk.data(), keys_out, n * sizeof(unsigned int), cudaMemcpyDeviceToHost)) != cudaSuccess) return e;
 			n_valid = (int)(std::lower_bound(hk.begin(), hk.end(), g.n_cells) - hk.begin());
 		}
 	}
@@ -488,8 +488,7 @@ int strain_launch(int mode, float* d_pois, size_t n, float radius, int k_min, fl
 				(int)only);
 		(*launches)++;
 	}
-	*err = cudaGetLastError();
-	return *err == cudaSuccess ? 0 : -2;
+	return cudaGetLastError();
 }
 
 } // namespace ocb
