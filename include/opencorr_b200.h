@@ -243,6 +243,42 @@ int ocb_nr2d_prepare(ocb_ctx* ctx);
 int ocb_nr2d1(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry, float conv, float stop);
 int ocb_nr2d1_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry, float conv, float stop);
 
+/* ---- IC-LM over an image series.  Replaces the loop a reference user writes over a load series with an IC-LM method:
+ *        for f: dic.setImages(ref, tar[f]); iclm.prepare(); iclm.compute(queue)
+ *               (ICLM2D1::compute(std::vector<POI2D>&) src/oc_iclm.cpp:360-368, ICLM2D2 :732-740)
+ *      over the series set by ocb_set_series_2d*.  Frame f's records are, bit for bit, what ocb_iclm2d gives on (ref, tars[f])
+ *      with the same damping for frame f - 1's records (frame 0: the seeds) in one launch over the same n POIs (OCB_ICGN2D_WPP,
+ *      the warps per POI, as for ocb_icgn2d_series).  Each POI's reference subset and undamped Hessian are built once for the
+ *      whole series; the damping restarts from lambda in every frame, as a pair call does.  lambda, alpha, beta as for
+ *      ocb_iclm2d, passed through unchecked.  Everything else (order, seeds, out, chunking, _dev borrowing, group contexts,
+ *      errors) as for ocb_icgn2d_series; the _reseed variants follow ocb_icgn2d_series_reseed's rules 1-5 with IC-LM (the same
+ *      damping) in place of IC-GN. */
+int ocb_iclm2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, float lambda,
+	float alpha, float beta);
+int ocb_iclm2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop, float lambda,
+	float alpha, float beta);
+int ocb_iclm2d_series_reseed(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, float lambda,
+	float alpha, float beta, int fft_rx, int fft_ry, float zncc_min, size_t* reseeded);
+int ocb_iclm2d_series_reseed_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
+	float lambda, float alpha, float beta, int fft_rx, int fft_ry, float zncc_min, size_t* reseeded);
+
+/* ---- NR2D1 over an image series.  Replaces the loop a reference user writes over a load series with NR2D1:
+ *        for f: dic.setImages(ref, tar[f]); nr.prepare() (NR2D1::prepare src/oc_nr.cpp:119-156);
+ *               nr.compute(queue) (NR2D1::compute(std::vector<POI2D>&) :327-334)
+ *      over the series set by ocb_set_series_2d*.  Frame f's records are, bit for bit, what ocb_nr2d1 gives on (ref, tars[f])
+ *      for frame f - 1's records (frame 0: the seeds).  A POI that fails the guard gets the pair call's code in each later
+ *      frame too: -1, or -4 / -5 from the tests NR2D1 runs on every record, so its code can change from frame to frame.  Each
+ *      POI's reference subset is staged once for the whole series; the target gradients are rebuilt in every frame.
+ *      No order argument; everything else (seeds, out, chunking, _dev borrowing, group contexts, errors) as for
+ *      ocb_icgn2d_series, with the radius refused as by ocb_nr2d1; the _reseed variants follow ocb_icgn2d_series_reseed's
+ *      rules 1-5 with NR2D1 in place of IC-GN. */
+int ocb_nr2d1_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop);
+int ocb_nr2d1_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop);
+int ocb_nr2d1_series_reseed(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, int fft_rx, int fft_ry,
+	float zncc_min, size_t* reseeded);
+int ocb_nr2d1_series_reseed_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop, int fft_rx,
+	int fft_ry, float zncc_min, size_t* reseeded);
+
 /* ---- EpipolarSearch (SURVEY.md section 8(f) N4): EpipolarSearch::compute(std::vector<POI2D>&) src/oc_epipolar_search.cpp:197-205
  *      (per POI :133-195) as one batch: every POI spawns its candidates along the epipolar line of the secondary view
  *      (centre + every search_step pixels in x below search_radius, both directions), ICGN2D1(rx, ry, conv, stop) registers

@@ -73,6 +73,14 @@ SIGNATURES = {
     "ocb_icgn3d_series_reseed_dev": (_i, [_vp, _vp, _vp, _sz, _i, _i, _i, _f, _f, _i, _i, _i, _f, _vp]),
     "ocb_iclm2d": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
     "ocb_iclm2d_dev": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
+    "ocb_iclm2d_series": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
+    "ocb_iclm2d_series_dev": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f, _f, _f, _f]),
+    "ocb_iclm2d_series_reseed": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f, _f, _f, _f, _i, _i, _f, _vp]),
+    "ocb_iclm2d_series_reseed_dev": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f, _f, _f, _f, _i, _i, _f, _vp]),
+    "ocb_nr2d1_series": (_i, [_vp, _vp, _vp, _sz, _i, _i, _f, _f]),
+    "ocb_nr2d1_series_dev": (_i, [_vp, _vp, _vp, _sz, _i, _i, _f, _f]),
+    "ocb_nr2d1_series_reseed": (_i, [_vp, _vp, _vp, _sz, _i, _i, _f, _f, _i, _i, _f, _vp]),
+    "ocb_nr2d1_series_reseed_dev": (_i, [_vp, _vp, _vp, _sz, _i, _i, _f, _f, _i, _i, _f, _vp]),
     "ocb_epipolar_search2d": (_i, [_vp, _vp, _sz, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f]),
     "ocb_epipolar_search2d_dev": (_i, [_vp, _vp, _sz, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f]),
     "ocb_strain2d": (_i, [_vp, _vp, _sz, _f, _i, _f, _i]),

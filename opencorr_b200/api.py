@@ -265,6 +265,47 @@ class Engine:
                                                     int(fft_ry), float(zncc_min), _vp(counts)))
         return out, counts.astype(np.int64)
 
+    def iclm2d_series(self, order, seeds, rx, ry, conv, stop, damping=(100.0, 0.1, 10.0)):
+        """ICLM2D1 (order 1) / ICLM2D2 (order 2) over the series set by set_series_2d, frame f seeded by frame f - 1's records
+        (frame 0 by `seeds`, [n, 25]); damping = (lambda, alpha, beta), restarted in every frame.  Returns the records of every
+        frame, float32 (F, n, 25); seeds are not changed."""
+        _check_queue(seeds, POI2D_FLOATS)
+        out = np.empty((self._series_frames("2d", "iclm2d_series"), seeds.shape[0], POI2D_FLOATS), np.float32)
+        self._ck(self._lib.ocb_iclm2d_series(self._ctx, int(order), _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop, float(damping[0]),
+                                             float(damping[1]), float(damping[2])))
+        return out
+
+    def iclm2d_series_reseed(self, order, seeds, rx, ry, conv, stop, fft_rx, fft_ry, zncc_min, damping=(100.0, 0.1, 10.0)):
+        """iclm2d_series that re-seeds lost POIs with FFTCC2D and IC-LM in the frame where they are lost (see
+        icgn2d_series_reseed).  Returns (records float32 (F, n, 25), reseeded int64 (F,))."""
+        _check_queue(seeds, POI2D_FLOATS)
+        n_frames = self._series_frames("2d", "iclm2d_series_reseed")
+        out = np.empty((n_frames, seeds.shape[0], POI2D_FLOATS), np.float32)
+        counts = np.zeros(n_frames, np.uint64)
+        self._ck(self._lib.ocb_iclm2d_series_reseed(self._ctx, int(order), _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop,
+                                                    float(damping[0]), float(damping[1]), float(damping[2]), int(fft_rx), int(fft_ry),
+                                                    float(zncc_min), _vp(counts)))
+        return out, counts.astype(np.int64)
+
+    def nr2d1_series(self, seeds, rx, ry, conv, stop):
+        """NR2D1 over the series set by set_series_2d, frame f seeded by frame f - 1's records (frame 0 by `seeds`, [n, 25]).
+        Returns the records of every frame, float32 (F, n, 25); seeds are not changed."""
+        _check_queue(seeds, POI2D_FLOATS)
+        out = np.empty((self._series_frames("2d", "nr2d1_series"), seeds.shape[0], POI2D_FLOATS), np.float32)
+        self._ck(self._lib.ocb_nr2d1_series(self._ctx, _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop))
+        return out
+
+    def nr2d1_series_reseed(self, seeds, rx, ry, conv, stop, fft_rx, fft_ry, zncc_min):
+        """nr2d1_series that re-seeds lost POIs with FFTCC2D and NR2D1 in the frame where they are lost (see
+        icgn2d_series_reseed).  Returns (records float32 (F, n, 25), reseeded int64 (F,))."""
+        _check_queue(seeds, POI2D_FLOATS)
+        n_frames = self._series_frames("2d", "nr2d1_series_reseed")
+        out = np.empty((n_frames, seeds.shape[0], POI2D_FLOATS), np.float32)
+        counts = np.zeros(n_frames, np.uint64)
+        self._ck(self._lib.ocb_nr2d1_series_reseed(self._ctx, _vp(seeds), _vp(out), seeds.shape[0], rx, ry, conv, stop, int(fft_rx), int(fft_ry),
+                                                   float(zncc_min), _vp(counts)))
+        return out, counts.astype(np.int64)
+
     def icgn3d_series_reseed(self, seeds, rx, ry, rz, conv, stop, fft_rx, fft_ry, fft_rz, zncc_min):
         """icgn3d_series that re-seeds lost POIs with FFTCC3D (radii fft_rx, fft_ry, fft_rz) in the frame where they are lost (see
         icgn2d_series_reseed).  Returns (records float32 (F, n, 31), reseeded int64 (F,))."""
@@ -378,6 +419,30 @@ class Engine:
         counts = np.zeros(self._series_frames("2d", "icgn2d_series_reseed"), np.uint64)
         self._ck(self._lib.ocb_icgn2d_series_reseed_dev(self._ctx, int(order), int(d_seeds), int(d_out), n, rx, ry, conv, stop, int(fft_rx), int(fft_ry),
                                                         float(zncc_min), _vp(counts)))
+        return counts.astype(np.int64)
+
+    def iclm2d_series_dev(self, order, d_seeds, d_out, n, rx, ry, conv, stop, damping=(100.0, 0.1, 10.0)):
+        """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
+        self._ck(self._lib.ocb_iclm2d_series_dev(self._ctx, int(order), int(d_seeds), int(d_out), n, rx, ry, conv, stop, float(damping[0]),
+                                                 float(damping[1]), float(damping[2])))
+
+    def iclm2d_series_reseed_dev(self, order, d_seeds, d_out, n, rx, ry, conv, stop, fft_rx, fft_ry, zncc_min, damping=(100.0, 0.1, 10.0)):
+        """iclm2d_series_reseed on device pointers; synchronises the stream.  Returns reseeded, int64 (F,)."""
+        counts = np.zeros(self._series_frames("2d", "iclm2d_series_reseed"), np.uint64)
+        self._ck(self._lib.ocb_iclm2d_series_reseed_dev(self._ctx, int(order), int(d_seeds), int(d_out), n, rx, ry, conv, stop, float(damping[0]),
+                                                        float(damping[1]), float(damping[2]), int(fft_rx), int(fft_ry), float(zncc_min),
+                                                        _vp(counts)))
+        return counts.astype(np.int64)
+
+    def nr2d1_series_dev(self, d_seeds, d_out, n, rx, ry, conv, stop):
+        """n seed records in, n_frames x n records out (frame-major), device pointers; enqueue only."""
+        self._ck(self._lib.ocb_nr2d1_series_dev(self._ctx, int(d_seeds), int(d_out), n, rx, ry, conv, stop))
+
+    def nr2d1_series_reseed_dev(self, d_seeds, d_out, n, rx, ry, conv, stop, fft_rx, fft_ry, zncc_min):
+        """nr2d1_series_reseed on device pointers; synchronises the stream.  Returns reseeded, int64 (F,)."""
+        counts = np.zeros(self._series_frames("2d", "nr2d1_series_reseed"), np.uint64)
+        self._ck(self._lib.ocb_nr2d1_series_reseed_dev(self._ctx, int(d_seeds), int(d_out), n, rx, ry, conv, stop, int(fft_rx), int(fft_ry),
+                                                       float(zncc_min), _vp(counts)))
         return counts.astype(np.int64)
 
     def icgn3d1_dev(self, d_q, n, rx, ry, rz, conv, stop):

@@ -557,7 +557,8 @@ __device__ __noinline__ bool icgn2d_exact_negative(const float* Aw, float pcx, f
 // SERIES: one reference against n_frames targets (img.tar is the frame-major stack [n_frames][h][w], tm_tar a 3D map over it).
 // A POI's setup pass runs once; each frame then runs the same guard, target staging, iterations and result code as a pair
 // call, seeded by the previous frame's record, which stays in registers.  Every frame's record is stored whole to
-// frames_out[f n_poi + poi]; `pois` holds the seeds and is only read.
+// frames_out[f n_poi + poi]; `pois` holds the seeds and is only read.  LM: what carries over is the undamped Hessian in sH
+// (every iteration damps and factorises a copy of it) and the damping restarts from lm_lambda, as a pair call on the frame does.
 // (the second launch bound keeps the register file from limiting residency below what the slab allows: 16 one-warp CTAs for the
 //  6-parameter kernels of any radius, 12 for the r = 16 specialisation, whose 20 KB slab admits 11)
 __host__ __device__ constexpr int icgn2d_min_ctas(int np, int rc, int wpp) { return np == 6 ? (rc == 16 ? 12 : ICGN2D_MIN_CTAS) / wpp : 7; }
@@ -566,7 +567,6 @@ template <int NP, int RC, bool LM, int WPP, bool SERIES>
 __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__ pois, float* __restrict__ frames_out, int n_frames, int n_poi,
 	int rx_arg, int ry_arg, float conv_criterion, float stop_condition, int* __restrict__ work_counter, const CUtensorMap& tm_ref,
 	const CUtensorMap& tm_tar, int use_tma, const float* __restrict__ center_offsets, float lm_lambda, float lm_alpha, float lm_beta) {
-	static_assert(!(SERIES && LM), "series are IC-GN only");
 	extern __shared__ __align__(128) float smem[];
 	using Warp = std::conditional_t<NP == 6, Warp2D1, Warp2D2>;
 	constexpr int NH = NP * (NP + 1) / 2;
@@ -1135,18 +1135,21 @@ __global__ void __launch_bounds__(32 * WPP, icgn2d_min_ctas(NP, RC, WPP)) icgn2d
 		use_tma, center_offsets, lm_lambda, lm_alpha, lm_beta);
 }
 
-// img.tar: the frame-major target stack; tm_tars: its 3D map (box depth 1)
-template <int NP, int RC, int WPP>
+// img.tar: the frame-major target stack; tm_tars: its 3D map (box depth 1).  The damping comes last, so the IC-GN instantiations
+// see the parameters they had before IC-LM series existed.
+template <int NP, int RC, bool LM, int WPP>
 __global__ void __launch_bounds__(32 * WPP, icgn2d_min_ctas(NP, RC, WPP)) icgn2d_series_kernel(Image2D img, const float* __restrict__ seeds,
 	float* __restrict__ out, int n_frames, int n_poi, int rx_arg, int ry_arg, float conv_criterion, float stop_condition,
-	int* __restrict__ work_counter, const __grid_constant__ CUtensorMap tm_ref, const __grid_constant__ CUtensorMap tm_tars, int use_tma) {
-	icgn2d_poi_loop<NP, RC, false, WPP, true>(img, const_cast<float*>(seeds), out, n_frames, n_poi, rx_arg, ry_arg, conv_criterion, stop_condition,
-		work_counter, tm_ref, tm_tars, use_tma, nullptr, 0.f, 0.f, 0.f);
+	int* __restrict__ work_counter, const __grid_constant__ CUtensorMap tm_ref, const __grid_constant__ CUtensorMap tm_tars, int use_tma,
+	float lm_lambda, float lm_alpha, float lm_beta) {
+	icgn2d_poi_loop<NP, RC, LM, WPP, true>(img, const_cast<float*>(seeds), out, n_frames, n_poi, rx_arg, ry_arg, conv_criterion, stop_condition,
+		work_counter, tm_ref, tm_tars, use_tma, nullptr, lm_lambda, lm_alpha, lm_beta);
 }
 
 // host-side launch ---------------------------------------------------------------------------
 typedef void (*Icgn2dKernel)(Image2D, float*, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int, const float*, float, float, float);
-typedef void (*Icgn2dSeriesKernel)(Image2D, const float*, float*, int, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int);
+typedef void (*Icgn2dSeriesKernel)(Image2D, const float*, float*, int, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int,
+	float, float, float);
 
 template <int WPP>
 static Icgn2dKernel icgn2d_pick(int np, int rc, bool lm) {
@@ -1155,9 +1158,10 @@ static Icgn2dKernel icgn2d_pick(int np, int rc, bool lm) {
 	return rc == 20 ? icgn2d_kernel<12, 20, false, WPP> : icgn2d_kernel<12, 0, false, WPP>;
 }
 template <int WPP>
-static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rc) {
-	if (np == 6) return rc == 16 ? icgn2d_series_kernel<6, 16, WPP> : icgn2d_series_kernel<6, 0, WPP>;
-	return rc == 20 ? icgn2d_series_kernel<12, 20, WPP> : icgn2d_series_kernel<12, 0, WPP>;
+static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rc, bool lm) {
+	if (lm) return (np == 6) ? icgn2d_series_kernel<6, 0, true, WPP> : icgn2d_series_kernel<12, 0, true, WPP>;
+	if (np == 6) return rc == 16 ? icgn2d_series_kernel<6, 16, false, WPP> : icgn2d_series_kernel<6, 0, false, WPP>;
+	return rc == 20 ? icgn2d_series_kernel<12, 20, false, WPP> : icgn2d_series_kernel<12, 0, false, WPP>;
 }
 
 // The work-queue head of a launch: [0] of the context's heads, zeroed here, for two warps per POI; [32] for the one-warp-per-POI
@@ -1187,7 +1191,8 @@ cudaError_t icgn2d_launch(int np, const Icgn2dPlan& p, const Image2D& img, float
 }
 
 cudaError_t icgn2d_series_launch(int np, const Icgn2dPlan& p, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n,
-	int rx, int ry, float conv, float stop, int* d_counter, cudaStream_t stream) {
+	int rx, int ry, float conv, float stop, int* d_counter, const float* lm_damping, cudaStream_t stream) {
+	const bool lm = lm_damping != nullptr;
 	cudaError_t e = icgn2d_counter(p, &d_counter, stream);
 	if (e != cudaSuccess) return e;
 	CUtensorMap tm_ref, tm_tars;
@@ -1196,9 +1201,9 @@ cudaError_t icgn2d_series_launch(int np, const Icgn2dPlan& p, const Image2D& img
 	const int dims[3] = { img.w, img.h, n_frames };
 	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[3] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry), 1 };
 	const int use_tma = tma_enabled() && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tars, img.tar, 3, dims, box_tar);
-	Icgn2dSeriesKernel kern = p.wpp == 2 ? icgn2d_series_pick<2>(np, p.rc) : icgn2d_series_pick<1>(np, p.rc);
+	Icgn2dSeriesKernel kern = p.wpp == 2 ? icgn2d_series_pick<2>(np, p.rc, lm) : icgn2d_series_pick<1>(np, p.rc, lm);
 	return launch_smem(kern, p.grid, p.wpp * 32, p.smem, stream, img, d_seeds, d_out, n_frames, (int)n, rx, ry, conv, stop, d_counter, tm_ref,
-		tm_tars, use_tma);
+		tm_tars, use_tma, lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
 }
 
 } // namespace ocb

@@ -1285,26 +1285,69 @@ static int reseed_gather(ocb_ctx* ctx, int dim, ReseedWs* w, const float* d_seed
 	return rc ? rc : launched(ctx, "reseed_rebuild", ocb::reseed_rebuild_launch(dim, d_seeds, prev, w->idx, m, zncc_min, w->anchor, sub, ctx->sm_count, ctx->stream));
 }
 
-// The 2D series of reference s.ref against the F frames of the stack s.tar, over the n device seeds into d_out (F x n records,
-// frame-major), re-seeding lost POIs when rs is set.
+// A 2D subset method of the image series calls: IC-GN (order 1 or 2), IC-LM (the same order with its damping (lambda, alpha, beta),
+// passed through unchecked as by ocb_iclm2d) or NR2D1.  It supplies the series launch over frames of a stack and the pair launch
+// on re-seeded records against one frame.
+struct SubsetMethod2D {
+	bool nr;                 // NR2D1; otherwise IC-GN / IC-LM
+	int order;               // IC-GN / IC-LM: the shape-function order
+	const float* lm_damping; // IC-LM: (lambda, alpha, beta); null: IC-GN
+	int np() const { return order == 1 ? 6 : 12; }
+};
+
+// The launch geometry of NR2D1, or OCB_ERR_UNSUPPORTED when one warp's slab does not fit in shared memory
+static int nr2d1_plan_or_error(ocb_ctx* ctx, int rx, int ry, ocb::Nr2dPlan* plan) {
+	if (ocb::nr2d1_plan(rx, ry, ctx->smem_optin, plan)) return OCB_OK;
+	return set_error(ctx, OCB_ERR_UNSUPPORTED, "nr2d1: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
+}
+
+// NR2D1 of the n device records q (1 <= n < 2^31) against img, on ctx's device (current) and stream.  The pair calls pass their
+// image pair, the re-seeding series calls one frame of the series.
+static int nr2d1_run(ocb_ctx* ctx, const ocb::Image2D& img, float* q, size_t n, int rx, int ry, float conv, float stop) {
+	ocb::Nr2dPlan plan;
+	if (const int rc = nr2d1_plan_or_error(ctx, rx, ry, &plan)) return rc;
+	return launched(ctx, "nr2d1", ocb::nr2d1_launch(plan, img, q, n, rx, ry, conv, stop, ctx->sm_count, ctx->d_counter, ctx->stream));
+}
+
+// The method's series launch: the m seeds through the frames of img.tar into out (frames x m records, frame-major).  IC-GN and
+// IC-LM take the warps per POI of a launch over plan_n POIs; NR2D1's plan does not depend on the queue.
+static int subset2d_series_launch(ocb_ctx* ctx, const SubsetMethod2D& sm, const ocb::Image2D& img, int frames, const float* seeds, float* out,
+	size_t m, size_t plan_n, int rx, int ry, float conv, float stop) {
+	if (sm.nr) {
+		ocb::Nr2dPlan plan;
+		if (const int r = nr2d1_plan_or_error(ctx, rx, ry, &plan)) return r;
+		return launched(ctx, "nr2d1_series",
+			ocb::nr2d1_series_launch(plan, img, frames, seeds, out, m, rx, ry, conv, stop, ctx->sm_count, ctx->d_counter, ctx->stream));
+	}
+	ocb::Icgn2dPlan plan;
+	if (const int r = icgn2d_plan_or_error(ctx, m, plan_n, sm.np(), rx, ry, sm.lm_damping != nullptr, &plan)) return r;
+	return launched(ctx, sm.lm_damping ? "iclm2d_series" : "icgn2d_series",
+		ocb::icgn2d_series_launch(sm.np(), plan, img, frames, seeds, out, m, rx, ry, conv, stop, ctx->d_counter, sm.lm_damping, ctx->stream));
+}
+
+// The method's pair launch on the m device records q against the image pair img, with the warps per POI of plan_n POIs
+static int subset2d_pair_run(ocb_ctx* ctx, const SubsetMethod2D& sm, const ocb::Image2D& img, float* q, size_t m, size_t plan_n, int rx, int ry,
+	float conv, float stop) {
+	if (sm.nr) return nr2d1_run(ctx, img, q, m, rx, ry, conv, stop);
+	return icgn2d_run(ctx, sm.np(), img, q, m, plan_n, rx, ry, conv, stop, nullptr, sm.lm_damping);
+}
+
+// The 2D series of reference s.ref against the F frames of the stack s.tar with the subset method sm, over the n device seeds
+// into d_out (F x n records, frame-major), re-seeding lost POIs when rs is set.
 // Without rs this is one series launch.  With it:
 //   1. the same series launch over all n POIs and frames;
 //   2. one scan of every record for each POI's first lost frame, whose per-frame counts come back in one copy (none: done);
-//   3. for the smallest frame f with losses: its m lost POIs are gathered and rebuilt, FFT-CC and IC-GN run on them against
-//      frame f and the results go to out[f]; then one series launch carries those m records through frames f + 1 ... F - 1
-//      (into ctx->reseed_cont) and they are scattered into out; those m POIs alone are scanned again for a later loss;
+//   3. for the smallest frame f with losses: its m lost POIs are gathered and rebuilt, FFT-CC and the method's pair launch run on
+//      them against frame f and the results go to out[f]; then one series launch carries those m records through frames
+//      f + 1 ... F - 1 (into ctx->reseed_cont) and they are scattered into out; those m POIs alone are scanned again for a later
+//      loss;
 //   4. step 3 repeats for the next frame with losses: one synchronisation per such frame.
-// Every IC-GN launch takes the warps per POI of a launch over all n POIs, so each POI splits its sums as in step 1.
-static int icgn2d_series_run(ocb_ctx* ctx, int np, const ocb::Image2D& s, int F, const float* d_seeds, float* d_out, size_t n, int rx, int ry,
-	float conv, float stop, const SeriesReseed* rs) {
+// Every IC-GN / IC-LM launch takes the warps per POI of a launch over all n POIs, so each POI splits its sums as in step 1.
+static int subset2d_series_run(ocb_ctx* ctx, const SubsetMethod2D& sm, const ocb::Image2D& s, int F, const float* d_seeds, float* d_out, size_t n,
+	int rx, int ry, float conv, float stop, const SeriesReseed* rs) {
 	const size_t frame_px = (size_t)s.w * s.h;
-	auto series = [&](const ocb::Image2D& img, int frames, const float* seeds, float* out, size_t m) -> int {
-		ocb::Icgn2dPlan plan;
-		if (const int r = icgn2d_plan_or_error(ctx, m, n, np, rx, ry, false, &plan)) return r;
-		return launched(ctx, "icgn2d_series", ocb::icgn2d_series_launch(np, plan, img, frames, seeds, out, m, rx, ry, conv, stop, ctx->d_counter, ctx->stream));
-	};
 	int rc;
-	if ((rc = series(s, F, d_seeds, d_out, n))) return rc;
+	if ((rc = subset2d_series_launch(ctx, sm, s, F, d_seeds, d_out, n, n, rx, ry, conv, stop))) return rc;
 	if (!rs) return OCB_OK;
 	const size_t rec = OCB_POI2D_FLOATS;
 	const float zmin = rs->zncc_min;
@@ -1325,14 +1368,15 @@ static int icgn2d_series_run(ocb_ctx* ctx, int np, const ocb::Image2D& s, int F,
 		if ((rc = reseed_gather(ctx, 2, &w, d_seeds, f ? d_out + (size_t)(f - 1) * n * rec : nullptr, n, f, m, zmin, sub))) return rc;
 		const ocb::Image2D frame{ s.ref, s.tar + (size_t)f * frame_px, s.w, s.h };
 		if ((rc = fftcc2d_run(ctx, frame, sub, m, rs->fft_r[0], rs->fft_r[1]))) return rc;
-		if ((rc = icgn2d_run(ctx, np, frame, sub, m, n, rx, ry, conv, stop, nullptr, nullptr))) return rc;
+		if ((rc = subset2d_pair_run(ctx, sm, frame, sub, m, n, rx, ry, conv, stop))) return rc;
 		if ((rc = launched(ctx, "reseed_scatter", ocb::reseed_scatter_launch(2, sub, m, 1, w.idx, d_out, n, f, ctx->sm_count, ctx->stream)))) return rc;
 		rs->counts[f] = m;
 		if (f + 1 == F) break;
 		const int rest = F - f - 1;
 		if ((rc = grow(ctx, ctx->reseed_cont, (size_t)rest * m * rec * sizeof(float)))) return rc;
 		float* const cont = ctx->reseed_cont.as<float>();
-		if ((rc = series(ocb::Image2D{ s.ref, s.tar + (size_t)(f + 1) * frame_px, s.w, s.h }, rest, sub, cont, m))) return rc;
+		const ocb::Image2D later{ s.ref, s.tar + (size_t)(f + 1) * frame_px, s.w, s.h };
+		if ((rc = subset2d_series_launch(ctx, sm, later, rest, sub, cont, m, n, rx, ry, conv, stop))) return rc;
 		if ((rc = launched(ctx, "reseed_scatter", ocb::reseed_scatter_launch(2, cont, m, rest, w.idx, d_out, n, f + 1, ctx->sm_count, ctx->stream)))
 			|| (rc = launched(ctx, "reseed_scan", ocb::reseed_scan_launch(2, d_out, n, f + 1, F, w.idx, m, zmin, w.first, w.hist, ctx->sm_count, ctx->stream)))
 			|| (rc = reseed_read_hist(ctx, &w)))
@@ -1342,10 +1386,10 @@ static int icgn2d_series_run(ocb_ctx* ctx, int np, const ocb::Image2D& s, int F,
 }
 
 // Checks and runs a 2D series call on a single-device context: device seeds and output; rs null for the plain series.
-static int icgn2d_series_dev(ocb_ctx* ctx, const char* what, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv,
-	float stop, const SeriesReseed* rs) {
+static int subset2d_series_dev(ocb_ctx* ctx, const char* what, const SubsetMethod2D& sm, const void* d_seeds, void* d_out, size_t n, int rx, int ry,
+	float conv, float stop, const SeriesReseed* rs) {
 	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
-	if (order != 1 && order != 2) return set_error(ctx, OCB_ERR_ARG, "%s: order must be 1 or 2", what);
+	if (!sm.nr && sm.order != 1 && sm.order != 2) return set_error(ctx, OCB_ERR_ARG, "%s: order must be 1 or 2", what);
 	const SeriesStore& s = ctx->series2d;
 	if (!s.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
 	int rc;
@@ -1353,39 +1397,100 @@ static int icgn2d_series_dev(ocb_ctx* ctx, const char* what, int order, const vo
 	if (n == 0) return OCB_OK;
 	if ((rc = series_size_check(ctx, what, n, s.frames, OCB_POI2D_FLOATS * sizeof(float), false))) return rc;
 	if (ensure_device(ctx)) return OCB_ERR_CUDA;
-	return icgn2d_series_run(ctx, order == 1 ? 6 : 12, s.view2(0), s.frames, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv, stop, rs);
+	return subset2d_series_run(ctx, sm, s.view2(0), s.frames, (const float*)d_seeds, (float*)d_out, n, rx, ry, conv, stop, rs);
 }
 
-static int icgn2d_series_host(ocb_ctx* ctx, const char* what, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop,
-	const SeriesReseed* rs) {
+static int subset2d_series_host(ocb_ctx* ctx, const char* what, const SubsetMethod2D& sm, const void* seeds, void* out, size_t n, int rx, int ry,
+	float conv, float stop, const SeriesReseed* rs) {
 	return series_host(ctx, what, &ocb_ctx::series2d, n, { seeds }, OCB_POI2D_FLOATS, { { out, OCB_POI2D_FLOATS } },
-		[&](ocb_ctx* x, const float* const* d_in, float* const* d_out) { return icgn2d_series_dev(x, what, order, d_in[0], d_out[0], n, rx, ry, conv, stop, rs); });
+		[&](ocb_ctx* x, const float* const* d_in, float* const* d_out) { return subset2d_series_dev(x, what, sm, d_in[0], d_out[0], n, rx, ry, conv, stop, rs); });
+}
+
+// The plain and the re-seeding series calls of one method (dev: device seeds and out)
+static int subset2d_series_call(ocb_ctx* ctx, const char* what, const SubsetMethod2D& sm, bool dev, const void* seeds, void* out, size_t n, int rx,
+	int ry, float conv, float stop) {
+	return dev ? subset2d_series_dev(ctx, what, sm, seeds, out, n, rx, ry, conv, stop, nullptr)
+		: subset2d_series_host(ctx, what, sm, seeds, out, n, rx, ry, conv, stop, nullptr);
+}
+static int subset2d_series_reseed_call(ocb_ctx* ctx, const char* what, const SubsetMethod2D& sm, bool dev, const void* seeds, void* out, size_t n,
+	int rx, int ry, float conv, float stop, int fft_rx, int fft_ry, float zncc_min, size_t* reseeded) {
+	return series_reseed(ctx, &ocb_ctx::series2d, dev, n, reseeded, [&](size_t* counts) {
+		const SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts };
+		return dev ? subset2d_series_dev(ctx, what, sm, seeds, out, n, rx, ry, conv, stop, &rs)
+			: subset2d_series_host(ctx, what, sm, seeds, out, n, rx, ry, conv, stop, &rs);
+	});
 }
 
 int ocb_icgn2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop) {
 	OCB_NO_GROUP(ctx, "icgn2d_series_dev");
-	return icgn2d_series_dev(ctx, "icgn2d_series", order, d_seeds, d_out, n, rx, ry, conv, stop, nullptr);
+	return subset2d_series_call(ctx, "icgn2d_series", { false, order, nullptr }, true, d_seeds, d_out, n, rx, ry, conv, stop);
 }
 
 int ocb_icgn2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop) {
-	return icgn2d_series_host(ctx, "icgn2d_series", order, seeds, out, n, rx, ry, conv, stop, nullptr);
+	return subset2d_series_call(ctx, "icgn2d_series", { false, order, nullptr }, false, seeds, out, n, rx, ry, conv, stop);
 }
 
 int ocb_icgn2d_series_reseed_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
 	int fft_rx, int fft_ry, float zncc_min, size_t* reseeded) {
 	OCB_NO_GROUP(ctx, "icgn2d_series_reseed_dev");
-	return series_reseed(ctx, &ocb_ctx::series2d, true, n, reseeded, [&](size_t* counts) {
-		const SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts };
-		return icgn2d_series_dev(ctx, "icgn2d_series_reseed", order, d_seeds, d_out, n, rx, ry, conv, stop, &rs);
-	});
+	return subset2d_series_reseed_call(ctx, "icgn2d_series_reseed", { false, order, nullptr }, true, d_seeds, d_out, n, rx, ry, conv, stop, fft_rx,
+		fft_ry, zncc_min, reseeded);
 }
 
 int ocb_icgn2d_series_reseed(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, int fft_rx,
 	int fft_ry, float zncc_min, size_t* reseeded) {
-	return series_reseed(ctx, &ocb_ctx::series2d, false, n, reseeded, [&](size_t* counts) {
-		const SeriesReseed rs{ { fft_rx, fft_ry, 1 }, zncc_min, counts };
-		return icgn2d_series_host(ctx, "icgn2d_series_reseed", order, seeds, out, n, rx, ry, conv, stop, &rs);
-	});
+	return subset2d_series_reseed_call(ctx, "icgn2d_series_reseed", { false, order, nullptr }, false, seeds, out, n, rx, ry, conv, stop, fft_rx,
+		fft_ry, zncc_min, reseeded);
+}
+
+int ocb_iclm2d_series_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop, float lambda,
+	float alpha, float beta) {
+	OCB_NO_GROUP(ctx, "iclm2d_series_dev");
+	const float damping[3] = { lambda, alpha, beta };
+	return subset2d_series_call(ctx, "iclm2d_series", { false, order, damping }, true, d_seeds, d_out, n, rx, ry, conv, stop);
+}
+
+int ocb_iclm2d_series(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, float lambda, float alpha,
+	float beta) {
+	const float damping[3] = { lambda, alpha, beta };
+	return subset2d_series_call(ctx, "iclm2d_series", { false, order, damping }, false, seeds, out, n, rx, ry, conv, stop);
+}
+
+int ocb_iclm2d_series_reseed_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
+	float lambda, float alpha, float beta, int fft_rx, int fft_ry, float zncc_min, size_t* reseeded) {
+	OCB_NO_GROUP(ctx, "iclm2d_series_reseed_dev");
+	const float damping[3] = { lambda, alpha, beta };
+	return subset2d_series_reseed_call(ctx, "iclm2d_series_reseed", { false, order, damping }, true, d_seeds, d_out, n, rx, ry, conv, stop, fft_rx,
+		fft_ry, zncc_min, reseeded);
+}
+
+int ocb_iclm2d_series_reseed(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, float lambda,
+	float alpha, float beta, int fft_rx, int fft_ry, float zncc_min, size_t* reseeded) {
+	const float damping[3] = { lambda, alpha, beta };
+	return subset2d_series_reseed_call(ctx, "iclm2d_series_reseed", { false, order, damping }, false, seeds, out, n, rx, ry, conv, stop, fft_rx,
+		fft_ry, zncc_min, reseeded);
+}
+
+int ocb_nr2d1_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop) {
+	OCB_NO_GROUP(ctx, "nr2d1_series_dev");
+	return subset2d_series_call(ctx, "nr2d1_series", { true, 1, nullptr }, true, d_seeds, d_out, n, rx, ry, conv, stop);
+}
+
+int ocb_nr2d1_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop) {
+	return subset2d_series_call(ctx, "nr2d1_series", { true, 1, nullptr }, false, seeds, out, n, rx, ry, conv, stop);
+}
+
+int ocb_nr2d1_series_reseed_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop, int fft_rx,
+	int fft_ry, float zncc_min, size_t* reseeded) {
+	OCB_NO_GROUP(ctx, "nr2d1_series_reseed_dev");
+	return subset2d_series_reseed_call(ctx, "nr2d1_series_reseed", { true, 1, nullptr }, true, d_seeds, d_out, n, rx, ry, conv, stop, fft_rx, fft_ry,
+		zncc_min, reseeded);
+}
+
+int ocb_nr2d1_series_reseed(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, int fft_rx, int fft_ry,
+	float zncc_min, size_t* reseeded) {
+	return subset2d_series_reseed_call(ctx, "nr2d1_series_reseed", { true, 1, nullptr }, false, seeds, out, n, rx, ry, conv, stop, fft_rx, fft_ry,
+		zncc_min, reseeded);
 }
 
 // one launch over a host queue (all POIs share the radius), optional host offsets
@@ -1474,18 +1579,9 @@ int ocb_nr2d_prepare(ocb_ctx* ctx) {
 	return OCB_OK;
 }
 
-// The launch geometry of NR2D1, or OCB_ERR_UNSUPPORTED when one warp's slab does not fit in shared memory
-static int nr2d1_plan_or_error(ocb_ctx* ctx, int rx, int ry, ocb::Nr2dPlan* plan) {
-	if (ocb::nr2d1_plan(rx, ry, ctx->smem_optin, plan)) return OCB_OK;
-	return set_error(ctx, OCB_ERR_UNSUPPORTED, "nr2d1: subset radius (%d,%d) exceeds the shared-memory design limit", rx, ry);
-}
-
 int ocb_nr2d1_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, int rx, int ry, float conv, float stop) {
-	int rc = pair_checks(ctx, "nr2d1", d_poi2d, n, rx >= 1 && ry >= 1, nullptr, 2, &ocb_ctx::prepared_nr2, true);
-	if (rc != PAIR_GO) return rc;
-	ocb::Nr2dPlan plan;
-	if ((rc = nr2d1_plan_or_error(ctx, rx, ry, &plan))) return rc;
-	return launched(ctx, "nr2d1", ocb::nr2d1_launch(plan, ctx->img2, (float*)d_poi2d, n, rx, ry, conv, stop, ctx->sm_count, ctx->d_counter, ctx->stream));
+	const int rc = pair_checks(ctx, "nr2d1", d_poi2d, n, rx >= 1 && ry >= 1, nullptr, 2, &ocb_ctx::prepared_nr2, true);
+	return rc == PAIR_GO ? nr2d1_run(ctx, ctx->img2, (float*)d_poi2d, n, rx, ry, conv, stop) : rc;
 }
 
 int ocb_nr2d1(ocb_ctx* ctx, void* poi2d, size_t n, int rx, int ry, float conv, float stop) {
@@ -2006,8 +2102,8 @@ static int stereo_series_dev(ocb_ctx* x, const ocb::StereoCam& c1, const ocb::St
 	ocb::Icgn2dPlan plan;
 	if ((rc = icgn2d_plan_or_error(x, n, n, np1, rx, ry, false, &plan)) || (rc = icgn2d_plan_or_error(x, n, n, np2, rx, ry, false, &plan))) return rc;
 	if (ensure_device(x)) return OCB_ERR_CUDA;
-	if ((rc = icgn2d_series_run(x, np1, s.view2(0), s.frames, d_seeds1, d_out1, n, rx, ry, conv, stop, nullptr))) return rc;
-	if ((rc = icgn2d_series_run(x, np2, s.view2(1), s.frames, d_seeds2, d_out2, n, rx, ry, conv, stop, nullptr))) return rc;
+	if ((rc = subset2d_series_run(x, { false, order1, nullptr }, s.view2(0), s.frames, d_seeds1, d_out1, n, rx, ry, conv, stop, nullptr))) return rc;
+	if ((rc = subset2d_series_run(x, { false, order2, nullptr }, s.view2(1), s.frames, d_seeds2, d_out2, n, rx, ry, conv, stop, nullptr))) return rc;
 	return launched(x, "stereo_poi2ds", ocb::stereo_poi2ds_launch(c1, c2, d_stereo, d_seeds1, d_out1, d_out2, d_out2ds, n, s.frames, x->stream));
 }
 

@@ -129,9 +129,10 @@ inline bool icgn2d_plan(size_t n, int np, int rx, int ry, bool lm, int sm_count,
 // work-queue heads (64 ints; see ocb_create).
 cudaError_t icgn2d_launch(int np, const Icgn2dPlan& plan, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop,
 	int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream);
-// one reference (img.ref) against the frame-major stack img.tar [n_frames][h][w]: n seeds in, n_frames x n records out (frame-major)
+// one reference (img.ref) against the frame-major stack img.tar [n_frames][h][w]: n seeds in, n_frames x n records out (frame-major);
+// lm_damping as for icgn2d_launch
 cudaError_t icgn2d_series_launch(int np, const Icgn2dPlan& plan, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n,
-	int rx, int ry, float conv, float stop, int* d_counter, cudaStream_t stream);
+	int rx, int ry, float conv, float stop, int* d_counter, const float* lm_damping, cudaStream_t stream);
 // series_reseed.cu: the lost-POI scan, compaction, rebuild and scatter of the re-seeding series calls (dim: 2 or 3; records
 // frame-major, out[f * n + i]).
 // scan: for the POIs idx[0..m) (0..m when idx is null), first[i] = the first frame in [f_begin, f_end) with !(zncc >= zncc_min), or
@@ -188,6 +189,9 @@ inline bool nr2d1_plan(int rx, int ry, size_t smem_optin, Nr2dPlan* p) {
 }
 cudaError_t nr2d1_launch(const Nr2dPlan& plan, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop, int sm_count,
 	int* d_counter, cudaStream_t stream);
+// one reference (img.ref) against the frame-major stack img.tar [n_frames][h][w]: n seeds in, n_frames x n records out (frame-major)
+cudaError_t nr2d1_series_launch(const Nr2dPlan& plan, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n, int rx, int ry,
+	float conv, float stop, int sm_count, int* d_counter, cudaStream_t stream);
 // epipolar.cu
 int epipolar_slots(int search_radius, int search_step);
 cudaError_t epipolar_candidates_launch(const float* d_pois, size_t poi0, size_t n_poi, const float* fundamental, const float* parallax_x,
