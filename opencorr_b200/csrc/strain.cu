@@ -9,7 +9,7 @@
 // colPivHouseholderQr in the reference); the plane's slopes are the displacement gradients, from
 // which the Cauchy or Green strains follow.
 //
-// GPU mapping: no tree.  The POIs are binned into a uniform grid (cell edge >= radius) by one
+// GPU mapping: no tree.  The POIs are binned into a uniform grid (cell edge >= |radius|) by one
 // stable radix sort of (cell id, POI index); a warp per POI then scans the 3 (2D) / 9 (3D) runs of
 // x-adjacent cells that can hold neighbours -- contiguous in the sorted order, found by binary
 // search -- with coalesced 16-byte loads, and accumulates the normal equations in FP64 (12 / 22
@@ -430,9 +430,11 @@ cudaError_t strain_launch(int mode, float* d_pois, size_t n, float radius, int k
 		const float hi = d < dim ? ordered_to_float(hb[3 + d]) : 0.f;
 		if (hi - g.lo[d] > extent) extent = hi - g.lo[d];
 	}
-	// cell edge >= radius so that the 3^D block around a POI's cell holds every point within the radius;
-	// grown until the grid has < 2^30 cells
-	double cell = radius > 0.f ? (double)radius : (double)extent / 64.0 + 1.0;
+	// cell edge >= |radius| so that the 3^D block around a POI's cell holds every point within the radius (the test is
+	// dist^2 < radius^2, so a negative radius acts as its magnitude); a non-finite radius takes one cell over the bbox
+	// (+-inf: every POI is a neighbour, NaN: none is); grown until the grid has < 2^30 cells
+	const float abs_radius = fabsf(radius);
+	double cell = !isfinite(abs_radius) ? (double)extent + 1.0 : abs_radius > 0.f ? (double)abs_radius : (double)extent / 64.0 + 1.0;
 	if (!(cell > 0.0) || !isfinite(cell)) cell = 1.0;
 	while (true) {
 		double total = 1.0;

@@ -1247,17 +1247,32 @@ void run_strain(float* pois, long n, float radius, int k_min, float zncc_thresho
 	typedef StrainLayout<MODE> L;
 	constexpr int NF = L::NF, D = L::SD, FD = L::FD, NE = FD == 2 ? 3 : 6; // D: search dimensions
 	auto finite = [&](const float* p) { for (int d = 0; d < D; d++) if (!std::isfinite(p[d])) return false; return true; };
-	// uniform grid over the POI positions, cell edge = radius
-	float lo[3] = { 0, 0, 0 }, hi[3] = { 0, 0, 0 };
-	for (int d = 0; d < D; d++) { lo[d] = 1e30f; hi[d] = -1e30f; }
+	if (approximation != 1 && approximation != 2) return; // the reference writes no strain for any other value (:220-233)
+	// uniform grid over the POI positions
+	double lo[3] = { 0, 0, 0 }, hi[3] = { 0, 0, 0 };
+	for (int d = 0; d < D; d++) { lo[d] = HUGE_VAL; hi[d] = -HUGE_VAL; }
 	for (long i = 0; i < n; i++)
 		if (finite(pois + i * NF))
-			for (int d = 0; d < D; d++) { lo[d] = std::min(lo[d], pois[i * NF + d]); hi[d] = std::max(hi[d], pois[i * NF + d]); }
+			for (int d = 0; d < D; d++) { lo[d] = std::min(lo[d], (double)pois[i * NF + d]); hi[d] = std::max(hi[d], (double)pois[i * NF + d]); }
 	if (lo[0] > hi[0]) return; // no POI with a finite position
-	const float cell = radius > 0 ? radius : 1.f;
+	// cell edge > |radius| (the test is dist^2 < radius^2, so a negative radius acts as its magnitude; the 0.1 % covers a
+	// float dist^2 that rounds below radius^2), one cell over the bbox for a non-finite radius (+-inf: every POI is a
+	// neighbour, NaN: none is), doubled until the grid has no more cells than a few per POI
+	double extent = 0;
+	for (int d = 0; d < D; d++) extent = std::max(extent, hi[d] - lo[d]);
+	const double abs_radius = std::fabs((double)radius);
+	double cell = !std::isfinite(abs_radius) ? extent + 1.0 : abs_radius > 0 ? abs_radius * 1.001 : 1.0;
 	long nc[3] = { 1, 1, 1 };
+	while (true) {
+		double total = 1;
+		for (int d = 0; d < D; d++) total *= std::floor((hi[d] - lo[d]) / cell) + 1;
+		if (total <= 4.0 * (double)n + 1024.0) break;
+		cell *= 2;
+	}
 	for (int d = 0; d < D; d++) nc[d] = (long)std::floor((hi[d] - lo[d]) / cell) + 1;
-	auto cell_of = [&](const float* p, long* c) { for (int d = 0; d < 3; d++) c[d] = d < D ? (long)std::floor((p[d] - lo[d]) / cell) : 0; };
+	auto cell_of = [&](const float* p, long* c) {
+		for (int d = 0; d < 3; d++) c[d] = d < D ? std::min(nc[d] - 1, (long)std::floor(((double)p[d] - lo[d]) / cell)) : 0;
+	};
 	std::vector<long> start((size_t)(nc[0] * nc[1] * nc[2]) + 1, 0), order(n);
 	for (long i = 0; i < n; i++) {
 		if (!finite(pois + i * NF)) continue;
