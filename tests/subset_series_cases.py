@@ -1,19 +1,24 @@
-"""Shared cases of the IC-LM and NR2D1 image-series tests: the synthetic series, the method's pair call and series calls, and the
-witness loops of pair calls the series calls must equal byte for byte."""
+"""Shared cases of the IC-GN, IC-LM and NR2D1 image-series tests: the synthetic series; each method's pair call, series calls and
+raw C series calls; the witness loops of pair calls the series calls must equal byte for byte; and the checks the three test
+files run, each with its own methods."""
+import ctypes
+
 import numpy as np
 
 import opencorr_b200 as ob
-from opencorr_b200 import synth
+from opencorr_b200 import _capi, synth
+from util import assert_same, compare_2d
 
 CONV, STOP = 0.001, 10
 DAMPING = (100.0, 0.1, 10.0)  # ocb_iclm2d's defaults (DampingParameter, src/oc_iclm.h)
 OTHER_DAMPING = (30.0, 0.3, 4.0)
 
 
-def render_series(width, height, n_frames, second_order=False, vy_step=0.0, rho=2.0, seed=synth.REF_SEED):
+def render_series(width, height, n_frames, second_order=False, vy_step=0.0, jump=None, rho=2.0, seed=synth.REF_SEED):
     """ref and n_frames targets: the speckles of synth.speckle_pair_2d moved by (f + 1) / n_frames of its displacement field,
     so the last frame carries the full field.  vy_step adds a vertical stretch about the image centre of (f + 1) vy_step in
-    frame f."""
+    frame f.  jump = (k, x0, y0, x1, y1, du, dv): from frame k on, the speckles whose reference centre lies in the box move by
+    (du, dv) more."""
     rng = np.random.default_rng(seed)
     n = int(0.5 * width * height / (np.pi * rho * rho))
     cx = rng.uniform(-8, width + 8, n)
@@ -21,11 +26,17 @@ def render_series(width, height, n_frames, second_order=False, vy_step=0.0, rho=
     amp = rng.uniform(0.4, 1.0, n)
     u, v = synth.displacement_2d(cx, cy, width, height, second_order)
 
-    def image(s, stretch):
-        im = synth._render((height, width), np.stack([cy + s * v + stretch * (cy - height / 2), cx + s * u], 1), amp, rho)
+    def image(f):  # f = -1: the reference
+        s = (f + 1) / n_frames
+        y, x = cy + s * v + (f + 1) * vy_step * (cy - height / 2), cx + s * u
+        if jump is not None and f >= jump[0]:
+            k, x0, y0, x1, y1, du, dv = jump
+            inside = (cx >= x0) & (cx < x1) & (cy >= y0) & (cy < y1)
+            y, x = y + np.where(inside, dv, 0.0), x + np.where(inside, du, 0.0)
+        im = synth._render((height, width), np.stack([y, x], 1), amp, rho)
         return np.round(np.clip(synth.BACKGROUND + (255.0 - synth.BACKGROUND) * im, 0, 255)).astype(np.float32)
 
-    return image(0.0, 0.0), np.stack([image((f + 1) / n_frames, (f + 1) * vy_step) for f in range(n_frames)])
+    return image(-1), np.stack([image(f) for f in range(n_frames)])
 
 
 def true_displacement(xy, shape, n_frames, f, second_order=False, vy_step=0.0):
@@ -36,12 +47,6 @@ def true_displacement(xy, shape, n_frames, f, second_order=False, vy_step=0.0):
     return s * u, s * v + (f + 1) * vy_step * (xy[:, 1] - h / 2)
 
 
-def assert_same(a, b, label):
-    assert a.shape == b.shape, label
-    bad = a.view(np.uint32) != b.view(np.uint32)
-    assert not bad.any(), "%s: %d floats differ, first at %s" % (label, bad.sum(), np.argwhere(bad)[:5].tolist())
-
-
 def fftcc_seeds(eng, ref, tar, xy, r):
     q = ob.make_poi2d(xy)
     eng.set_images_2d(ref, tar)
@@ -50,49 +55,58 @@ def fftcc_seeds(eng, ref, tar, xy, r):
 
 
 class Method:
-    """A 2D subset method: "iclm" (order 1 or 2, damping) or "nr" (NR2D1)."""
+    """A 2D subset method: "icgn" (IC-GN), "iclm" (IC-LM with damping), both of shape-function order 1 or 2, or "nr" (NR2D1)."""
 
     def __init__(self, kind, order=1, damping=DAMPING):
         self.kind, self.order, self.damping = kind, order, damping
+        self.name = {"icgn": "icgn2d", "iclm": "iclm2d", "nr": "nr2d1"}[kind]  # of the engine's and the C ABI's series calls
 
     def __repr__(self):
-        return "ICLM2D%d" % self.order if self.kind == "iclm" else "NR2D1"
+        return "NR2D1" if self.kind == "nr" else "%s2D%d" % (self.kind.upper(), self.order)
 
-    def pair(self, eng, q, r, stop=STOP):
-        """prepare() and compute(queue) on the pair set on eng"""
-        if self.kind == "iclm":
-            eng.icgn2d_prepare()
+    def pair(self, eng, q, r, stop=STOP, prepare=True):
+        """prepare() (unless prepare is False) and compute(queue) on the pair set on eng"""
+        if prepare:
+            (eng.nr2d_prepare if self.kind == "nr" else eng.icgn2d_prepare)()
+        if self.kind == "icgn":
+            (eng.icgn2d1 if self.order == 1 else eng.icgn2d2)(q, r, r, CONV, stop)
+        elif self.kind == "iclm":
             eng.iclm2d(self.order, q, r, r, CONV, stop, self.damping)
         else:
-            eng.nr2d_prepare()
             eng.nr2d1(q, r, r, CONV, stop)
 
-    def oracle(self, o, q, r, stop=STOP):
-        if self.kind == "iclm":
-            o.iclm2d(self.order, q, r, r, CONV, stop, self.damping)
+    def oracle(self, o, q, r, stop=STOP, exact=False):
+        if self.kind == "icgn":
+            (o.icgn2d1 if self.order == 1 else o.icgn2d2)(q, r, r, CONV, stop, exact=exact)
+        elif self.kind == "iclm":
+            o.iclm2d(self.order, q, r, r, CONV, stop, self.damping, exact=exact)
         else:
-            o.nr2d1(q, r, r, CONV, stop)
+            o.nr2d1(q, r, r, CONV, stop, exact=exact)
+
+    def _series_call(self, eng, suffix, *args):
+        """eng.<name><suffix>([order,] *args[, damping=damping])"""
+        lead = () if self.kind == "nr" else (self.order,)
+        kw = dict(damping=self.damping) if self.kind == "iclm" else {}
+        return getattr(eng, self.name + suffix)(*lead, *args, **kw)
 
     def series(self, eng, seeds, r, stop=STOP):
-        if self.kind == "iclm":
-            return eng.iclm2d_series(self.order, seeds, r, r, CONV, stop, self.damping)
-        return eng.nr2d1_series(seeds, r, r, CONV, stop)
+        return self._series_call(eng, "_series", seeds, r, r, CONV, stop)
 
     def series_reseed(self, eng, seeds, r, fr, zncc_min, stop=STOP):
-        if self.kind == "iclm":
-            return eng.iclm2d_series_reseed(self.order, seeds, r, r, CONV, stop, fr, fr, zncc_min, self.damping)
-        return eng.nr2d1_series_reseed(seeds, r, r, CONV, stop, fr, fr, zncc_min)
+        return self._series_call(eng, "_series_reseed", seeds, r, r, CONV, stop, fr, fr, zncc_min)
 
     def series_dev(self, eng, d_seeds, d_out, n, r):
-        if self.kind == "iclm":
-            eng.iclm2d_series_dev(self.order, d_seeds, d_out, n, r, r, CONV, STOP, self.damping)
-        else:
-            eng.nr2d1_series_dev(d_seeds, d_out, n, r, r, CONV, STOP)
+        self._series_call(eng, "_series_dev", d_seeds, d_out, n, r, r, CONV, STOP)
 
     def series_reseed_dev(self, eng, d_seeds, d_out, n, r, fr, zncc_min):
-        if self.kind == "iclm":
-            return eng.iclm2d_series_reseed_dev(self.order, d_seeds, d_out, n, r, r, CONV, STOP, fr, fr, zncc_min, self.damping)
-        return eng.nr2d1_series_reseed_dev(d_seeds, d_out, n, r, r, CONV, STOP, fr, fr, zncc_min)
+        return self._series_call(eng, "_series_reseed_dev", d_seeds, d_out, n, r, r, CONV, STOP, fr, fr, zncc_min)
+
+    def c_series(self, lib, ctx, suffix, order, seeds, out, n, r, *reseed):
+        """The C ABI's ocb_<name>_series<suffix>(ctx, [order,] seeds, out, n, r, r, CONV, STOP, [damping,] *reseed) on raw
+        pointers; order None: the method's."""
+        lead = () if self.kind == "nr" else (self.order if order is None else order,)
+        damping = tuple(self.damping) if self.kind == "iclm" else ()
+        return getattr(lib, "ocb_%s_series%s" % (self.name, suffix))(ctx, *lead, seeds, out, n, r, r, CONV, STOP, *damping, *reseed)
 
 
 def pair_loop(eng, method, ref, tars, seeds, r, stop=STOP):
@@ -108,7 +122,7 @@ def pair_loop(eng, method, ref, tars, seeds, r, stop=STOP):
 
 def reseed_pair_loop(eng, method, ref, tars, seeds, r, fr, zncc_min):
     """pair_loop that re-seeds the POIs lost in frame f from their seeds at their latest good translation, then runs FFT-CC and
-    the method on them against frame f (the rules of ocb_icgn2d_series_reseed)"""
+    the method on them against frame f (the rules of the ocb_*2d*_series_reseed calls)"""
     q = seeds.copy()
     anchor = seeds[:, [2, 8]].copy()
     out, counts = [], []
@@ -148,10 +162,11 @@ def long_grid(r):
     return synth.grid_2d(r + 4, r + 4, 112, 70, 3, 4)  # 7840 POIs: more than the resident slots at these radii
 
 
-# ---- the checks both test files run, each with its own methods ---------------------------------------------------------------
+# ---- the checks the test files run, each with its own methods ----------------------------------------------------------------
 
-def check_equals_pair_loop(eng, method, ref, tars, xy, r, label):
-    seeds = fftcc_seeds(eng, ref, tars[0], xy, min(r, 16))
+def check_equals_pair_loop(eng, method, ref, tars, xy, r, label, fft_r=None):
+    """seeded by FFT-CC of radius fft_r (None: min(r, 16))"""
+    seeds = fftcc_seeds(eng, ref, tars[0], xy, fft_r or min(r, 16))
     for n_frames in (1, len(tars)):
         expect = pair_loop(eng, method, ref, tars[:n_frames], seeds, r)
         eng.set_series_2d(ref, tars[:n_frames])
@@ -195,15 +210,17 @@ def check_chunks(eng, method, ref, tars, r):
     assert_same(np.concatenate([a, b]), whole, "%s in two chunks" % method)
 
 
-def check_pair_state_undisturbed(eng, method, ref, tars, r):
+def check_pair_state_undisturbed(eng, method, ref, tars, r, series_method=None):
+    """method's pair call returns the same records after series calls of series_method (None: method) on another stack"""
+    series_method = series_method or method
     seeds = fftcc_seeds(eng, ref, tars[-1], short_grid(), 16)
     before = seeds.copy()
     method.pair(eng, before, r)
     eng.set_series_2d(ref[::-1].copy(), tars[:, ::-1].copy())
-    method.series(eng, seeds, r)
-    method.series_reseed(eng, seeds, r, 16, 0.99)
+    series_method.series(eng, seeds, r)
+    series_method.series_reseed(eng, seeds, r, 16, 0.99)
     after = seeds.copy()
-    method.pair(eng, after, r)  # the pair (ref, tars[-1]) is still set
+    method.pair(eng, after, r, prepare=False)  # the pair (ref, tars[-1]) is still set and prepared
     assert_same(after, before, "%s pair call after series calls" % method)
 
 
@@ -257,7 +274,8 @@ def check_nothing_lost(eng, method, ref, tars, xy, r):
 
 
 def lossy_series(width=387, height=320, n_frames=6):
-    """Frame 2 occludes a block of POIs; three seeds arrive failed (index 3, 17, 40)."""
+    """(ref, tars, xy, [(frame, POIs occluded in it)]): frame 2 occludes a block of POIs.  check_reseed_equals_pair_loop fails
+    three seeds (index 3, 17, 40)."""
     ref, tars = render_series(width, height, n_frames)
     xy = synth.grid_2d(50, 50, 8, 6, 40, 40)
     sel = (xy[:, 0] >= 130) & (xy[:, 0] < 210) & (xy[:, 1] >= 130) & (xy[:, 1] < 210)
@@ -265,11 +283,11 @@ def lossy_series(width=387, height=320, n_frames=6):
     x0, y0 = xy[sel].min(0) + (u[0], v[0])
     x1, y1 = xy[sel].max(0) + (u[0], v[0])
     tars = occlude(tars, 2, (int(x0) - 24, int(y0) - 24, int(x1) + 25, int(y1) + 25))
-    return ref, tars, xy, sel
+    return ref, tars, xy, [(2, sel)]
 
 
 def check_reseed_equals_pair_loop(eng, method, lossy, r, fr):
-    ref, tars, xy, sel = lossy
+    ref, tars, xy, occluded = lossy
     seeds = fftcc_seeds(eng, ref, tars[0], xy, 16)
     seeds[[3, 17, 40], 16] = -1.0
     for n_frames in (1, len(tars)):
@@ -280,22 +298,65 @@ def check_reseed_equals_pair_loop(eng, method, lossy, r, fr):
         assert np.array_equal(counts, expect_counts), (counts, expect_counts)
         assert counts[0] >= 3
         if n_frames == len(tars):
-            assert counts[2] >= sel.sum()
+            for k, sel in occluded:  # the last frame is re-seeded too
+                assert counts[k] >= sel.sum(), (k, counts)
 
 
-def check_oracle_and_ground_truth(eng, method, ref, tars, r, second_order=False, vy_step=0.0, bound=0.05):
+def check_oracle_and_ground_truth(eng, method, ref, tars, r, second_order=False, vy_step=0.0, bound=0.05, fft_r=16, every_frame=False):
+    """The last frame (every_frame: every frame, against the oracle's exact mode) matches the float64 oracle run from the GPU's
+    records of the frame before, and the last frame the ground truth.  Seeded by FFT-CC of radius fft_r."""
     from oracle.oracle import Oracle2D
-    from util import compare_2d
     xy = synth.grid_2d(40, 40, 12, 10, 27, 24)
-    seeds = fftcc_seeds(eng, ref, tars[0], xy, 16)
+    seeds = fftcc_seeds(eng, ref, tars[0], xy, fft_r)
     eng.set_series_2d(ref, tars)
     got = method.series(eng, seeds, r)
-    f = len(tars) - 1
-    q = got[f - 1].copy()  # the last frame from the same records as the GPU's
-    method.oracle(Oracle2D(ref, tars[f]), q, r)
-    compare_2d(got[f], q, "%s last frame" % method, order=method.order)
-    last = got[-1]
-    ok = last[:, 16] >= 0
+    last = len(tars) - 1
+    for f in range(len(tars)) if every_frame else [last]:
+        q = (seeds if f == 0 else got[f - 1]).copy()  # from the same records as the GPU's
+        method.oracle(Oracle2D(ref, tars[f]), q, r, exact=every_frame)
+        compare_2d(got[f], q, "%s frame %d" % (method, f), order=method.order)
+    ok = got[last][:, 16] >= 0
     assert ok.mean() > 0.95
-    u, v = true_displacement(xy, ref.shape, len(tars), f, second_order, vy_step)
-    assert np.abs(last[ok, 2] - u[ok]).max() < bound and np.abs(last[ok, 8] - v[ok]).max() < bound
+    u, v = true_displacement(xy, ref.shape, len(tars), last, second_order, vy_step)
+    assert np.abs(got[last][ok, 2] - u[ok]).max() < bound and np.abs(got[last][ok, 8] - v[ok]).max() < bound
+
+
+def check_errors_leave_out_untouched(method):
+    """Refused series calls of the method, plain and re-seeding, with host and device pointers, leave out and the re-seed counts
+    untouched; refused set_series_2d calls set nothing; the engine stays usable."""
+    eng = ob.Engine(0)
+    lib, ctx = eng._lib, eng._ctx
+    ref, tars = render_series(96, 80, 2)
+    seeds = ob.make_poi2d(synth.grid_2d(40, 40, 2, 2, 10, 10))
+    n = len(seeds)
+    out = np.full((2, n, 25), 7.0, np.float32)
+    counts = np.full(2, 99, np.uint64)
+    vp = lambda a: None if a is None else ctypes.c_void_p(a.ctypes.data)
+
+    def call(order=None, r=8, s=seeds, o=out, count=n):
+        return method.c_series(lib, ctx, "", order, vp(s), vp(o), count, r)
+
+    def reseed(order=None, r=8, fr=8, zmin=0.5, s=seeds, o=out, count=n):
+        return method.c_series(lib, ctx, "_reseed", order, vp(s), vp(o), count, r, fr, fr, zmin, vp(counts))
+
+    assert call() == _capi.OCB_ERR_STATE and reseed() == _capi.OCB_ERR_STATE
+    assert lib.ocb_set_series_2d(ctx, vp(ref), vp(tars), 0, 96, 80) == _capi.OCB_ERR_ARG
+    assert lib.ocb_set_series_2d(ctx, vp(ref), None, 2, 96, 80) == _capi.OCB_ERR_ARG
+    assert call() == _capi.OCB_ERR_STATE and reseed() == _capi.OCB_ERR_STATE  # the refused calls set nothing
+    assert lib.ocb_set_series_2d(ctx, vp(ref), vp(tars), 2, 96, 80) == _capi.OCB_OK
+    bad = [dict(r=0), dict(s=None), dict(o=None), dict(count=1 << 40)] + ([] if method.kind == "nr" else [dict(order=0), dict(order=3)])
+    for kw in bad:
+        assert call(**kw) == _capi.OCB_ERR_ARG and reseed(**kw) == _capi.OCB_ERR_ARG, kw
+    too_large = "nr2d1: subset radius" if method.kind == "nr" else "exceeds the shared-memory design limit"
+    for c in (call, reseed):
+        assert c(r=200) == _capi.OCB_ERR_UNSUPPORTED and too_large in _capi.last_error(ctx)
+    assert reseed(zmin=float("nan")) == _capi.OCB_ERR_ARG
+    assert reseed(fr=0) == _capi.OCB_ERR_ARG
+    assert reseed(fr=37) == _capi.OCB_ERR_UNSUPPORTED and "prime factor > 31" in _capi.last_error(ctx)
+    assert method.c_series(lib, ctx, "_dev", None, None, None, 5, 8) == _capi.OCB_ERR_ARG
+    assert method.c_series(lib, ctx, "_reseed_dev", None, None, None, 5, 8, 8, 8, 0.5, vp(counts)) == _capi.OCB_ERR_ARG
+    assert (out == 7.0).all() and (counts == 99).all()
+    assert call() == _capi.OCB_OK and not (out == 7.0).all()  # the engine is still usable
+    out[:] = 7.0
+    assert reseed() == _capi.OCB_OK and not (out == 7.0).all() and (counts < 99).all()
+    eng.close()

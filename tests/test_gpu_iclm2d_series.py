@@ -3,13 +3,9 @@ loop of pair calls
     set_images_2d(ref, tars[f]); icgn2d_prepare(); iclm2d(order, q, ..., damping)
 gives when one queue q is carried from frame to frame, with the warps per POI forced (OCB_ICGN2D_WPP) so that the pair calls
 split their sums as the series launch over all POIs does."""
-import ctypes
-
-import numpy as np
 import pytest
 
-import opencorr_b200 as ob
-from opencorr_b200 import _capi, synth
+from opencorr_b200 import _capi
 import subset_series_cases as sc
 
 pytestmark = pytest.mark.gpu
@@ -54,41 +50,7 @@ def test_series_chunks(engine, stacks):
 
 
 def test_series_errors_leave_out_untouched():
-    eng = ob.Engine(0)
-    lib, ctx = eng._lib, eng._ctx
-    ref, tars = sc.render_series(96, 80, 2)
-    seeds = ob.make_poi2d(synth.grid_2d(40, 40, 2, 2, 10, 10))
-    n = len(seeds)
-    out = np.full((2, n, 25), 7.0, np.float32)
-    counts = np.full(2, 99, np.uint64)
-    vp = lambda a: ctypes.c_void_p(a.ctypes.data)
-
-    def call(order=1, r=8, s=seeds, o=out, count=n):
-        return lib.ocb_iclm2d_series(ctx, order, vp(s) if s is not None else None, vp(o) if o is not None else None, count, r, r, sc.CONV,
-                                     sc.STOP, 100.0, 0.1, 10.0)
-
-    def reseed(order=1, r=8, fr=8, zmin=0.5):
-        return lib.ocb_iclm2d_series_reseed(ctx, order, vp(seeds), vp(out), n, r, r, sc.CONV, sc.STOP, 100.0, 0.1, 10.0, fr, fr, zmin, vp(counts))
-
-    assert call() == _capi.OCB_ERR_STATE and reseed() == _capi.OCB_ERR_STATE
-    assert lib.ocb_set_series_2d(ctx, vp(ref), vp(tars), 2, 96, 80) == _capi.OCB_OK
-    assert call(order=3) == _capi.OCB_ERR_ARG and reseed(order=0) == _capi.OCB_ERR_ARG
-    assert call(s=None) == _capi.OCB_ERR_ARG
-    assert call(o=None) == _capi.OCB_ERR_ARG
-    assert call(count=1 << 40) == _capi.OCB_ERR_ARG
-    assert call(r=200) == _capi.OCB_ERR_UNSUPPORTED
-    assert "exceeds the shared-memory design limit" in _capi.last_error(ctx)
-    assert reseed(zmin=float("nan")) == _capi.OCB_ERR_ARG
-    assert reseed(fr=0) == _capi.OCB_ERR_ARG
-    assert reseed(fr=37) == _capi.OCB_ERR_UNSUPPORTED
-    assert "prime factor > 31" in _capi.last_error(ctx)
-    assert reseed(r=200) == _capi.OCB_ERR_UNSUPPORTED
-    assert lib.ocb_iclm2d_series_dev(ctx, 1, None, None, 5, 8, 8, sc.CONV, sc.STOP, 100.0, 0.1, 10.0) == _capi.OCB_ERR_ARG
-    assert (out == 7.0).all() and (counts == 99).all()
-    assert call() == _capi.OCB_OK  # the engine is still usable
-    assert not (out == 7.0).all()
-    assert reseed() == _capi.OCB_OK and (counts < 99).all()
-    eng.close()
+    sc.check_errors_leave_out_untouched(sc.Method("iclm", 1))
 
 
 def test_pair_state_undisturbed(engine, stacks):

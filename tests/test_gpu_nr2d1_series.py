@@ -2,14 +2,12 @@
 loop of pair calls
     set_images_2d(ref, tars[f]); nr2d_prepare(); nr2d1(q, ...)
 gives when one queue q is carried from frame to frame."""
-import ctypes
-
 import numpy as np
 import pytest
 
-import opencorr_b200 as ob
 from opencorr_b200 import _capi, synth
 import subset_series_cases as sc
+from util import assert_same
 
 pytestmark = pytest.mark.gpu
 
@@ -59,7 +57,7 @@ def test_failed_codes_follow_the_pair_guard(engine, stacks):
     expect = sc.pair_loop(engine, NR, ref, tars, seeds, 16)
     engine.set_series_2d(ref, tars)
     got = NR.series(engine, seeds, 16)
-    sc.assert_same(got, expect, "failed seeds")
+    assert_same(got, expect, "failed seeds")
     assert (got[:, 0, 16] == -1).all() and (got[:, 1, 16] == -4).all() and (got[:, 2, 16] == -5).all()
 
 
@@ -69,40 +67,7 @@ def test_series_chunks(engine, stacks):
 
 
 def test_series_errors_leave_out_untouched():
-    eng = ob.Engine(0)
-    lib, ctx = eng._lib, eng._ctx
-    ref, tars = sc.render_series(96, 80, 2)
-    seeds = ob.make_poi2d(synth.grid_2d(40, 40, 2, 2, 10, 10))
-    n = len(seeds)
-    out = np.full((2, n, 25), 7.0, np.float32)
-    counts = np.full(2, 99, np.uint64)
-    vp = lambda a: ctypes.c_void_p(a.ctypes.data)
-
-    def call(r=8, s=seeds, o=out, count=n):
-        return lib.ocb_nr2d1_series(ctx, vp(s) if s is not None else None, vp(o) if o is not None else None, count, r, r, sc.CONV, sc.STOP)
-
-    def reseed(r=8, fr=8, zmin=0.5):
-        return lib.ocb_nr2d1_series_reseed(ctx, vp(seeds), vp(out), n, r, r, sc.CONV, sc.STOP, fr, fr, zmin, vp(counts))
-
-    assert call() == _capi.OCB_ERR_STATE and reseed() == _capi.OCB_ERR_STATE
-    assert lib.ocb_set_series_2d(ctx, vp(ref), vp(tars), 2, 96, 80) == _capi.OCB_OK
-    assert call(r=0) == _capi.OCB_ERR_ARG
-    assert call(s=None) == _capi.OCB_ERR_ARG
-    assert call(o=None) == _capi.OCB_ERR_ARG
-    assert call(count=1 << 40) == _capi.OCB_ERR_ARG
-    assert call(r=200) == _capi.OCB_ERR_UNSUPPORTED
-    assert "nr2d1: subset radius" in _capi.last_error(ctx)
-    assert reseed(zmin=float("nan")) == _capi.OCB_ERR_ARG
-    assert reseed(fr=0) == _capi.OCB_ERR_ARG
-    assert reseed(fr=37) == _capi.OCB_ERR_UNSUPPORTED
-    assert "prime factor > 31" in _capi.last_error(ctx)
-    assert reseed(r=200) == _capi.OCB_ERR_UNSUPPORTED
-    assert lib.ocb_nr2d1_series_dev(ctx, None, None, 5, 8, 8, sc.CONV, sc.STOP) == _capi.OCB_ERR_ARG
-    assert (out == 7.0).all() and (counts == 99).all()
-    assert call() == _capi.OCB_OK  # the engine is still usable
-    assert not (out == 7.0).all()
-    assert reseed() == _capi.OCB_OK and (counts < 99).all()
-    eng.close()
+    sc.check_errors_leave_out_untouched(NR)
 
 
 def test_pair_state_undisturbed(engine, stacks):

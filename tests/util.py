@@ -36,6 +36,13 @@ def al_foam_crop():
     return d["ref"].astype(np.float32), d["tar"].astype(np.float32), int(d["z_offset"]), d["cpu_table"], d["gpu_table"]
 
 
+def assert_same(a, b, label):
+    """a and b hold the same float32 bits (a NaN equals only the same NaN)"""
+    assert a.shape == b.shape, label
+    bad = a.view(np.uint32) != b.view(np.uint32)
+    assert not bad.any(), "%s: %d floats differ, first at %s" % (label, bad.sum(), np.argwhere(bad)[:5].tolist())
+
+
 def compare_2d(a, b, label="", tol_disp=1e-4, tol_zncc=1e-5, max_iter_mismatch_frac=0.01, order=1, flip_tol_disp=1e-3, flip_tol_zncc=1e-4):
     """a, b: POI2D arrays [n,25].  Sentinel codes and integer outputs must agree exactly on every POI;
     displacement/ZNCC tolerances (north_star: 1e-4 px, 1e-5) apply to POIs whose iteration counts
