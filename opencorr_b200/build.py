@@ -48,8 +48,8 @@ def build(force=False, verbose=False, variant=None, variant_flags=(), variant_so
     under lib/obj/ so that only stale sources are recompiled.
 
     variant: build lib/variants/<variant>.so instead (A/B experiments, selected at run time with OCB_LIB_PATH): the
-    sources named in variant_sources are compiled with variant_flags added (e.g. -DICGN3D_PAIRS=0), the rest is linked
-    from the regular objects."""
+    sources named in variant_sources are compiled with variant_flags added (e.g. -DNAME=VALUE for a macro an experiment
+    tests), the rest is linked from the regular objects."""
     if variant is None and not force and not is_stale():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)

@@ -3,9 +3,10 @@ the launches the call made (launch_count() delta).  Two builds of the library (s
 and do the same work print the same lines.
 
 Calls: FFTCC2D (all three kernels), FFTCC3D, ICGN2D1, ICGN2D2, ICGN2D_EX (centre offsets; self-adaptive), ICLM2D, NR2D1,
-EpipolarSearch, Strain (2D, 3D, POI2DS, single POI), ICGN3D1 and stereo reconstruction, with host buffers and with device
-pointers.  Host queues include one of >= 16384 records (the four-stream pipeline) and one page-locked queue (read and written in
-place), and every call that shards a host queue also runs once on a one-member group context.
+EpipolarSearch, Strain (2D, 3D, POI2DS, single POI), ICGN3D1 (every kernel variant; sheared guesses) and stereo reconstruction,
+with host buffers and with device pointers.  Host queues include one of >= 16384 records (the four-stream pipeline) and one
+page-locked queue (read and written in place), and every call that shards a host queue also runs once on a one-member group
+context.
 
     python tools/pair_digest.py > a.txt; OCB_LIB_PATH=other.so python tools/pair_digest.py > b.txt; diff a.txt b.txt
 """
@@ -24,6 +25,7 @@ from opencorr_b200.api import POI2D_FLOATS, POI2DS_FLOATS, POI3D_FLOATS  # noqa:
 
 CONV, STOP = 0.001, 10.0
 W, H, D = 512, 384, 64
+DL = 96  # room for a 61^3 subvolume
 FUND = np.array([0, 0, 0, 0, 0, -1, 0, 1, 0], np.float32)  # a rectified pair
 PAR = np.zeros(3, np.float32)
 ST = (40.0, 6, 0.5, 1)  # strain: radius, min_neighbors, zncc_threshold, approximation
@@ -81,8 +83,8 @@ def queue_2d(step=20, margin=40):
     return q
 
 
-def queue_3d(step=8, margin=16):
-    k = (D - 2 * margin) // step + 1
+def queue_3d(step=8, margin=16, dim=D):
+    k = (dim - 2 * margin) // step + 1
     xyz = synth.grid_3d(margin, margin, margin, k, k, k, step, step, step)
     q = np.zeros((len(xyz), POI3D_FLOATS), np.float32)
     q[:, :3] = xyz
@@ -163,6 +165,26 @@ def run_3d(run, lib, ctx, group):
     run.host("strain3d_single", lambda p: lib.ocb_strain3d_single(ctx, p, n, 3, *ST), out)
 
 
+def run_3d_kernels(run, lib, ctx):
+    """ICGN3D1 at every kernel it selects, on a DL^3 pair: <16,256> (tail column), a generic <0,512> radius, <30,512>, and a
+    queue whose guesses carry shears of three sizes, so that both row-pair samples of a step fall in different blocks (small
+    shears) and whole slabs leave the tile (large ones)."""
+    r3, t3 = synth.speckle_pair_3d(DL, DL, DL)
+    assert lib.ocb_set_images_3d(ctx, vp(r3), vp(t3), DL, DL, DL) == 0
+    assert lib.ocb_icgn3d_prepare(ctx) == 0
+    q = queue_3d(step=12, margin=32, dim=DL)
+    n = len(q)
+    seeds = run.host("fftcc3d r=8 D=%d" % DL, lambda p: lib.ocb_fftcc3d(ctx, p, n, 8, 8, 8), q)[0]
+    for r in (16, 22, 30):
+        run.host("icgn3d1 r=%d" % r, lambda p: lib.ocb_icgn3d1(ctx, p, n, r, r, r, CONV, 20.0), seeds)
+    sheared = seeds.copy()
+    scale = np.array([0.01, 0.03, 0.15], np.float32)[np.arange(n) % 3]
+    for k, g in zip((4, 5, 6, 8, 9, 10, 12, 13, 14), (0.4, -0.6, 0.5, 0.7, 0.3, -0.5, -0.6, 0.8, 0.2)):  # ux uy uz vx vy vz wx wy wz
+        sheared[:, k] = scale * g
+    for r in (8, 16):
+        run.host("icgn3d1 r=%d sheared" % r, lambda p: lib.ocb_icgn3d1(ctx, p, n, r, r, r, CONV, 20.0), sheared)
+
+
 def run_stereo(run, lib, ctx):
     intr = np.array([900, 905, 0.5, W / 2, H / 2, 0.01, -0.002, 0, 0, 0, 0, 0.001, -0.001], np.float32)
     cal = []
@@ -205,6 +227,7 @@ def main():
     run = Runner(lib, ctx, "single")
     run_2d(run, lib, ctx, False)
     run_3d(run, lib, ctx, False)
+    run_3d_kernels(run, lib, ctx)
     run_stereo(run, lib, ctx)
     grun = Runner(lib, group, "group")
     run_2d(grun, lib, group, True)

@@ -2,7 +2,7 @@
 buffer, the reseeded counts and the launches the call made (launch_count() delta).  Two builds of the library (selected with
 OCB_LIB_PATH) that compute the same and do the same work print the same lines.
 
-Calls: the image series (ICGN2D1 and ICGN2D2), the volume series (float and 8-bit stacks) and the stereo series, each with host
+Calls: the image series (ICGN2D1, ICGN2D2 and NR2D1), the volume series (float and 8-bit stacks) and the stereo series, each with host
 buffers and with device pointers, plain and re-seeding (2D and 3D) at three zncc_min.
 
     python tools/series_digest.py > a.txt; OCB_LIB_PATH=other.so python tools/series_digest.py > b.txt; diff a.txt b.txt
@@ -74,6 +74,13 @@ def run_2d(eng):
             b = eng.launch_count()
             counts = eng.icgn2d_series_reseed_dev(order, d_seeds.data_ptr(), d_out.data_ptr(), len(seeds), 16, 16, CONV, STOP, 16, 16, zmin)
             report("icgn2d_series_reseed_dev order=%d zmin=%g" % (order, zmin), eng, b, [host_of(d_out)], counts)
+    eng.set_series_2d(ref, tars)
+    b = eng.launch_count()
+    report("nr2d1_series", eng, b, [eng.nr2d1_series(seeds, 16, 16, CONV, STOP)])
+    for zmin in ZMINS:
+        b = eng.launch_count()
+        out, counts = eng.nr2d1_series_reseed(seeds, 16, 16, CONV, STOP, 16, 16, zmin)
+        report("nr2d1_series_reseed zmin=%g" % zmin, eng, b, [out], counts)
 
 
 def run_3d(eng):
