@@ -30,9 +30,6 @@
 //   update  : solve with the Cholesky factors, compose W <- W * W(dp)^-1 in registers.
 // Samples whose 4x4 support leaves the staged tile (large deformation gradients) are read from
 // global memory instead, so results never depend on the tile size.
-#include <stdlib.h>
-#include <string.h>
-
 #include <type_traits>
 
 #include "ocb_kernels.h"
@@ -587,22 +584,18 @@ __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__
 	const int RW = icgn2d_ref_w(rx), RH = icgn2d_ref_h(ry);
 	const int TW = icgn2d_tar_w(rx), TH = icgn2d_tar_h(ry);
 	float* slab = smem;
-	uint64_t* bar = (uint64_t*)slab;
 	int* s_poi = (int*)(slab + 8);              // WPP > 1: the POI index fetched by thread 0
 	float* T = slab + 32;
 	float* sC = T + icgn2d_tile_floats(rx, ry); // per-sample constants, interleaved {R, gx, gy} (12-byte lane stride: conflict-free)
 	float* sH = sC + round_up32(3 * N);         // LM only: the undamped Hessian, packed lower triangle
 	float* sRedS = sH + (LM ? 96 : 0);          // WPP > 1: setup partials [WPP][ICGN2D_RED_SETUP]
 	float* sRedI = sRedS + WPP * ICGN2D_RED_SETUP; // WPP > 1: iteration partials [2][WPP][ICGN2D_RED_ITER]
-	uint32_t bar_phase = 0;
 	auto gsync = [&]() { // all warps of this POI
 		if constexpr (WPP > 1) __syncthreads();
 		else __syncwarp();
 	};
-	if (use_tma) {
-		if (poi_leader) mbar_init(bar, 1);
-		gsync();
-	}
+	TileLoad tiles = { (uint64_t*)slab, 0, use_tma };
+	tiles.init(poi_leader, gsync);
 	const float* __restrict__ ref = img.ref;
 	const int w = img.w, h = img.h;
 	const float inv_n = 1.0f / (float)N;
@@ -645,18 +638,21 @@ __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__
 		for (int f = 0; f < (SERIES ? n_frames : 1); f++) {
 			float* P = SERIES ? frames_out + ((size_t)f * n_poi + poi) * P2_N : pois + (size_t)poi * P2_N;
 			const float* __restrict__ tar = SERIES ? img.tar + (size_t)f * w * h : img.tar;
+			// a rejected POI: only the ZNCC field changes, to `code`; SERIES stores the whole record, the next frame's seed
+			auto store_rejection = [&](float code) {
+				if constexpr (SERIES) {
+					if (lane == P2_ZNCC) rec = code;
+					if (threadIdx.x < P2_N) P[lane] = rec;
+				} else {
+					if (poi_leader) P[P2_ZNCC] = code;
+				}
+			};
 			const float u_in = __shfl_sync(0xffffffffu, rec, P2_DEF + D2_U);
 			const float v_in = __shfl_sync(0xffffffffu, rec, P2_DEF + D2_V);
 			const float zncc_in = __shfl_sync(0xffffffffu, rec, P2_ZNCC);
 			// guard, reference src/oc_icgn.cpp:160-167 / :701-708 (NaN coordinates are rejected too)
-			if (py - ry < 0 || px - rx < 0 || py + ry > h - 1 || px + rx > w - 1 || fabsf(u_in) >= w || fabsf(v_in) >= h
-				|| zncc_in < 0 || is_nan_f(u_in) || is_nan_f(v_in) || is_nan_f(px) || is_nan_f(py)) {
-				if constexpr (SERIES) {
-					if (lane == P2_ZNCC) rec = zncc_in >= 0 ? -3.f : zncc_in;
-					if (threadIdx.x < P2_N) P[lane] = rec;
-				} else {
-					if (poi_leader) P[P2_ZNCC] = zncc_in >= 0 ? -3.f : zncc_in;
-				}
+			if (subset2d_guard_fails(px, py, rx, ry, w, h, u_in, v_in, zncc_in)) {
+				store_rejection(zncc_in >= 0 ? -3.f : zncc_in);
 				continue;
 			}
 			gsync(); // every warp has read the record before thread 0 may write results / TMA may overwrite the slab
@@ -676,18 +672,8 @@ __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__
 				// ---------------- stage the reference tile ----------------
 				const int x0 = (int)px - rx, y0 = (int)py - ry; // Subset2D::fill upper-left, src/oc_subset.cpp:41-42
 				const int rox = floor4(x0 - 2), ex = (x0 - 2) - rox; // 16-byte aligned tile origin, column offset 0..3
-				if (use_tma) {
-					if (poi_leader) {
-						fence_proxy_async(); // earlier generic-proxy accesses to T are ordered before the async-proxy write
-						mbar_expect_tx(bar, (uint32_t)(RW * RH * sizeof(float)));
-						tma_load_2d(T, &tm_ref, rox, y0 - 2, bar);
-					}
-					mbar_wait(bar, bar_phase);
-					bar_phase ^= 1;
-				} else {
-					if (sub == 0) stage_tile(T, ref, w, h, rox, y0 - 2, RW, RH, 0.f, lane);
-					gsync();
-				}
+				tiles.issue<false>(T, &tm_ref, ref, w, h, rox, y0 - 2, 0, RW, RH, poi_leader, sub == 0, lane);
+				tiles.wait(gsync);
 				c0 = T[(ry + 2) * RW + rx + 2 + ex]; // pilot value: the centre pixel
 
 				// ---------------- setup: R', gradients, factored Hessian sums ----------------
@@ -793,23 +779,21 @@ __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__
 			if constexpr (WPP == 1) __syncwarp();
 			const int tx0 = floor4((int)floorf(pcx + u_in) - rx - 1 - ICGN2D_TILE_MARGIN);
 			const int ty0 = (int)floorf(pcy + v_in) - ry - 1 - ICGN2D_TILE_MARGIN;
-			if (use_tma) {
-				if (poi_leader) {
-					fence_proxy_async();
-					mbar_expect_tx(bar, (uint32_t)(TW * TH * sizeof(float)));
-					if constexpr (SERIES) tma_load_3d(T, &tm_tar, tx0, ty0, f, bar);
-					else tma_load_2d(T, &tm_tar, tx0, ty0, bar);
-				}
-				mbar_wait(bar, bar_phase);
-				bar_phase ^= 1;
-			} else {
-				if (sub == 0) stage_tile(T, tar, w, h, tx0, ty0, TW, TH, 0.f, lane);
-				gsync();
-			}
+			tiles.issue<SERIES>(T, &tm_tar, tar, w, h, tx0, ty0, f, TW, TH, poi_leader, sub == 0, lane);
+			tiles.wait(gsync);
 			// a sample is "fast" when it is valid (src/oc_cubic_bspline.cpp:137-142) AND its support is in the tile
 			const float xlo = fmaxf(1.f, (float)(tx0 + 1)), xhi = fminf((float)(w - 2), (float)(tx0 + TW - 2));
 			const float ylo = fmaxf(1.f, (float)(ty0 + 1)), yhi = fminf((float)(h - 2), (float)(ty0 + TH - 2));
 			const float xmax = (float)(w - 2), ymax = (float)(h - 2);
+			// the checked sample at (X, Y): false when it is outside the interpolant's domain (NaN too) and IC-GN rejects the POI;
+			// otherwise t is the sample, from the tile when its support is there, and IC-LM takes the interpolant's -1 outside
+			auto sample_checked = [&](float X, float Y, float& t) {
+				const bool fast = (X >= xlo) && (X < xhi) && (Y >= ylo) && (Y < yhi);
+				const bool ok = fast || ((X >= 1.f) && (Y >= 1.f) && (X < xmax) && (Y < ymax));
+				if (!ok && !LM) return false;
+				t = ok ? bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, fast) : -1.f; // BicubicBspline::compute returns -1 outside
+				return true;
+			};
 
 			// ---------------- IC-GN iterations ----------------
 			Warp W;
@@ -989,15 +973,12 @@ __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__
 				} else {
 					for (int r = r_lo; r < r_hi; r++) {
 						const float yl = (float)(r - ry) - oy;
-						float X, Y;
+						float X, Y, t;
 						col.at(pcx, pcy, yl, X, Y);
 						if (lane_on) {
-							const bool fast = (X >= xlo) && (X < xhi) && (Y >= ylo) && (Y < yhi);
-							const bool ok = fast || ((X >= 1.f) && (Y >= 1.f) && (X < xmax) && (Y < ymax)); // NaN fails
-							if (!ok && !LM) {
+							if (!sample_checked(X, Y, t)) {
 								invalid = true;
 							} else {
-								const float t = ok ? bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, fast) : -1.f; // BicubicBspline::compute returns -1 outside
 								tmin = fminf(tmin, t);
 								const float* pc = sC + 3 * (r * sw + lane);
 								ps.add_row(t - pc[0], pc[0], pc[1], pc[2], yl);
@@ -1034,16 +1015,14 @@ __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__
 					for (int idx = sub * 32 + lane; idx < ntail; idx += 32 * WPP) {
 						const int r = idx / rem, c = 32 + (idx - r * rem);
 						const float xl = (float)(c - rx) - ox, yl = (float)(r - ry) - oy;
-						float X, Y;
+						float X, Y, t;
 						W.at(pcx, pcy, xl, yl, X, Y);
-						const bool fast = (X >= xlo) && (X < xhi) && (Y >= ylo) && (Y < yhi);
-						const bool ok = fast || ((X >= 1.f) && (Y >= 1.f) && (X < xmax) && (Y < ymax));
-						if (!ok && !LM) {
+						if (whole) t = T[wofs + r * TW + c] + 0.f; // a whole-pixel pass has every sample in the tile
+						else if (!sample_checked(X, Y, t)) {
 							invalid = true;
-						} else {
-							const float t = whole ? T[wofs + r * TW + c] + 0.f : ok ? bicubic_sample(T, TW, tx0, ty0, tar, w, X, Y, fast) : -1.f;
-							tail_sums(r, c, xl, yl, t);
+							continue;
 						}
+						tail_sums(r, c, xl, yl, t);
 					}
 				}
 				if constexpr (!LM) { // src/oc_icgn.cpp:251-255: any sample < 0 rejects the POI (the ICLM siblings have no such test)
@@ -1102,12 +1081,7 @@ __device__ __forceinline__ void icgn2d_poi_loop(Image2D img, float* __restrict__
 			} while ((float)iteration < stop_condition && dp_norm >= conv_criterion);
 
 			if (left_image) {
-				if constexpr (SERIES) {
-					if (lane == P2_ZNCC) rec = -3.f;
-					if (threadIdx.x < P2_N) P[lane] = rec;
-				} else {
-					if (poi_leader) P[P2_ZNCC] = -3.f;
-				}
+				store_rejection(-3.f);
 				__syncwarp();
 				continue;
 			}
@@ -1175,21 +1149,22 @@ __global__ void __launch_bounds__(32 * WPP, icgn2d_min_ctas(NP, RC, WPP)) icgn2d
 }
 
 // host-side launch ---------------------------------------------------------------------------
-typedef void (*Icgn2dKernel)(Image2D, float*, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int, const float*, float, float, float);
-typedef void (*Icgn2dSeriesKernel)(Image2D, const float*, float*, int, int, int, int, float, float, int*, const CUtensorMap, const CUtensorMap, int,
-	float, float, float);
-
-template <int WPP>
-static Icgn2dKernel icgn2d_pick(int np, int rc, bool lm) {
-	if (lm) return (np == 6) ? icgn2d_kernel<6, 0, true, WPP> : icgn2d_kernel<12, 0, true, WPP>;
-	if (np == 6) return rc == 16 ? icgn2d_kernel<6, 16, false, WPP> : icgn2d_kernel<6, 0, false, WPP>;
-	return rc == 20 ? icgn2d_kernel<12, 20, false, WPP> : icgn2d_kernel<12, 0, false, WPP>;
+template <bool SERIES, int NP, int RC, bool LM, int WPP>
+static constexpr auto icgn2d_kernel_of() {
+	if constexpr (SERIES) return icgn2d_series_kernel<NP, RC, LM, WPP>;
+	else return icgn2d_kernel<NP, RC, LM, WPP>;
 }
-template <int WPP>
-static Icgn2dSeriesKernel icgn2d_series_pick(int np, int rc, bool lm) {
-	if (lm) return (np == 6) ? icgn2d_series_kernel<6, 0, true, WPP> : icgn2d_series_kernel<12, 0, true, WPP>;
-	if (np == 6) return rc == 16 ? icgn2d_series_kernel<6, 16, false, WPP> : icgn2d_series_kernel<6, 0, false, WPP>;
-	return rc == 20 ? icgn2d_series_kernel<12, 20, false, WPP> : icgn2d_series_kernel<12, 0, false, WPP>;
+
+// the instantiation a launch runs: IC-LM has the generic radius only; IC-GN has r = 16 (6 parameters) and r = 20 (12 parameters)
+template <bool SERIES>
+static auto icgn2d_pick(int np, int rc, bool lm, int wpp) {
+	auto pick = [=](auto wpp_) {
+		constexpr int WPP = decltype(wpp_)::value;
+		if (lm) return np == 6 ? icgn2d_kernel_of<SERIES, 6, 0, true, WPP>() : icgn2d_kernel_of<SERIES, 12, 0, true, WPP>();
+		if (np == 6) return rc == 16 ? icgn2d_kernel_of<SERIES, 6, 16, false, WPP>() : icgn2d_kernel_of<SERIES, 6, 0, false, WPP>();
+		return rc == 20 ? icgn2d_kernel_of<SERIES, 12, 20, false, WPP>() : icgn2d_kernel_of<SERIES, 12, 0, false, WPP>();
+	};
+	return wpp == 2 ? pick(std::integral_constant<int, 2>()) : pick(std::integral_constant<int, 1>());
 }
 
 // The work-queue head of a launch: [0] of the context's heads, zeroed here, for two warps per POI; [32] for the one-warp-per-POI
@@ -1202,20 +1177,21 @@ static cudaError_t icgn2d_counter(const Icgn2dPlan& p, int** d_counter, cudaStre
 	return cudaMemsetAsync(*d_counter, 0, sizeof(int), stream);
 }
 
+// tensor maps of the reference image and of the target (n_frames == 0: one image; else the frame-major stack); 0: stage the tiles
+static int icgn2d_maps(const Image2D& img, int n_frames, int rx, int ry, CUtensorMap* tm_ref, CUtensorMap* tm_tar) {
+	return tma_enabled() && tma_image_map(tm_ref, img.ref, img.w, img.h, 0, icgn2d_ref_w(rx), icgn2d_ref_h(ry))
+		&& tma_image_map(tm_tar, img.tar, img.w, img.h, n_frames, icgn2d_tar_w(rx), icgn2d_tar_h(ry));
+}
+
 cudaError_t icgn2d_launch(int np, const Icgn2dPlan& p, const Image2D& img, float* d_pois, size_t n, int rx, int ry, float conv, float stop,
 	int* d_counter, const float* d_center_offsets, const float* lm_damping, cudaStream_t stream) {
 	const bool lm = lm_damping != nullptr;
 	cudaError_t e = icgn2d_counter(p, &d_counter, stream);
 	if (e != cudaSuccess) return e;
-	CUtensorMap tm_ref, tm_tar;
-	memset(&tm_ref, 0, sizeof(tm_ref));
-	memset(&tm_tar, 0, sizeof(tm_tar));
-	const int dims[2] = { img.w, img.h };
-	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[2] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry) };
-	const int use_tma = tma_enabled() && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tar, img.tar, 2, dims, box_tar);
-	Icgn2dKernel kern = p.wpp == 2 ? icgn2d_pick<2>(np, p.rc, lm) : icgn2d_pick<1>(np, p.rc, lm);
-	return launch_smem(kern, p.grid, p.wpp * 32, p.smem, stream, img, d_pois, (int)n, rx, ry, conv, stop, d_counter, tm_ref, tm_tar, use_tma,
-		d_center_offsets, lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
+	CUtensorMap tm_ref{}, tm_tar{};
+	const int use_tma = icgn2d_maps(img, 0, rx, ry, &tm_ref, &tm_tar);
+	return launch_smem(icgn2d_pick<false>(np, p.rc, lm, p.wpp), p.grid, p.wpp * 32, p.smem, stream, img, d_pois, (int)n, rx, ry, conv, stop,
+		d_counter, tm_ref, tm_tar, use_tma, d_center_offsets, lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
 }
 
 cudaError_t icgn2d_series_launch(int np, const Icgn2dPlan& p, const Image2D& img, int n_frames, const float* d_seeds, float* d_out, size_t n,
@@ -1223,15 +1199,10 @@ cudaError_t icgn2d_series_launch(int np, const Icgn2dPlan& p, const Image2D& img
 	const bool lm = lm_damping != nullptr;
 	cudaError_t e = icgn2d_counter(p, &d_counter, stream);
 	if (e != cudaSuccess) return e;
-	CUtensorMap tm_ref, tm_tars;
-	memset(&tm_ref, 0, sizeof(tm_ref));
-	memset(&tm_tars, 0, sizeof(tm_tars));
-	const int dims[3] = { img.w, img.h, n_frames };
-	const int box_ref[2] = { icgn2d_ref_w(rx), icgn2d_ref_h(ry) }, box_tar[3] = { icgn2d_tar_w(rx), icgn2d_tar_h(ry), 1 };
-	const int use_tma = tma_enabled() && tma_make_map(&tm_ref, img.ref, 2, dims, box_ref) && tma_make_map(&tm_tars, img.tar, 3, dims, box_tar);
-	Icgn2dSeriesKernel kern = p.wpp == 2 ? icgn2d_series_pick<2>(np, p.rc, lm) : icgn2d_series_pick<1>(np, p.rc, lm);
-	return launch_smem(kern, p.grid, p.wpp * 32, p.smem, stream, img, d_seeds, d_out, n_frames, (int)n, rx, ry, conv, stop, d_counter, tm_ref,
-		tm_tars, use_tma, lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
+	CUtensorMap tm_ref{}, tm_tars{};
+	const int use_tma = icgn2d_maps(img, n_frames, rx, ry, &tm_ref, &tm_tars);
+	return launch_smem(icgn2d_pick<true>(np, p.rc, lm, p.wpp), p.grid, p.wpp * 32, p.smem, stream, img, d_seeds, d_out, n_frames, (int)n, rx,
+		ry, conv, stop, d_counter, tm_ref, tm_tars, use_tma, lm ? lm_damping[0] : 0.f, lm ? lm_damping[1] : 0.f, lm ? lm_damping[2] : 0.f);
 }
 
 } // namespace ocb

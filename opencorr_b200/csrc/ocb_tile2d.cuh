@@ -1,8 +1,17 @@
-// ocb_tile2d.cuh -- per-warp 2D tile staging and bicubic B-spline sampling shared by icgn2d.cu and nr2d.cu.
+// ocb_tile2d.cuh -- the subset guard, per-warp 2D tile loads and bicubic B-spline sampling shared by icgn2d.cu and nr2d.cu.
 #pragma once
 #include "ocb_common.cuh"
+#include "ocb_tma.cuh"
 
 namespace ocb {
+
+// The reference's guard in front of a 2D subset registration (src/oc_icgn.cpp:160-167 / :701-708, src/oc_nr.cpp:165-171): the
+// subset must lie inside the image, the initial displacement within the image's extent and the incoming ZNCC not negative; NaN
+// coordinates fail too.  Each method writes its own code for a POI that fails it.
+__device__ __forceinline__ bool subset2d_guard_fails(float px, float py, int rx, int ry, int w, int h, float u, float v, float zncc) {
+	return py - ry < 0 || px - rx < 0 || py + ry > h - 1 || px + rx > w - 1 || fabsf(u) >= w || fabsf(v) >= h || zncc < 0 || is_nan_f(u)
+		|| is_nan_f(v) || is_nan_f(px) || is_nan_f(py);
+}
 
 // Stage a (rows x cols) window of a row-major image into smem (row pitch `cols`), origin (ox, oy),
 // subtracting `shift`; pixels outside the image read as -shift.  Lanes run along x (coalesced).
@@ -19,6 +28,49 @@ __device__ __forceinline__ void stage_tile(float* dst, const float* __restrict__
 			dst[row * cols + col] = v - shift;
 		}
 	}
+}
+
+// A (cols x rows) tile load into smem for the threads of one POI: a TMA copy completing on the mbarrier `bar` when the launch has
+// a tensor map, otherwise stage_tile by one warp.  issue() starts the load and wait() returns once the tile may be read, so work
+// that does not touch the tile can run in between.  sync: the barrier of the POI's threads.
+struct TileLoad {
+	uint64_t* bar;
+	uint32_t phase;
+	int tma; // the launch has a tensor map
+	template <class Sync>
+	__device__ __forceinline__ void init(bool leader, Sync sync) {
+		if (tma) {
+			if (leader) mbar_init(bar, 1);
+			sync();
+		}
+	}
+	// STACK: map is 3D over a frame-major stack (box depth 1) and the tile comes from frame z; img is that frame.
+	// leader issues the TMA copy; stager (a whole warp) stages the tile without one.
+	template <bool STACK>
+	__device__ __forceinline__ void issue(float* dst, const CUtensorMap* map, const float* __restrict__ img, int w, int h, int x, int y, int z,
+		int cols, int rows, bool leader, bool stager, int lane) {
+		if (tma) {
+			if (leader) {
+				fence_proxy_async(); // earlier generic-proxy accesses to dst are ordered before the async-proxy write
+				mbar_expect_tx(bar, (uint32_t)(cols * rows * sizeof(float)));
+				if constexpr (STACK) tma_load_3d(dst, map, x, y, z, bar);
+				else tma_load_2d(dst, map, x, y, bar);
+			}
+		} else if (stager) stage_tile(dst, img, w, h, x, y, cols, rows, 0.f, lane);
+	}
+	// a TMA tile is visible to every thread that waited on the barrier; a staged one after sync()
+	template <class Sync>
+	__device__ __forceinline__ void wait(Sync sync) {
+		if (tma) { mbar_wait(bar, phase); phase ^= 1; }
+		else sync();
+	}
+};
+
+// Tensor map for tile loads from one row-major (w x h) image (n_frames == 0: 2D) or from a frame-major stack of n_frames of them
+// (3D, box depth 1: a load reads one frame).  false: no map can be made (see tma_make_map) and the launch stages its tiles.
+inline bool tma_image_map(CUtensorMap* map, const float* base, int w, int h, int n_frames, int box_w, int box_h) {
+	const int dims[3] = { w, h, n_frames }, box[3] = { box_w, box_h, 1 };
+	return tma_make_map(map, base, n_frames > 0 ? 3 : 2, dims, box);
 }
 
 // The interpolant over one 4x4 block: each block row folded with the x weights, then the rows with the y weights, in this
