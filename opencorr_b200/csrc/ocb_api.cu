@@ -1622,53 +1622,51 @@ int ocb_epipolar_search2d(ocb_ctx* ctx, void* poi2d, size_t n, const float* fund
 }
 
 // ---- Strain (SURVEY.md section 8(f) N4) ---------------------------------------------------------------
-static int strain_dev(ocb_ctx* ctx, int dim, void* d_poi, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation,
-	long long only = -1) {
+static_assert(ocb::poi_floats(ocb::PoiKind::POI2D) == OCB_POI2D_FLOATS && ocb::poi_floats(ocb::PoiKind::POI3D) == OCB_POI3D_FLOATS
+	&& ocb::poi_floats(ocb::PoiKind::POI2DS) == OCB_POI2DS_FLOATS, "the kernels' record lengths are the C ABI's");
+static int strain_dev(ocb_ctx* ctx, ocb::PoiKind kind, void* d_poi, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation, long long only = -1) {
 	int rc = pair_checks(ctx, "strain", d_poi, n, only < (long long)n, nullptr, 0, nullptr, true);
 	if (rc != PAIR_GO) return rc;
 	if ((rc = grow(ctx, ctx->d_strain_ws, ocb::strain_workspace_bytes(n)))) return rc;
-	const cudaError_t e = ocb::strain_launch(dim, (float*)d_poi, n, radius, min_neighbors, zncc_threshold, approximation, only, ctx->d_strain_ws.p,
+	const cudaError_t e = ocb::strain_launch(kind, (float*)d_poi, n, radius, min_neighbors, zncc_threshold, approximation, only, ctx->d_strain_ws.p,
 		ctx->sm_count, ctx->stream, &ctx->launches);
 	if (e != cudaSuccess) return set_error(ctx, OCB_ERR_CUDA, "strain launch failed: %s", cudaGetErrorString(e));
 	return OCB_OK;
 }
 
-static int strain_host(ocb_ctx* ctx, int dim, void* poi, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation,
+static int strain_host(ocb_ctx* ctx, ocb::PoiKind kind, void* poi, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation,
 	long long only = -1) {
-	if (is_group(ctx)) { // every POI needs its neighbours wherever they are in the queue: not sharded, the first member runs it
-		const int rc = strain_host(ctx->members[0], dim, poi, n, radius, min_neighbors, zncc_threshold, approximation, only);
-		if (rc) ctx->last_error = ctx->members[0]->last_error;
-		return rc;
-	}
-	const size_t rec_floats = dim == 2 ? OCB_POI2D_FLOATS : (dim == 3 ? OCB_POI3D_FLOATS : OCB_POI2DS_FLOATS);
-	return run_host_queue(ctx, "strain", poi, n, rec_floats, [&](float* d, size_t m, size_t) {
-		return strain_dev(ctx, dim, d, m, radius, min_neighbors, zncc_threshold, approximation, only);
+	if (is_group(ctx)) // every POI needs its neighbours wherever they are in the queue: not sharded, the first member runs it
+		return on_exec(ctx, [&](ocb_ctx* x) { return strain_host(x, kind, poi, n, radius, min_neighbors, zncc_threshold, approximation, only); });
+	return run_host_queue(ctx, "strain", poi, n, ocb::poi_floats(kind), [&](float* d, size_t m, size_t) {
+		return strain_dev(ctx, kind, d, m, radius, min_neighbors, zncc_threshold, approximation, only);
 	}, STAGED);
 }
 
 int ocb_strain2d(ocb_ctx* ctx, void* poi2d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_host(ctx, 2, poi2d, n, radius, min_neighbors, zncc_threshold, approximation);
+	return strain_host(ctx, ocb::PoiKind::POI2D, poi2d, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 int ocb_strain3d(ocb_ctx* ctx, void* poi3d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_host(ctx, 3, poi3d, n, radius, min_neighbors, zncc_threshold, approximation);
+	return strain_host(ctx, ocb::PoiKind::POI3D, poi3d, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 int ocb_strain2ds(ocb_ctx* ctx, void* poi2ds, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_host(ctx, 23, poi2ds, n, radius, min_neighbors, zncc_threshold, approximation);
+	return strain_host(ctx, ocb::PoiKind::POI2DS, poi2ds, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 int ocb_strain2ds_dev(ocb_ctx* ctx, void* d_poi2ds, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_dev(ctx, 23, d_poi2ds, n, radius, min_neighbors, zncc_threshold, approximation);
+	return strain_dev(ctx, ocb::PoiKind::POI2DS, d_poi2ds, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 int ocb_strain2d_single(ocb_ctx* ctx, void* poi2d, size_t n, size_t index, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_host(ctx, 2, poi2d, n, radius, min_neighbors, zncc_threshold, approximation, (long long)index);
+	return strain_host(ctx, ocb::PoiKind::POI2D, poi2d, n, radius, min_neighbors, zncc_threshold, approximation, (long long)index);
 }
 int ocb_strain3d_single(ocb_ctx* ctx, void* poi3d, size_t n, size_t index, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_host(ctx, 3, poi3d, n, radius, min_neighbors, zncc_threshold, approximation, (long long)index);
+	return strain_host(ctx, ocb::PoiKind::POI3D, poi3d, n, radius, min_neighbors, zncc_threshold, approximation, (long long)index);
 }
 int ocb_strain2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_dev(ctx, 2, d_poi2d, n, radius, min_neighbors, zncc_threshold, approximation);
+	return strain_dev(ctx, ocb::PoiKind::POI2D, d_poi2d, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 int ocb_strain3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
-	return strain_dev(ctx, 3, d_poi3d, n, radius, min_neighbors, zncc_threshold, approximation);
+	return strain_dev(ctx, ocb::PoiKind::POI3D, d_poi3d, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 
 // TricubicBspline::prepare: the B-spline coefficients of volume tar into coef, in three passes x -> coef, y -> tmp, z -> coef

@@ -16,6 +16,9 @@ enum { D2_U = 0, D2_UX = 1, D2_UY = 2, D2_UXX = 3, D2_UXY = 4, D2_UYY = 5,
 enum { P3_X = 0, P3_Y = 1, P3_Z = 2, P3_DEF = 3, P3_U0 = 15, P3_V0 = 16, P3_W0 = 17, P3_ZNCC = 18,
        P3_ITER = 19, P3_CONV = 20, P3_FEAT = 21, P3_STRAIN = 22, P3_RX = 28, P3_RY = 29, P3_RZ = 30, P3_N = 31 };
 // 3D deformation vector order: u ux uy uz v vx vy vz w wx wy wz
+// POI2DS (stereo DIC, src/oc_poi.h:140-186): x y | u v w | r1r2 r1t1 r1t2 ZNCC | r2_x r2_y t1_x t1_y t2_x t2_y | ref_coor |
+// tar_coor | e[6] | subset_radius
+enum { P2DS_U = 2, P2DS_ZNCC = 5, P2DS_REF = 14, P2DS_STRAIN = 20, P2DS_N = 28 };
 
 struct Image2D {
 	const float* ref;

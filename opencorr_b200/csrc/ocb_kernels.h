@@ -198,10 +198,54 @@ cudaError_t epipolar_candidates_launch(const float* d_pois, size_t poi0, size_t 
 	const float* parallax_y, int search_radius, int search_step, int rx, int ry, int w, int h, int slots, float* d_cand, int sm_count,
 	cudaStream_t stream);
 cudaError_t epipolar_select_launch(float* d_pois, size_t poi0, size_t n_poi, int slots, const float* d_cand, int sm_count, cudaStream_t stream);
-// strain.cu
+// strain.cu: Strain over a queue of POI2D, POI3D or POI2DS (stereo DIC) records
+enum class PoiKind { POI2D, POI3D, POI2DS };
+__host__ __device__ constexpr int poi_floats(PoiKind k) { return k == PoiKind::POI2D ? (int)P2_N : (k == PoiKind::POI3D ? (int)P3_N : (int)P2DS_N); }
+
+// The uniform grid the POIs are binned into: a position p lies in cell c_d = floor((p_d - lo_d) * inv_cell), clamped to
+// [0, nc_d), of key (c_2 nc_1 + c_1) nc_0 + c_0; a POI with a non-finite position takes the key n_cells.
+struct StrainGrid {
+	float lo[3];
+	float inv_cell;
+	int nc[3];
+	unsigned int n_cells;
+};
+
+// The grid over the bounding box [lo, hi] of the finite positions (axes d < dims) for the neighbour radius `radius`; returns
+// the cell edge.  The edge is >= |radius|, so that the 3^D block around a POI's cell holds every point within the radius (the
+// test is dist^2 < radius^2, so a negative radius acts as its magnitude); a non-finite radius takes one cell over the bbox
+// (+-inf: every POI is a neighbour, NaN: none is).  The edge doubles until the grid has < 2^30 cells.
+inline double strain_grid_plan(int dims, const float* lo, const float* hi, float radius, StrainGrid* g) {
+	float extent = 0.f;
+	for (int d = 0; d < 3; d++) {
+		g->lo[d] = d < dims ? lo[d] : 0.f;
+		const float h = d < dims ? hi[d] : 0.f;
+		if (h - g->lo[d] > extent) extent = h - g->lo[d];
+	}
+	const float abs_radius = fabsf(radius);
+	double cell = !isfinite(abs_radius) ? (double)extent + 1.0 : abs_radius > 0.f ? (double)abs_radius : (double)extent / 64.0 + 1.0;
+	if (!(cell > 0.0) || !isfinite(cell)) cell = 1.0;
+	while (true) {
+		double total = 1.0;
+		for (int d = 0; d < 3; d++) {
+			const double cnt = d < dims ? floor(((double)hi[d] - (double)g->lo[d]) / cell) + 2.0 : 1.0;
+			g->nc[d] = (int)(cnt < 1.0 ? 1.0 : (cnt > 2e9 ? 2e9 : cnt));
+			total *= cnt;
+		}
+		if (total < 1073741824.0) break;
+		cell *= 2.0;
+	}
+	g->inv_cell = (float)(1.0 / cell);
+	// the float product (p - lo) * inv_cell may round a point's cell index by one; the neighbourhood scan needs
+	// |cell(p) - cell(q)| <= 1 for every pair within the radius, which holds with a 0.1 % safety margin on the edge
+	g->inv_cell *= 0.999f;
+	g->n_cells = (unsigned int)g->nc[0] * (unsigned int)g->nc[1] * (unsigned int)g->nc[2];
+	return cell;
+}
+
 size_t strain_workspace_bytes(size_t n);
-// *launches grows by the kernels it launched
-cudaError_t strain_launch(int dim, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only,
+// *launches grows by each kernel once it has launched (the radix sort counts as one)
+cudaError_t strain_launch(PoiKind kind, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only,
 	void* workspace, int sm_count, cudaStream_t stream, long long* launches);
 // FFTCC2D: which of the three kernels a window takes, and what that kernel needs
 constexpr int FFTW32_WARPS = 4;     // fftcc2d_w32.cu: one-POI warps per CTA

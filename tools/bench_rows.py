@@ -45,7 +45,8 @@ def main():
     eng.icgn2d1_dev(d_q.copy_(d_q0).data_ptr(), n, r, r, 0.001, 10)
     torch.cuda.synchronize()
     d_conv = d_q.clone()
-    q_conv = d_conv.cpu().numpy()
+    d_nan = d_conv.clone()
+    d_nan[n // 2, 0] = float("nan")  # one POI without a finite position: never binned, never a neighbour
 
     rows = {
         "ICGN2D1": (lambda p: lib.ocb_icgn2d1_dev(ctx, p, n, r, r, 0.001, 10.0), d_q0),
@@ -55,6 +56,7 @@ def main():
         "NR2D1": (lambda p: lib.ocb_nr2d1_dev(ctx, p, n, r, r, 0.001, 10.0), d_q0),
         "Strain2D(r=20,k=5)": (lambda p: lib.ocb_strain2d_dev(ctx, p, n, 20.0, 5, 0.9, 1), d_conv),
         "Strain2D(r=60,k=5)": (lambda p: lib.ocb_strain2d_dev(ctx, p, n, 60.0, 5, 0.9, 1), d_conv),
+        "Strain2D(r=20,k=5,one NaN x)": (lambda p: lib.ocb_strain2d_dev(ctx, p, n, 20.0, 5, 0.9, 1), d_nan),
     }
     o = Oracle2D(ref, tar)
     o.prepare()
@@ -68,6 +70,7 @@ def main():
         "NR2D1": lambda q: o.nr2d1(q, r, r, 0.001, 10),
         "Strain2D(r=20,k=5)": lambda q: oracle.strain(q, 20.0, 5, 0.9, 1),
         "Strain2D(r=60,k=5)": lambda q: oracle.strain(q, 60.0, 5, 0.9, 1),
+        "Strain2D(r=20,k=5,one NaN x)": lambda q: oracle.strain(q, 20.0, 5, 0.9, 1),
     }
     o.nr2d1(q_fft[:64].copy(), r, r, 0.001, 10)  # builds the NR tables outside the timed region
     for name, (fn, src) in rows.items():
@@ -87,7 +90,7 @@ def main():
         res = d_q.cpu().numpy()
         ms = float(np.median(ts))
         if name.startswith("Strain"):
-            cq = q_conv.copy()          # strain needs the whole queue (neighbour search): time it whole
+            cq = src.cpu().numpy()      # strain needs the whole queue (neighbour search): time it whole
             t0 = time.perf_counter()
             cpu[name](cq)
             cpu_s = time.perf_counter() - t0
