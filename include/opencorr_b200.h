@@ -309,6 +309,25 @@ int ocb_strain2ds(ocb_ctx* ctx, void* poi2ds, size_t n, float radius, int min_ne
 int ocb_strain2ds_dev(ocb_ctx* ctx, void* d_poi2ds, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation);
 int ocb_strain2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation);
 int ocb_strain3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation);
+/* Strain over a series: n_frames frames of n records each, frame-major (the layout the series calls write).  Frame f's records
+ * become, bit for bit, what ocb_strain*_dev(ctx, records + f * n * floats, n, ...) leaves on them, for every radius and
+ * approximation; the neighbours of each POI are searched once for all frames, and only the ZNCC filter, the displacements and
+ * (POI2DS) ref_coor are read per frame.  Every frame's search coordinates (x, y; POI3D: x, y, z) must be frame 0's, bit for
+ * bit (NaN included): otherwise OCB_ERR_ARG and nothing is written.  OCB_ERR_ARG as well, before any kernel runs, for NULL
+ * records with n_frames * n > 0 and for n_frames * n * floats floats that overflow a size_t; n per frame has the pair call's
+ * limit.  n_frames = 0 or n = 0 does nothing.  The host variants copy; the _dev variants take BORROWED device records and only
+ * enqueue (single-device context); a call makes the same launches and one readback whatever n_frames.  On a group context the
+ * first member runs the host variants. */
+int ocb_strain2d_series(ocb_ctx* ctx, void* poi2d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation);
+int ocb_strain3d_series(ocb_ctx* ctx, void* poi3d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation);
+int ocb_strain2ds_series(ocb_ctx* ctx, void* poi2ds, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation);
+int ocb_strain2d_series_dev(ocb_ctx* ctx, void* d_poi2d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation);
+int ocb_strain3d_series_dev(ocb_ctx* ctx, void* d_poi3d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation);
+int ocb_strain2ds_series_dev(ocb_ctx* ctx, void* d_poi2ds, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation);
 
 /* ---- Stereo reconstruction: Calibration::prepare / undistort (src/oc_calibration.cpp:161-264) and
  *      Stereovision::reconstruct (src/oc_stereovision.cpp:70-133) ----------------------------------------------------------
@@ -354,7 +373,7 @@ int ocb_stereo_reconstruct_dev(ocb_ctx* ctx, const ocb_calib* calib1, const floa
  *   t2 = out2[f] location + (u, v), stored unclamped; ZNCCs r1r2 / r1t1 / r1t2 of stereo / out1[f] / out2[f] (failure codes
  *   included); ref_coor = reconstruct((x, y), r2), tar_coor = reconstruct(t1, t2), where reconstruct is ocb_stereo_reconstruct on
  *   copies of the points (clamped per camera; a NaN coordinate gives (0, 0, 0)); u, v, w = tar_coor - ref_coor; strain and
- *   subset_radius 0.  Strain over frame f: ocb_strain2ds(ctx, out2ds + f * n * OCB_POI2DS_FLOATS, n, ...).
+ *   subset_radius 0.  Strain over every frame: ocb_strain2ds_series(ctx, out2ds, n_frames, n, ...).
  * out1, out2: n_frames x n POI2D records, out2ds: n_frames x n POI2DS records, frame-major, overlapping no input.  A long series
  *   runs in chunks: the last frame's slices of out1 and out2 seed the next chunk.
  * The host variants copy (ocb_stereo_series blocks until the outputs are filled); the _dev variants take BORROWED device images,

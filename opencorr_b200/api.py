@@ -23,6 +23,7 @@ from . import _capi
 POI2D_FLOATS = 25
 POI3D_FLOATS = 31
 POI2DS_FLOATS = 28
+_STRAIN_SERIES = {POI2D_FLOATS: "2d", POI3D_FLOATS: "3d", POI2DS_FLOATS: "2ds"}  # record floats -> ocb_strain*_series suffix
 P2 = dict(x=0, y=1, u=2, ux=3, uy=4, uxx=5, uxy=6, uyy=7, v=8, vx=9, vy=10, vxx=11, vxy=12, vyy=13,
           u0=14, v0=15, zncc=16, iteration=17, convergence=18, feature=19, exx=20, eyy=21, exy=22,
           subset_rx=23, subset_ry=24)
@@ -379,6 +380,23 @@ class Engine:
             _check_queue(q, POI2D_FLOATS)
             fn = self._lib.ocb_strain2d
         self._ck(fn(self._ctx, _vp(q), q.shape[0], float(radius), int(min_neighbors), float(zncc_threshold), int(approximation)))
+
+    def strain_series(self, q, radius, min_neighbors, zncc_threshold=0.9, approximation=1):
+        """strain on every frame of a series, q a C-contiguous float32 [n_frames, n, floats] array of POI2D (25), POI3D (31) or
+        POI2DS (28) records whose positions are the same in every frame (include/opencorr_b200.h ocb_strain2d_series): each
+        frame's records become those strain leaves on that frame, with each POI's neighbours searched once."""
+        if not isinstance(q, np.ndarray) or q.dtype != np.float32 or q.ndim != 3 or q.shape[2] not in _STRAIN_SERIES \
+                or not q.flags.c_contiguous:
+            raise ValueError("strain_series takes a C-contiguous float32 array of shape [n_frames, n, 25 | 31 | 28]")
+        fn = getattr(self._lib, "ocb_strain%s_series" % _STRAIN_SERIES[q.shape[2]])
+        self._ck(fn(self._ctx, _vp(q), q.shape[0], q.shape[1], float(radius), int(min_neighbors), float(zncc_threshold), int(approximation)))
+
+    def strain_series_dev(self, kind, d_q, n_frames, n, radius, min_neighbors, zncc_threshold=0.9, approximation=1):
+        """strain_series on device records (a pointer as an int); kind "2d", "3d" or "2ds".  Only enqueues."""
+        if kind not in _STRAIN_SERIES.values():
+            raise ValueError("kind must be '2d', '3d' or '2ds'")
+        fn = getattr(self._lib, "ocb_strain%s_series_dev" % kind)
+        self._ck(fn(self._ctx, int(d_q), n_frames, n, float(radius), int(min_neighbors), float(zncc_threshold), int(approximation)))
 
     def nr2d_prepare(self):
         self._ck(self._lib.ocb_nr2d_prepare(self._ctx))

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdarg.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -1667,6 +1668,58 @@ int ocb_strain2d_dev(ocb_ctx* ctx, void* d_poi2d, size_t n, float radius, int mi
 }
 int ocb_strain3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
 	return strain_dev(ctx, ocb::PoiKind::POI3D, d_poi3d, n, radius, min_neighbors, zncc_threshold, approximation);
+}
+
+// Strain over a series: n_frames frames of n records, frame-major.  Their bytes, n_frames n rec_floats floats, must fit a size_t.
+static bool strain_series_fits(ocb::PoiKind kind, size_t n_frames, size_t n) {
+	const size_t rec = (size_t)ocb::poi_floats(kind) * sizeof(float);
+	return n == 0 || (n <= SIZE_MAX / rec && n_frames <= SIZE_MAX / (n * rec));
+}
+
+static int strain_series_dev(ocb_ctx* ctx, ocb::PoiKind kind, void* d_poi, size_t n_frames, size_t n, float radius, int min_neighbors,
+	float zncc_threshold, int approximation) {
+	int rc = pair_checks(ctx, "strain_series", d_poi, n_frames ? n : 0, strain_series_fits(kind, n_frames, n), nullptr, 0, nullptr, true);
+	if (rc != PAIR_GO) return rc;
+	if ((rc = grow(ctx, ctx->d_strain_ws, ocb::strain_workspace_bytes(n, n_frames)))) return rc;
+	bool moved = false;
+	const cudaError_t e = ocb::strain_series_launch(kind, (float*)d_poi, n_frames, n, radius, min_neighbors, zncc_threshold, approximation,
+		ctx->d_strain_ws.p, ctx->sm_count, ctx->stream, &ctx->launches, &moved);
+	if (e != cudaSuccess) return set_error(ctx, OCB_ERR_CUDA, "strain_series launch failed: %s", cudaGetErrorString(e));
+	if (moved) return set_error(ctx, OCB_ERR_ARG, "strain_series: the POI positions of some frame are not those of frame 0");
+	return OCB_OK;
+}
+
+static int strain_series_host(ocb_ctx* ctx, ocb::PoiKind kind, void* poi, size_t n_frames, size_t n, float radius, int min_neighbors,
+	float zncc_threshold, int approximation) {
+	if (is_group(ctx)) // as strain_host: the first member runs it
+		return on_exec(ctx, [&](ocb_ctx* x) { return strain_series_host(x, kind, poi, n_frames, n, radius, min_neighbors, zncc_threshold, approximation); });
+	if (!ctx || !strain_series_fits(kind, n_frames, n)) return set_error(ctx, OCB_ERR_ARG, "strain_series: bad arguments");
+	return run_host_queue(ctx, "strain_series", poi, n_frames * n, ocb::poi_floats(kind), [&](float* d, size_t, size_t) {
+		return strain_series_dev(ctx, kind, d, n_frames, n, radius, min_neighbors, zncc_threshold, approximation);
+	}, STAGED);
+}
+
+int ocb_strain2d_series(ocb_ctx* ctx, void* poi2d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
+	return strain_series_host(ctx, ocb::PoiKind::POI2D, poi2d, n_frames, n, radius, min_neighbors, zncc_threshold, approximation);
+}
+int ocb_strain3d_series(ocb_ctx* ctx, void* poi3d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold, int approximation) {
+	return strain_series_host(ctx, ocb::PoiKind::POI3D, poi3d, n_frames, n, radius, min_neighbors, zncc_threshold, approximation);
+}
+int ocb_strain2ds_series(ocb_ctx* ctx, void* poi2ds, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation) {
+	return strain_series_host(ctx, ocb::PoiKind::POI2DS, poi2ds, n_frames, n, radius, min_neighbors, zncc_threshold, approximation);
+}
+int ocb_strain2d_series_dev(ocb_ctx* ctx, void* d_poi2d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation) {
+	return strain_series_dev(ctx, ocb::PoiKind::POI2D, d_poi2d, n_frames, n, radius, min_neighbors, zncc_threshold, approximation);
+}
+int ocb_strain3d_series_dev(ocb_ctx* ctx, void* d_poi3d, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation) {
+	return strain_series_dev(ctx, ocb::PoiKind::POI3D, d_poi3d, n_frames, n, radius, min_neighbors, zncc_threshold, approximation);
+}
+int ocb_strain2ds_series_dev(ocb_ctx* ctx, void* d_poi2ds, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
+	int approximation) {
+	return strain_series_dev(ctx, ocb::PoiKind::POI2DS, d_poi2ds, n_frames, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 
 // TricubicBspline::prepare: the B-spline coefficients of volume tar into coef, in three passes x -> coef, y -> tmp, z -> coef

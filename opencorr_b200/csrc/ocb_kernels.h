@@ -243,10 +243,16 @@ inline double strain_grid_plan(int dims, const float* lo, const float* hi, float
 	return cell;
 }
 
-size_t strain_workspace_bytes(size_t n);
+// the workspace of a call over n_frames frames of n POIs (the pair call: one frame)
+size_t strain_workspace_bytes(size_t n, size_t n_frames = 1);
 // *launches grows by each kernel once it has launched (the radix sort counts as one)
 cudaError_t strain_launch(PoiKind kind, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only,
 	void* workspace, int sm_count, cudaStream_t stream, long long* launches);
+// Strain over n_frames frames of n records each, frame-major, whose search coordinates are the same in every frame: frame f's records
+// become those strain_launch leaves on them, with one readback and the same launches for any n_frames.  When some frame's
+// search coordinates differ from frame 0's as bits, *moved is set and nothing is written.
+cudaError_t strain_series_launch(PoiKind kind, float* d_pois, size_t n_frames, size_t n, float radius, int k_min, float zncc_threshold,
+	int approximation, void* workspace, int sm_count, cudaStream_t stream, long long* launches, bool* moved);
 // FFTCC2D: which of the three kernels a window takes, and what that kernel needs
 constexpr int FFTW32_WARPS = 4;     // fftcc2d_w32.cu: one-POI warps per CTA
 constexpr int FFTREG_THREADS = 128; // fftcc2d_reg.cu: one thread per window row, 128 / N POIs per CTA

@@ -15,6 +15,9 @@
 // search -- with coalesced 16-byte loads, and accumulates the normal equations in FP64 (12 / 22
 // sums per lane, shuffle-reduced).  Lane 0 solves the 3x3 / 4x4 system with pivoting.  The rare
 // k-nearest fallback is k brute-force selection passes over the sorted array by the same warp.
+//
+// Over a series of frames that share their positions (strain_series_kernel), the bbox, grid and sort run once on frame 0 and
+// each POI's neighbours are searched once; only the fits run per frame.
 #include <stdint.h>
 #include <string.h>
 
@@ -55,13 +58,24 @@ __device__ __forceinline__ bool finite_position(const float* p) {
 	return fin;
 }
 
-// bbox[0..2] = min (ordered encoding), bbox[3..5] = max, bbox[6] += the POIs with a finite position
-template <PoiKind K>
-__global__ void strain_bbox_kernel(const float* __restrict__ pois, int n, unsigned int* __restrict__ bbox) {
+// bbox[0..2] = min (ordered encoding), bbox[3..5] = max, bbox[6] += the POIs with a finite position.  SERIES: the records are
+// frame 0 of n_frames frames of n records each, and bbox[7] += the POIs whose search coordinates differ, as bits, in some frame
+// from frame 0's.
+template <PoiKind K, bool SERIES>
+__global__ void strain_bbox_kernel(const float* __restrict__ pois, int n, unsigned int* __restrict__ bbox, size_t n_frames) {
 	constexpr int D = SL<K>::SD;
-	unsigned int mn[3] = { 0xffffffffu, 0xffffffffu, 0xffffffffu }, mx[3] = { 0u, 0u, 0u }, finite = 0;
+	unsigned int mn[3] = { 0xffffffffu, 0xffffffffu, 0xffffffffu }, mx[3] = { 0u, 0u, 0u }, finite = 0, moved = 0;
 	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const float* p = pois + (size_t)i * poi_floats(K);
+		if (SERIES) {
+			for (size_t f = 1; f < n_frames; f++) {
+				const float* pf = p + f * (size_t)n * poi_floats(K);
+				bool same = true;
+#pragma unroll
+				for (int d = 0; d < D; d++) same = same && __float_as_uint(pf[d]) == __float_as_uint(p[d]);
+				if (!same) { moved++; break; }
+			}
+		}
 		if (!finite_position<K>(p)) continue;
 		finite++;
 #pragma unroll
@@ -74,6 +88,10 @@ __global__ void strain_bbox_kernel(const float* __restrict__ pois, int n, unsign
 	// one atomic per warp and field; the count is per lane because the grid-stride loop ends at different trips per lane
 	finite = __reduce_add_sync(0xffffffffu, finite);
 	if ((threadIdx.x & 31) == 0) atomicAdd(bbox + 6, finite);
+	if (SERIES) {
+		moved = __reduce_add_sync(0xffffffffu, moved);
+		if ((threadIdx.x & 31) == 0 && moved) atomicAdd(bbox + 7, moved);
+	}
 #pragma unroll
 	for (int d = 0; d < D; d++) {
 		mn[d] = __reduce_min_sync(0xffffffffu, mn[d]);
@@ -127,6 +145,27 @@ __global__ void strain_gather_kernel(const float* __restrict__ pois, int n, cons
 		pos[s] = make_float4(p[0], p[1], L::SD == 3 ? p[2] : 0.f, good ? 1.f : 0.f);
 		disp[s] = make_float4(p[L::U], p[L::V], L::FD == 3 ? p[L::W] : 0.f, 0.f);
 		if (L::FC != 0) fpos[s] = make_float4(p[L::FC], p[L::FC + 1], p[L::FC + 2], 0.f);
+	}
+}
+
+// The series' sorted, compact copies of the n_valid POIs with a finite position, over n_frames frames of n records:
+// pos[n_valid] = frame 0's {x, y, z|0, 0} (every frame's, as the bbox pass checked), and frame-major [n_frames][n_valid]
+// disp = {u, v, w|0, fit flag} and fpos (POI2DS: ref_coor) of each frame
+template <PoiKind K>
+__global__ void strain_series_gather_kernel(const float* __restrict__ pois, int n, size_t n_frames, int n_valid, const int* __restrict__ order,
+	float zncc_threshold, float4* __restrict__ pos, float4* __restrict__ disp, float4* __restrict__ fpos) {
+	typedef SL<K> L;
+	const size_t total = n_frames * (size_t)n_valid;
+	for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
+		const size_t f = t / (size_t)n_valid;
+		const int s = (int)(t - f * (size_t)n_valid);
+		const float* p = pois + (f * (size_t)n + (size_t)order[s]) * poi_floats(K);
+		bool good = true;
+#pragma unroll
+		for (int k = 0; k < L::NZ; k++) good = good && (p[L::Z0 + k] >= zncc_threshold);
+		if (f == 0) pos[s] = make_float4(p[0], p[1], L::SD == 3 ? p[2] : 0.f, 0.f);
+		disp[t] = make_float4(p[L::U], p[L::V], L::FD == 3 ? p[L::W] : 0.f, good ? 1.f : 0.f);
+		if (L::FC != 0) fpos[t] = make_float4(p[L::FC], p[L::FC + 1], p[L::FC + 2], 0.f);
 	}
 }
 
@@ -320,6 +359,60 @@ __device__ __forceinline__ void knn_fallback(FitSums<SL<K>::FD>& sums, const flo
 	}
 }
 
+// The series kernel's forms of radius_scan and knn_fallback: the same search, lane for lane and pass for pass, with what is done
+// with each neighbour left to the caller.  (The pair kernel keeps its own two so that its code stays as it is.)
+//
+// radius_scan's search: each lane calls visit(j, pos[j]) for the POIs of its share within the radius, in the order it meets
+// them.  Returns how many are within the radius (warp total).
+template <int D, class Visit>
+__device__ __forceinline__ int radius_visit(const float4& centre, int run_lo, int run_hi, float r2, const float4* __restrict__ pos, int lane,
+	Visit visit) {
+	int found = 0;
+#pragma unroll 1
+	for (int row = 0; row < (D == 2 ? 3 : 9); row++) {
+		const int lo = __shfl_sync(0xffffffffu, run_lo, row), hi = __shfl_sync(0xffffffffu, run_hi, row);
+		for (int j = lo + lane; j < hi; j += 32) {
+			const float4 q = __ldg(pos + j);
+			if (dist2<D>(centre, q) < r2) {
+				found++;
+				visit(j, q);
+			}
+		}
+	}
+	return __reduce_add_sync(0xffffffffu, found);
+}
+
+// knn_fallback's search: the whole warp calls visit(j) with the sorted index j of each of the k_min nearest POIs, nearest first.
+template <int D, class Visit>
+__device__ __forceinline__ void knn_visit(const float4& centre, int k_min, int n_valid, const int* __restrict__ order, const float4* __restrict__ pos,
+	int lane, Visit visit) {
+	float prev_d = -1.f;
+	int prev_i = -1;
+	const int k = k_min < n_valid ? k_min : n_valid;
+#pragma unroll 1
+	for (int pass = 0; pass < k; pass++) {
+		float bd = INFINITY;
+		int bi = 0x7fffffff, bs = -1;
+		for (int j = lane; j < n_valid; j += 32) {
+			const float d = dist2<D>(centre, __ldg(pos + j));
+			const int oi = __ldg(order + j);
+			const bool after = d > prev_d || (d == prev_d && oi > prev_i);
+			if (after && (d < bd || (d == bd && oi < bi))) { bd = d; bi = oi; bs = j; }
+		}
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) {
+			const float od = __shfl_xor_sync(0xffffffffu, bd, o);
+			const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+			const int os = __shfl_xor_sync(0xffffffffu, bs, o);
+			if (od < bd || (od == bd && oi < bi)) { bd = od; bi = oi; bs = os; }
+		}
+		if (bs < 0) break;
+		prev_d = bd;
+		prev_i = bi;
+		visit(bs);
+	}
+}
+
 // Lane 0, with the warp's sums: the plane fit, then the strains of POI `poi` from the displacement gradients
 // g_ki = G[k][i] = d u_k / d x_i (u, v, w over x, y, z): e_xx e_yy e_xy (FD = 2) or e_xx e_yy e_zz e_xy e_yz e_zx (FD = 3).
 // Green (approximation 2, src/oc_strain.cpp:229-235, :455-463): e_ii = g_ii + 1/2 sum_k g_ki^2, e_ij = 1/2 (g_ij + g_ji +
@@ -381,26 +474,101 @@ __global__ void __launch_bounds__(256) strain_kernel(float* __restrict__ pois, i
 	}
 }
 
-// Device workspace of a call over n POIs (one grow-only allocation owned by the context), regions 256-byte aligned:
-//   bbox[7] | keys_in[n] | keys_out[n] | vals_in[n] | vals_out[n] | pos[n] | disp[n] | fpos[n] | cub temp.  base null: sizes only.
+// The indices a lane keeps of its radius-search neighbours (a warp: 32 x this), and the most k-nearest neighbours a warp keeps
+constexpr int STRAIN_LIST = 32;
+constexpr int STRAIN_SERIES_THREADS = 256;
+
+// Strain over n_frames frames of n records that share their positions: one warp per sorted POI s < n_valid.  The neighbour search
+// runs once: each lane keeps the sorted indices its share of radius_visit met within the radius, in the order it met them (or lane
+// 0, the k-nearest visit's selection order).  Then per frame in which the POI's own ZNCC passes, the lanes replay their lists
+// against that frame's disp (fit flag in .w) and fpos, so that each lane adds the same neighbours in the same order as the pair
+// kernel does and the warp reduction is the same: every frame's records are bit for bit those of strain_kernel on that frame.
+// A POI whose lists outgrow STRAIN_LIST per lane (or STRAIN_LIST x 32 nearest) searches again in every frame instead.
+template <PoiKind K>
+__global__ void __launch_bounds__(STRAIN_SERIES_THREADS) strain_series_kernel(float* __restrict__ pois, size_t n, size_t n_frames, int n_valid, StrainGrid g,
+	const unsigned int* __restrict__ keys, const int* __restrict__ order, const float4* __restrict__ pos, const float4* __restrict__ disp,
+	const float4* __restrict__ fpos, float radius, int k_min, int approximation) {
+	typedef SL<K> L;
+	__shared__ int lists[STRAIN_SERIES_THREADS / 32][STRAIN_LIST * 32];
+	int* const list = lists[threadIdx.x >> 5];
+	const int lane = threadIdx.x & 31;
+	const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	const int n_warps = (gridDim.x * blockDim.x) >> 5;
+	const float r2 = __fmul_rn(radius, radius);
+	for (int s = warp_global; s < n_valid; s += n_warps) {
+		bool fitted = false; // the POI's own ZNCC passes in some frame
+		for (size_t f = lane; f < n_frames; f += 32) fitted = fitted || __ldg(disp + f * n_valid + s).w != 0.f;
+		if (!__any_sync(0xffffffffu, fitted)) continue;
+		const float4 centre = __ldg(pos + s);
+		int run_lo, run_hi;
+		neighbour_runs<L::SD>(g, centre, keys, n_valid, lane, run_lo, run_hi);
+		int kept = 0; // radius: this lane's list length; k-nearest: the warp's
+		const bool knn = radius_visit<L::SD>(centre, run_lo, run_hi, r2, pos, lane, [&](int j, const float4&) {
+			if (kept < STRAIN_LIST) list[kept * 32 + lane] = j;
+			kept++;
+		}) < k_min;
+		bool again; // search again in every frame
+		if (knn) {
+			kept = 0;
+			again = (k_min < n_valid ? k_min : n_valid) > STRAIN_LIST * 32;
+			if (!again) knn_visit<L::SD>(centre, k_min, n_valid, order, pos, lane, [&](int j) {
+				if (lane == 0) list[kept] = j;
+				kept++;
+			});
+		} else {
+			again = __any_sync(0xffffffffu, kept > STRAIN_LIST);
+		}
+		__syncwarp();
+		const int poi = __ldg(order + s);
+		for (size_t f = 0; f < n_frames; f++) {
+			const float4* const fdisp = disp + f * n_valid;
+			const float4* const ffpos = fpos + f * n_valid;
+			if (__ldg(fdisp + s).w == 0.f) continue; // below the threshold in this frame
+			const float4 fcentre = L::FC != 0 ? __ldg(ffpos + s) : centre;
+			FitSums<L::FD> sums;
+			sums.clear();
+			const auto add = [&](int j) {
+				const float4 dq = __ldg(fdisp + j);
+				if (dq.w != 0.f) sums.add(fcentre, L::FC != 0 ? __ldg(ffpos + j) : __ldg(pos + j), dq);
+			};
+			if (again && knn) {
+				knn_visit<L::SD>(centre, k_min, n_valid, order, pos, lane, [&](int j) { if (lane == 0) add(j); });
+			} else if (again) {
+				radius_visit<L::SD>(centre, run_lo, run_hi, r2, pos, lane, [&](int j, const float4&) { add(j); });
+			} else if (knn) {
+				if (lane == 0)
+					for (int t = 0; t < kept; t++) add(list[t]);
+			} else {
+				for (int t = 0; t < kept; t++) add(list[t * 32 + lane]);
+			}
+			sums.reduce();
+			if (lane == 0 && sums.a[0] >= (double)k_min) fit_and_write<K>(sums, pois + f * n * poi_floats(K), poi, approximation);
+		}
+		__syncwarp(); // the lists are rewritten by the next POI
+	}
+}
+
+// Device workspace of a call over n_frames frames of n POIs (one grow-only allocation owned by the context), regions 256-byte
+// aligned: bbox[8] | keys_in[n] | keys_out[n] | vals_in[n] | vals_out[n] | pos[n] | disp[n_frames n] | fpos[n_frames n] | cub temp.
+// base null: sizes only.
 struct StrainWs {
 	unsigned int *bbox, *keys_in, *keys_out;
 	int *vals_in, *vals_out;
 	float4 *pos, *disp, *fpos;
 	void* cub_temp;
 	size_t cub_bytes = 0, bytes = 0;
-	StrainWs(void* base, size_t n) {
+	StrainWs(void* base, size_t n, size_t n_frames) {
 		cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const unsigned int*)nullptr, (unsigned int*)nullptr, (const int*)nullptr, (int*)nullptr,
 			(int)n);
 		auto take = [&](size_t b) { const uintptr_t p = (uintptr_t)base + bytes; bytes += (b + 255) & ~(size_t)255; return (void*)p; };
-		bbox = (unsigned int*)take(7 * sizeof(unsigned int));
+		bbox = (unsigned int*)take(8 * sizeof(unsigned int));
 		keys_in = (unsigned int*)take(n * 4);
 		keys_out = (unsigned int*)take(n * 4);
 		vals_in = (int*)take(n * 4);
 		vals_out = (int*)take(n * 4);
 		pos = (float4*)take(n * 16);
-		disp = (float4*)take(n * 16);
-		fpos = (float4*)take(n * 16);
+		disp = (float4*)take(n_frames * n * 16);
+		fpos = (float4*)take(n_frames * n * 16);
 		cub_temp = take(cub_bytes);
 	}
 };
@@ -412,21 +580,28 @@ cudaError_t launched(long long* launches) {
 	return e;
 }
 
-// bbox and finite count (the call's one readback), keys, sort, gather, strain
+// bbox and finite count (the call's one readback), keys, sort, gather, strain.  moved null: the pair call over n records
+// (`only`: Strain::compute(POI*, queue)); else the series over n_frames frames of n records, which sets *moved instead of
+// writing anything when the positions of some frame are not frame 0's.
 template <PoiKind K>
-cudaError_t strain_run(float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only, const StrainWs& w,
-	int sm_count, cudaStream_t stream, long long* launches) {
+cudaError_t strain_run(float* d_pois, size_t n, size_t n_frames, float radius, int k_min, float zncc_threshold, int approximation, long long only,
+	const StrainWs& w, int sm_count, cudaStream_t stream, long long* launches, bool* moved) {
 	const int threads = 256;
 	int blocks = (int)((n + threads - 1) / threads);
 	if (blocks > sm_count * 8) blocks = sm_count * 8;
 	if (blocks < 1) blocks = 1;
 	cudaError_t e;
-	unsigned int hb[7] = { 0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u };
+	unsigned int hb[8] = { 0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u, 0u };
 	if ((e = cudaMemcpyAsync(w.bbox, hb, sizeof(hb), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-	strain_bbox_kernel<K><<<blocks, threads, 0, stream>>>(d_pois, (int)n, w.bbox);
+	if (n_frames > 1) strain_bbox_kernel<K, true><<<blocks, threads, 0, stream>>>(d_pois, (int)n, w.bbox, n_frames);
+	else strain_bbox_kernel<K, false><<<blocks, threads, 0, stream>>>(d_pois, (int)n, w.bbox, n_frames);
 	if ((e = launched(launches)) != cudaSuccess || (e = cudaMemcpyAsync(hb, w.bbox, sizeof(hb), cudaMemcpyDeviceToHost, stream)) != cudaSuccess
 		|| (e = cudaStreamSynchronize(stream)) != cudaSuccess)
 		return e;
+	if (hb[7]) {
+		*moved = true;
+		return cudaSuccess;
+	}
 	// exactly the POIs with a finite position get keys below the sentinel, so they lead the sorted order
 	const int n_valid = (int)hb[6];
 	if (n_valid == 0) return cudaSuccess;
@@ -441,26 +616,50 @@ cudaError_t strain_run(float* d_pois, size_t n, float radius, int k_min, float z
 	if ((e = cub::DeviceRadixSort::SortPairs(w.cub_temp, cub_bytes, w.keys_in, w.keys_out, w.vals_in, w.vals_out, (int)n, 0, end_bit, stream)) != cudaSuccess)
 		return e;
 	++*launches;
-	strain_gather_kernel<K><<<blocks, threads, 0, stream>>>(d_pois, (int)n, w.vals_out, zncc_threshold, w.pos, w.disp, w.fpos);
-	if ((e = launched(launches)) != cudaSuccess) return e;
 	long long grid = ((long long)n_valid * 32 + threads - 1) / threads;
 	if (grid > (long long)sm_count * 8) grid = (long long)sm_count * 8;
-	strain_kernel<K><<<(int)grid, threads, 0, stream>>>(d_pois, n_valid, g, w.keys_out, w.vals_out, w.pos, w.disp, w.fpos, radius, k_min, approximation,
-		(int)only);
+	if (!moved) {
+		strain_gather_kernel<K><<<blocks, threads, 0, stream>>>(d_pois, (int)n, w.vals_out, zncc_threshold, w.pos, w.disp, w.fpos);
+		if ((e = launched(launches)) != cudaSuccess) return e;
+		strain_kernel<K><<<(int)grid, threads, 0, stream>>>(d_pois, n_valid, g, w.keys_out, w.vals_out, w.pos, w.disp, w.fpos, radius, k_min, approximation,
+			(int)only);
+		return launched(launches);
+	}
+	long long gather_blocks = (long long)((n_frames * (size_t)n_valid + threads - 1) / threads);
+	if (gather_blocks > (long long)sm_count * 8) gather_blocks = (long long)sm_count * 8;
+	strain_series_gather_kernel<K><<<(int)gather_blocks, threads, 0, stream>>>(d_pois, (int)n, n_frames, n_valid, w.vals_out, zncc_threshold, w.pos,
+		w.disp, w.fpos);
+	if ((e = launched(launches)) != cudaSuccess) return e;
+	strain_series_kernel<K><<<(int)grid, STRAIN_SERIES_THREADS, 0, stream>>>(d_pois, n, n_frames, n_valid, g, w.keys_out, w.vals_out, w.pos,
+		w.disp, w.fpos, radius, k_min, approximation);
 	return launched(launches);
 }
 
 } // namespace
 
-size_t strain_workspace_bytes(size_t n) { return StrainWs(nullptr, n).bytes; }
+size_t strain_workspace_bytes(size_t n, size_t n_frames) { return StrainWs(nullptr, n, n_frames).bytes; }
 
 cudaError_t strain_launch(PoiKind kind, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only,
 	void* workspace, int sm_count, cudaStream_t stream, long long* launches) {
-	const StrainWs w(workspace, n);
+	const StrainWs w(workspace, n, 1);
 	switch (kind) {
-	case PoiKind::POI2D: return strain_run<PoiKind::POI2D>(d_pois, n, radius, k_min, zncc_threshold, approximation, only, w, sm_count, stream, launches);
-	case PoiKind::POI3D: return strain_run<PoiKind::POI3D>(d_pois, n, radius, k_min, zncc_threshold, approximation, only, w, sm_count, stream, launches);
-	default: return strain_run<PoiKind::POI2DS>(d_pois, n, radius, k_min, zncc_threshold, approximation, only, w, sm_count, stream, launches);
+	case PoiKind::POI2D: return strain_run<PoiKind::POI2D>(d_pois, n, 1, radius, k_min, zncc_threshold, approximation, only, w, sm_count, stream, launches, nullptr);
+	case PoiKind::POI3D: return strain_run<PoiKind::POI3D>(d_pois, n, 1, radius, k_min, zncc_threshold, approximation, only, w, sm_count, stream, launches, nullptr);
+	default: return strain_run<PoiKind::POI2DS>(d_pois, n, 1, radius, k_min, zncc_threshold, approximation, only, w, sm_count, stream, launches, nullptr);
+	}
+}
+
+cudaError_t strain_series_launch(PoiKind kind, float* d_pois, size_t n_frames, size_t n, float radius, int k_min, float zncc_threshold,
+	int approximation, void* workspace, int sm_count, cudaStream_t stream, long long* launches, bool* moved) {
+	const StrainWs w(workspace, n, n_frames);
+	*moved = false;
+	switch (kind) {
+	case PoiKind::POI2D:
+		return strain_run<PoiKind::POI2D>(d_pois, n, n_frames, radius, k_min, zncc_threshold, approximation, -1, w, sm_count, stream, launches, moved);
+	case PoiKind::POI3D:
+		return strain_run<PoiKind::POI3D>(d_pois, n, n_frames, radius, k_min, zncc_threshold, approximation, -1, w, sm_count, stream, launches, moved);
+	default:
+		return strain_run<PoiKind::POI2DS>(d_pois, n, n_frames, radius, k_min, zncc_threshold, approximation, -1, w, sm_count, stream, launches, moved);
 	}
 }
 
