@@ -398,8 +398,12 @@ int ocb_stereo_series_dev(ocb_ctx* ctx, const ocb_calib* calib1, const float* in
  * (the constructor's defaults, :142-152: 3, -, 8, 0.1, 0.9, 0.4, 1.15, 1.6, 1e-10, 0.2 * 128 / 768).
  * unit_xyz: the physical voxel size (setPhysicalUnit :197-202); matching_ratio: setMatchingRatio (:204-207, default 0.85).
  * Blocking.  *n_matched = number of matched pairs; *n_octave = the computed octave count (written back to sift_config by the
- * reference).  Either pointer may be NULL.  Results stay in the context until the next ocb_sift3d call.  Where the reference is
- * undefined (a mirrored blur index still out of range, reads past the end of its match list) DESIGN.md defines the result.
+ * reference).  Either pointer may be NULL.  Results stay in the context until the next ocb_sift3d call.  A call that fails
+ * before any device work (its argument checks, the pyramid plan's n_octave_layers, volume size and blur radius, or selecting the
+ * device) leaves the previous call's results readable, bit for bit.  A call that fails once its device work has begun (a CUDA
+ * error, or OCB_ERR_ARG "too many keypoints") leaves none: ocb_sift3d_get_matches, _inspect and _stage_times then report that
+ * ocb_sift3d has not run.  Where the reference is undefined (a mirrored blur index still out of range, reads past the end of its
+ * match list) DESIGN.md defines the result.
  * On a GROUP context the first member runs it.  There is no CPU path. */
 #define OCB_SIFT3D_CONFIG_FLOATS 10
 #define OCB_SIFT3D_KP_FLOATS 18 /* coor_layer xyz, coor_img xyz, octave, layer, scale, R[9] (rows q0, q1, q0 x q1) */

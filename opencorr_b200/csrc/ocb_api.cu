@@ -105,19 +105,7 @@ struct ocb_worker {
 	}
 };
 
-// Grow-only device buffer of a context (see grow).  Released when the context is deleted, after ocb_destroy has made its
-// device current.
-struct DevBuf {
-	void* p = nullptr;
-	size_t bytes = 0;
-	DevBuf() = default;
-	DevBuf(const DevBuf&) = delete;
-	DevBuf& operator=(const DevBuf&) = delete;
-	~DevBuf() {
-		if (p) cudaFree(p);
-	}
-	template <class T> T* as() const { return (T*)p; }
-};
+using ocb::DevBuf; // a context's buffers are freed by `delete ctx` in ocb_destroy, with its device current
 
 // One series (ocb_set_series_2d*, ocb_set_series_3d*, ocb_set_stereo_series_2d*): a float reference against the frame-major
 // stacks tars[0] and (stereo) tars[1], `frames` frames of w x h x d pixels (d = 1: images) starting `pitch` bytes apart (a float
@@ -240,26 +228,10 @@ static int launched(ocb_ctx* ctx, const char* what, cudaError_t e) {
 	return OCB_OK;
 }
 
-// Make b hold at least `bytes` (on ctx's device, which must be current).  It only grows, and its contents are not kept across
-// a growth.  Work already enqueued on ctx->stream may still use the old allocation, so the stream is drained before it is
-// released.  If the allocation fails, b is left empty and the next call tries again; the failure is cleared from the runtime's
-// last error, which the next launch's check would otherwise report.
+// ocb::grow on ctx's device (current) and stream, contents not kept
 static int grow(ocb_ctx* ctx, DevBuf& b, size_t bytes) {
-	if (bytes <= b.bytes) return OCB_OK;
-	if (b.p) {
-		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		cudaFree(b.p);
-		b.p = nullptr;
-		b.bytes = 0;
-	}
-	const cudaError_t e = cudaMalloc(&b.p, bytes);
-	if (e != cudaSuccess) {
-		cudaGetLastError();
-		b.p = nullptr;
-		return set_error(ctx, OCB_ERR_CUDA, "cudaMalloc(&b.p, bytes) failed: %s", cudaGetErrorString(e));
-	}
-	b.bytes = bytes;
-	return OCB_OK;
+	const cudaError_t e = ocb::grow(b, bytes, ctx->stream);
+	return e == cudaSuccess ? OCB_OK : set_error(ctx, OCB_ERR_CUDA, "growing a device buffer to %zu bytes failed: %s", bytes, cudaGetErrorString(e));
 }
 
 static int get_twiddles(ocb_ctx* ctx, int n, const float2** out) {
@@ -891,7 +863,7 @@ void ocb_destroy(ocb_ctx* ctx) {
 	for (int i = 0; i < 4; i++)
 		if (ctx->band_done[i]) cudaEventDestroy(ctx->band_done[i]);
 	cudaFree(ctx->d_counter);
-	ocb::sift3d_destroy(ctx->sift3d);
+	delete ctx->sift3d;
 	cudaStreamDestroy(ctx->own_stream);
 	delete ctx; // frees the DevBuf members on this device
 }
@@ -2184,6 +2156,16 @@ int ocb_stereo_series(ocb_ctx* ctx, const ocb_calib* calib1, const float* intrin
 
 // ---- SIFT3D: SIFT3D::compute (src/oc_sift.cpp:234-293) --------------------------------------------------------------------
 // On a group context the first member runs it and keeps the results (one pair of volumes; see DESIGN.md section 6).
+
+// The pyramid of ocb_sift3d on ctx's volumes, or OCB_ERR_ARG with the check it fails
+static int sift3d_plan_or_error(ocb_ctx* ctx, const float* config, const float* unit_xyz, ocb::Sift3dPlan* plan) {
+	if (ocb::sift3d_plan(ctx->img3.dx, ctx->img3.dy, ctx->img3.dz, config, unit_xyz, plan)) return OCB_OK;
+	if (plan->reject == ocb::Sift3dReject::OCTAVE_LAYERS)
+		return set_error(ctx, OCB_ERR_ARG, "sift3d: n_octave_layers must be in [1, %d]", ocb::SIFT3D_MAX_L - 3);
+	if (plan->reject == ocb::Sift3dReject::VOLUME_SIZE) return set_error(ctx, OCB_ERR_ARG, "sift3d: volume too large");
+	return set_error(ctx, OCB_ERR_ARG, "sift3d: blur radius exceeds %d voxels (physical units too anisotropic)", ocb::SIFT3D_MAX_R);
+}
+
 int ocb_sift3d(ocb_ctx* ctx, const float* config, const float* unit_xyz, float matching_ratio, size_t* n_matched, int* n_octave) {
 	if (!ctx || !config || !unit_xyz) return set_error(ctx, OCB_ERR_ARG, "sift3d: null argument");
 	return on_exec(ctx, [&](ocb_ctx* x) -> int {
@@ -2191,14 +2173,21 @@ int ocb_sift3d(ocb_ctx* ctx, const float* config, const float* unit_xyz, float m
 		for (int a = 0; a < 3; a++)
 			if (!(unit_xyz[a] > 0.f) || !std::isfinite(unit_xyz[a])) return set_error(x, OCB_ERR_ARG, "sift3d: physical units must be positive");
 		if (!(config[0] >= 1.f) || !(config[2] >= 1.f)) return set_error(x, OCB_ERR_ARG, "sift3d: n_octave_layers and min_dimension must be >= 1");
+		ocb::Sift3dPlan plan;
+		if (const int rc = sift3d_plan_or_error(x, config, unit_xyz, &plan)) return rc;
 		if (ensure_device(x)) return OCB_ERR_CUDA;
-		if (!x->sift3d) x->sift3d = ocb::sift3d_create();
-		std::string err;
-		const int r = ocb::sift3d_run(x->sift3d, x->img3.ref, x->img3.tar, x->img3.dx, x->img3.dy, x->img3.dz, config, unit_xyz, matching_ratio, x->sm_count,
-			x->stream, &x->launches, &err);
-		if (r) return set_error(x, r == -2 ? OCB_ERR_ARG : OCB_ERR_CUDA, "%s", err.c_str());
-		if (n_matched) *n_matched = ocb::sift3d_n_matched(x->sift3d);
-		if (n_octave) *n_octave = ocb::sift3d_n_octave(x->sift3d, 1);
+		if (!x->sift3d) x->sift3d = new ocb::Sift3d;
+		const cudaError_t e =
+			ocb::sift3d_run(x->sift3d, plan, x->img3.ref, x->img3.tar, config, matching_ratio, x->sm_count, x->stream, &x->launches);
+		if (e != cudaSuccess) { // no results (include/opencorr_b200.h)
+			cudaGetLastError(); // a failed copy or event call must not surface as the next launch's error
+			delete x->sift3d;
+			x->sift3d = nullptr;
+			if (e == ocb::SIFT3D_TOO_MANY_KEYPOINTS) return set_error(x, OCB_ERR_ARG, "sift3d: too many keypoints");
+			return set_error(x, OCB_ERR_CUDA, "sift3d failed: %s", cudaGetErrorString(e));
+		}
+		if (n_matched) *n_matched = x->sift3d->ref_xyz.size() / 3;
+		if (n_octave) *n_octave = plan.n_octave;
 		return OCB_OK;
 	});
 }
@@ -2207,7 +2196,8 @@ int ocb_sift3d_get_matches(ocb_ctx* ctx, float* ref_xyz, float* tar_xyz) {
 	if (!ctx) return set_error(nullptr, OCB_ERR_ARG, "null context");
 	ocb_ctx* x = exec_member(ctx);
 	if (!x->sift3d) return relay_error(ctx, x, set_error(x, OCB_ERR_STATE, "sift3d_get_matches: ocb_sift3d has not run"));
-	ocb::sift3d_get_matches(x->sift3d, ref_xyz, tar_xyz);
+	if (ref_xyz) std::copy(x->sift3d->ref_xyz.begin(), x->sift3d->ref_xyz.end(), ref_xyz);
+	if (tar_xyz) std::copy(x->sift3d->tar_xyz.begin(), x->sift3d->tar_xyz.end(), tar_xyz);
 	return OCB_OK;
 }
 
@@ -2216,9 +2206,16 @@ int ocb_sift3d_inspect(ocb_ctx* ctx, int image, size_t* counts, int* candidates,
 	return on_exec(ctx, [&](ocb_ctx* x) -> int {
 		if (!x->sift3d) return set_error(x, OCB_ERR_STATE, "sift3d_inspect: ocb_sift3d has not run");
 		if (ensure_device(x)) return OCB_ERR_CUDA;
-		std::string err;
-		if (ocb::sift3d_inspect(x->sift3d, image, counts, candidates, max_abs, keypoints, descriptors, x->stream, &err))
-			return set_error(x, OCB_ERR_CUDA, "%s", err.c_str());
+		const ocb::Sift3dImage& im = x->sift3d->img[image];
+		const size_t n[3] = { im.n_cand, im.max_abs.size(), im.n_kp };
+		std::copy(n, n + 3, counts);
+		if (max_abs) std::copy(im.max_abs.begin(), im.max_abs.end(), max_abs);
+		const size_t cand_bytes = 5 * im.n_cand * sizeof(int), kp_bytes = im.n_kp * s3::KP_FLOATS * sizeof(float);
+		if (candidates && im.n_cand) OCB_CUDA(x, cudaMemcpyAsync(candidates, im.cand.p, cand_bytes, cudaMemcpyDeviceToHost, x->stream));
+		if (keypoints && im.n_kp) OCB_CUDA(x, cudaMemcpyAsync(keypoints, im.kp.p, kp_bytes, cudaMemcpyDeviceToHost, x->stream));
+		if (descriptors && im.n_kp)
+			OCB_CUDA(x, cudaMemcpyAsync(descriptors, im.desc.p, im.n_kp * s3::DESC * sizeof(float), cudaMemcpyDeviceToHost, x->stream));
+		OCB_CUDA(x, cudaStreamSynchronize(x->stream));
 		return OCB_OK;
 	});
 }
@@ -2227,8 +2224,7 @@ int ocb_sift3d_stage_times(ocb_ctx* ctx, float* ms) {
 	if (!ctx || !ms) return set_error(ctx, OCB_ERR_ARG, "sift3d_stage_times: bad arguments");
 	ocb_ctx* x = exec_member(ctx);
 	if (!x->sift3d) return relay_error(ctx, x, set_error(x, OCB_ERR_STATE, "sift3d_stage_times: ocb_sift3d has not run"));
-	const float* t = ocb::sift3d_stage_ms(x->sift3d);
-	std::copy(t, t + ocb::SIFT3D_STAGES, ms);
+	std::copy(x->sift3d->stage_ms, x->sift3d->stage_ms + ocb::SIFT3D_STAGES, ms);
 	return OCB_OK;
 }
 

@@ -2,11 +2,13 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
+#include <string.h>
 
-#include <string>
+#include <vector>
 
 #include "ocb_common.cuh"
 #include "ocb_tma.cuh"
+#include "sift3d_common.h"
 
 namespace ocb {
 
@@ -21,6 +23,59 @@ inline cudaError_t launch_smem(K kern, int grid, int block, size_t smem, cudaStr
 	if (e != cudaSuccess) return e;
 	kern<<<grid, block, smem, stream>>>(args...);
 	return cudaGetLastError();
+}
+
+// the kernel just enqueued: its launch error, or cudaSuccess and one more launch counted
+inline cudaError_t launched(long long* launches) {
+	const cudaError_t e = cudaGetLastError();
+	if (e == cudaSuccess) ++*launches;
+	return e;
+}
+
+// Grow-only device buffer (see grow).  Released when its owner is deleted, with the owner's device current.
+struct DevBuf {
+	void* p = nullptr;
+	size_t bytes = 0;
+	DevBuf() = default;
+	DevBuf(const DevBuf&) = delete;
+	DevBuf& operator=(const DevBuf&) = delete;
+	~DevBuf() {
+		if (p) cudaFree(p);
+	}
+	template <class T> T* as() const { return (T*)p; }
+};
+
+// Make b hold at least `bytes` on the current device; it only grows.  The stream is drained before the old allocation is freed.
+// keep_bytes = 0: the old allocation is freed first and exactly `bytes` are allocated (on failure b is left empty).  keep_bytes > 0:
+// its first keep_bytes are copied into an allocation of at least twice the capacity (on failure b is left as it was).  A failed
+// allocation or copy is cleared from the runtime's last error, which the next launch's check would otherwise report.
+inline cudaError_t grow(DevBuf& b, size_t bytes, cudaStream_t stream, size_t keep_bytes = 0) {
+	if (bytes <= b.bytes) return cudaSuccess;
+	cudaError_t e;
+	if (keep_bytes == 0 && b.p) {
+		if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+		cudaFree(b.p);
+		b.p = nullptr;
+		b.bytes = 0;
+	}
+	if (keep_bytes && bytes < 2 * b.bytes) bytes = 2 * b.bytes;
+	void* q = nullptr;
+	if ((e = cudaMalloc(&q, bytes)) != cudaSuccess) {
+		cudaGetLastError();
+		return e;
+	}
+	if (b.p) {
+		if ((e = cudaMemcpyAsync(q, b.p, keep_bytes, cudaMemcpyDeviceToDevice, stream)) != cudaSuccess
+			|| (e = cudaStreamSynchronize(stream)) != cudaSuccess) {
+			cudaGetLastError();
+			cudaFree(q);
+			return e;
+		}
+		cudaFree(b.p);
+	}
+	b.p = q;
+	b.bytes = bytes;
+	return cudaSuccess;
 }
 
 // Factorisation of one FFT axis into Stockham stages (radix 4/2/3/5, generic odd radix <= 31).
@@ -48,18 +103,103 @@ inline bool fft_plan_axis(int n, FftAxis* ax) {
 	return true;
 }
 
-// sift3d.cu (SIFT3D feature extraction and matching; state kept between ocb_sift3d and the calls that read its results)
-struct Sift3d;
+// sift3d.cu: SIFT3D feature extraction and matching
+constexpr int SIFT3D_MAX_R = 64; // largest blur radius per axis (8 at the default settings, x2 per doubling of unit anisotropy)
+constexpr int SIFT3D_MAX_L = 16; // largest n_octave_layers + 3
+struct BlurW {
+	float w[SIFT3D_MAX_R + 1];
+};
+// One Gaussian layer: its scale, and the blur that makes it from the layer below (s3::blur_kernels: sigma, radii, half kernels)
+struct Sift3dLayer {
+	float scale, sigma;
+	int radius[3];
+	BlurW w[3];
+};
+struct Sift3dOctave {
+	int nx, ny, nz;
+	float unit[3];
+};
+enum class Sift3dReject { NONE, OCTAVE_LAYERS, VOLUME_SIZE, BLUR_RADIUS };
+// The Gaussian pyramid of createGaussianPyramid (src/oc_sift.cpp:676-739): layer l of octave o is entry o * L + l.
+struct Sift3dPlan {
+	int n_octave;
+	int L;     // Gaussian layers per octave: n_octave_layers + 3
+	float kappa; // scale ratio of neighbouring layers
+	std::vector<Sift3dOctave> octave;
+	std::vector<Sift3dLayer> layer; // no blur for layer 0 of octave o > 0, which is downsampled from octave o - 1
+	Sift3dReject reject;          // why the plan is refused
+};
+
+// false, with the failed check in p->reject, when n_octave_layers is outside [1, SIFT3D_MAX_L - 3], n_octave_layers times the
+// voxel count exceeds 2^62 (the candidates' 64-bit index), or a blur radius exceeds SIFT3D_MAX_R voxels.  cfg: the
+// s3::CFG_FIELDS floats of the C ABI; unit: the voxel size.
+inline bool sift3d_plan(int nx, int ny, int nz, const float* cfg, const float* unit, Sift3dPlan* p) {
+	const int nol = (int)cfg[s3::CFG_N_OCTAVE_LAYERS], L = nol + 3;
+	p->L = L;
+	p->reject = Sift3dReject::OCTAVE_LAYERS;
+	if (nol < 1 || L > SIFT3D_MAX_L) return false;
+	p->reject = Sift3dReject::VOLUME_SIZE;
+	if ((size_t)nol * ((size_t)nx * ny * nz) > (size_t)1 << 62) return false;
+	p->reject = Sift3dReject::BLUR_RADIUS; // the check left, made layer by layer below
+	const int dim_min = nx < ny ? (nx < nz ? nx : nz) : (ny < nz ? ny : nz);
+	const int n_octave = s3::octave_count(dim_min, (int)cfg[s3::CFG_MIN_DIMENSION]);
+	const float kappa = s3::kappa_of(nol);
+	p->n_octave = n_octave;
+	p->kappa = kappa;
+	p->octave.assign(n_octave, Sift3dOctave{ nx, ny, nz, { unit[0], unit[1], unit[2] } });
+	p->layer.assign((size_t)n_octave * L, Sift3dLayer{});
+	for (int i = 0; i < n_octave * L; i++) {
+		const int o = i / L, l = i % L;
+		Sift3dLayer& b = p->layer[i];
+		if (i == 0) {
+			b.scale = 1.f / kappa * cfg[s3::CFG_SIGMA_BASE];
+			b.sigma = sqrtf(b.scale * b.scale - cfg[s3::CFG_SIGMA_SOURCE] * cfg[s3::CFG_SIGMA_SOURCE]);
+		} else if (l == 0) {
+			const Sift3dOctave& u = p->octave[o - 1];
+			p->octave[o] = Sift3dOctave{ u.nx / 2, u.ny / 2, u.nz / 2, { u.unit[0] * 2, u.unit[1] * 2, u.unit[2] * 2 } };
+			b.scale = p->layer[(o - 1) * L + nol].scale;
+			continue;
+		} else {
+			b.scale = kappa * p->layer[i - 1].scale;
+			b.sigma = sqrtf(kappa * kappa - 1.f) * p->layer[l - 1].scale;
+		}
+		float w[3 * (SIFT3D_MAX_R + 1)] = {};
+		if (!s3::blur_kernels(b.sigma, p->octave[o].unit, SIFT3D_MAX_R, b.radius, w)) return false;
+		for (int a = 0; a < 3; a++) memcpy(b.w[a].w, w + a * (SIFT3D_MAX_R + 1), sizeof(BlurW));
+	}
+	p->reject = Sift3dReject::NONE;
+	return true;
+}
+
+// One image's products of the last ocb_sift3d call, on the device
+struct Sift3dImage {
+	size_t n_cand = 0, n_kp = 0;
+	DevBuf cand; // 5 ints per candidate
+	DevBuf kp;   // s3::KP_FLOATS floats per keypoint
+	DevBuf desc; // s3::DESC floats per keypoint
+	std::vector<float> max_abs;
+};
+
 enum { SIFT3D_STAGES = 10 }; // ref: pyramid, extrema, orientation, descriptors; tar: the same four; matching; host post-pass
-Sift3d* sift3d_create();
-void sift3d_destroy(Sift3d* s);
-int sift3d_run(Sift3d* s, const float* d_ref, const float* d_tar, int nx, int ny, int nz, const float* cfg, const float* unit, float ratio,
-	int sm_count, cudaStream_t stream, long long* launches, std::string* err);
-size_t sift3d_n_matched(const Sift3d* s);
-int sift3d_n_octave(const Sift3d* s, int which);
-const float* sift3d_stage_ms(const Sift3d* s);
-void sift3d_get_matches(const Sift3d* s, float* ref_xyz, float* tar_xyz);
-int sift3d_inspect(const Sift3d* s, int which, size_t* counts, int* cand, float* max_abs, float* kp, float* desc, cudaStream_t stream, std::string* err);
+// The products of the last ocb_sift3d call and the working buffers that made them
+struct Sift3d {
+	Sift3dImage img[2];
+	std::vector<float> ref_xyz, tar_xyz; // the matched keypoints' coor_img, 3 floats each
+	float stage_ms[SIFT3D_STAGES] = {};
+	DevBuf layers, tmp, kp_tmp, top2, part, sel, keep, kept_idx, counters, cub_ws;
+	cudaEvent_t ev[2 * SIFT3D_STAGES] = {}; // start and end of each timed stage
+	~Sift3d() {
+		for (cudaEvent_t e : ev)
+			if (e) cudaEventDestroy(e);
+	}
+};
+
+// sift3d_run's result when an image has more than 2^31 - 1 keypoints, which the matching kernels cannot index
+constexpr cudaError_t SIFT3D_TOO_MANY_KEYPOINTS = static_cast<cudaError_t>(cudaErrorUnknown + 1);
+// Both images' pyramids, keypoints and descriptors as `plan` (sift3d_plan of their size) schedules them, then the matches.
+// *launches grows by each kernel once it has launched (a cub selection counts as one).
+cudaError_t sift3d_run(Sift3d* s, const Sift3dPlan& plan, const float* d_ref, const float* d_tar, const float* cfg, float ratio, int sm_count,
+	cudaStream_t stream, long long* launches);
 // icgn2d.cu
 constexpr int ICGN2D_TILE_MARGIN = 1; // slack (pixels) around subset+support in the target tile
 // TMA tile loads need the innermost coordinate 16-byte aligned (x multiple of 4 floats; seen: an

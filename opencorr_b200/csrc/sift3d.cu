@@ -12,24 +12,15 @@
 #include <algorithm>
 #include <chrono>
 #include <cstring>
-#include <string>
 #include <vector>
 
 #include "ocb_kernels.h"
-#include "sift3d_common.h"
 
 namespace ocb {
 namespace {
 
 __constant__ float c_ico_v[36] = S3_ICO_VERTICES;
 __constant__ int c_ico_f[60] = S3_ICO_FACES;
-
-constexpr int MAX_R = 64; // largest blur radius per axis (8 at the default settings, x2 per doubling of unit anisotropy)
-constexpr int MAX_L = 16; // largest n_octave_layers + 3
-
-struct BlurW {
-	float w[MAX_R + 1];
-};
 
 // One axis of gaussianBlur (:404-540): out = k0 * s[c]; out += k_r * (s[lower tap] + s[upper tap]).  Threads run along x, so
 // every pass reads and writes coalesced rows; the taps of neighbouring threads hit L1.
@@ -78,17 +69,17 @@ __global__ void max_abs_kernel(const float* __restrict__ g0, const float* __rest
 }
 
 struct OctaveView {
-	const float* g[MAX_L];
+	const float* g[SIFT3D_MAX_L];
 	int nx, ny, nz;
 	float unit[3];
-	float scale[MAX_L];
+	float scale[SIFT3D_MAX_L];
 };
 
 // detectExtrema (:795-847) as a predicate over the flattened (layer - 1, z, y, x) index of an octave: cub's order-preserving
 // selection then lists the candidates in the reference's (layer, z, y, x) order.
 struct ExtremumPred {
 	OctaveView v;
-	float thr[MAX_L];
+	float thr[SIFT3D_MAX_L];
 	__device__ bool operator()(const long long idx) const {
 		const size_t N = (size_t)v.nx * v.ny * v.nz;
 		const int n = 1 + (int)(idx / (long long)N);
@@ -468,255 +459,148 @@ __global__ void match_merge_kernel(const float4* __restrict__ part, int n1, int 
 	out[3 * i + 2] = t.d1;
 }
 
-} // namespace
-
 // ---- host side -----------------------------------------------------------------------------------------------------------
 
-// Device array that keeps its contents when it grows (the per-image lists grow octave by octave).
-template <class T> struct DevVec {
-	T* p = nullptr;
-	size_t cap = 0;
-	~DevVec() {
-		if (p) cudaFree(p);
-	}
-	cudaError_t reserve(size_t n, size_t keep, cudaStream_t s) {
-		if (n <= cap) return cudaSuccess;
-		size_t c = std::max(n, cap * 2);
-		T* q = nullptr;
-		cudaError_t e = cudaMalloc(&q, c * sizeof(T));
-		if (e != cudaSuccess) return e;
-		if (p && keep) cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, s);
-		if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return e;
-		if (p) cudaFree(p);
-		p = q;
-		cap = c;
-		return cudaSuccess;
-	}
-};
-
-struct Sift3dImage {
-	int n_octave = 0;
-	size_t n_cand = 0, n_kp = 0;
-	DevVec<int> cand;   // 5 ints per candidate
-	DevVec<float> kp;   // s3::KP_FLOATS per keypoint
-	DevVec<float> desc; // 768 per keypoint
-	std::vector<float> max_abs;
-};
-
-struct Sift3d {
-	Sift3dImage img[2];
-	std::vector<float> ref_xyz, tar_xyz;
-	float stage_ms[SIFT3D_STAGES] = {};
-	DevVec<float> layers, tmp, kp_tmp, top2;
-	DevVec<float4> part;
-	DevVec<long long> sel;
-	DevVec<int> keep, kept_idx, max_bits, counters;
-	DevVec<unsigned char> cub_ws;
-	std::vector<cudaEvent_t> ev;
-	~Sift3d() {
-		for (cudaEvent_t e : ev) cudaEventDestroy(e);
-	}
-};
-
-Sift3d* sift3d_create() { return new Sift3d; }
-void sift3d_destroy(Sift3d* s) { delete s; }
-
-namespace {
-
-#define S3_CK(call)                                                   \
-	do {                                                              \
-		cudaError_t e_ = (call);                                      \
-		if (e_ != cudaSuccess) {                                      \
-			*err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-			return -1;                                                \
-		}                                                             \
-	} while (0)
-
-inline int float_bits(float f) {
-	int i;
-	memcpy(&i, &f, sizeof(int));
-	return i;
-}
-
-// Times a stretch of stream work into one stage slot; elapsed times are read after the next synchronisation.
+// Times stretches of stream work into stage slots.  A stage runs at most once between two collections, so it has one pair of
+// events (Sift3d::ev); elapsed times are read after the next synchronisation.
 struct StageTimer {
 	Sift3d* s;
 	cudaStream_t st;
-	std::vector<std::pair<int, int>> open; // (stage, event index)
-	int next = 0;
-	cudaEvent_t get() {
-		if (next == (int)s->ev.size()) {
-			cudaEvent_t e;
-			cudaEventCreate(&e);
-			s->ev.push_back(e);
-		}
-		return s->ev[next++];
+	unsigned pending = 0;
+	cudaError_t begin(int k) { return cudaEventRecord(s->ev[2 * k], st); }
+	cudaError_t end(int k) {
+		pending |= 1u << k;
+		return cudaEventRecord(s->ev[2 * k + 1], st);
 	}
-	void begin(int stage) {
-		open.push_back({ stage, next });
-		cudaEventRecord(get(), st);
-		get(); // recorded by end()
-	}
-	void end() { cudaEventRecord(s->ev[open.back().second + 1], st); }
 	void collect() { // after a synchronisation
-		for (auto& o : open) {
+		for (int k = 0; k < SIFT3D_STAGES; k++) {
 			float ms = 0.f;
-			if (cudaEventElapsedTime(&ms, s->ev[o.second], s->ev[o.second + 1]) == cudaSuccess) s->stage_ms[o.first] += ms;
+			if ((pending >> k & 1) && cudaEventElapsedTime(&ms, s->ev[2 * k], s->ev[2 * k + 1]) == cudaSuccess) s->stage_ms[k] += ms;
 		}
-		open.clear();
-		next = 0;
+		pending = 0;
+	}
+	// end stage k, copy `bytes` back from the device, wait for them and collect
+	cudaError_t finish(int k, void* dst, const void* src, size_t bytes) {
+		cudaError_t e = end(k);
+		if (e == cudaSuccess && (e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st)) == cudaSuccess) e = cudaStreamSynchronize(st);
+		if (e == cudaSuccess) collect();
+		return e;
 	}
 };
 
-int extract(Sift3d* s, int which, const float* d_img, int nx0, int ny0, int nz0, const float* cfg, const float* unit0, int sm_count, cudaStream_t st,
-	long long* launches, std::string* err) {
+// The three passes of one blur (x, y into the scratch volume, z) of an oc.nx x oc.ny x oc.nz layer
+cudaError_t blur(const float* src, float* dst, float* tmp, const Sift3dOctave& oc, const Sift3dLayer& b, cudaStream_t st, long long* launches) {
+	const dim3 blk(32, 8), grd((oc.nx + 31) / 32, (oc.ny + 7) / 8, std::min(oc.nz, 64));
+	cudaError_t e;
+	blur_axis_kernel<0><<<grd, blk, 0, st>>>(src, dst, oc.nx, oc.ny, oc.nz, b.radius[0], b.w[0]);
+	if ((e = launched(launches)) != cudaSuccess) return e;
+	blur_axis_kernel<1><<<grd, blk, 0, st>>>(dst, tmp, oc.nx, oc.ny, oc.nz, b.radius[1], b.w[1]);
+	if ((e = launched(launches)) != cudaSuccess) return e;
+	blur_axis_kernel<2><<<grd, blk, 0, st>>>(tmp, dst, oc.nx, oc.ny, oc.nz, b.radius[2], b.w[2]);
+	return launched(launches);
+}
+
+// One image's candidates, max|DoG|, keypoints and descriptors into s->img[which], octave by octave.  counters: the max|DoG| bits
+// of the octave's DoG layers, then the candidate and the kept count.
+cudaError_t extract(Sift3d* s, const Sift3dPlan& plan, int which, const float* d_img, const float* cfg, int sm_count, cudaStream_t st,
+	StageTimer& tm, long long* launches) {
 	Sift3dImage& out = s->img[which];
-	const int nol = (int)cfg[s3::CFG_N_OCTAVE_LAYERS], L = nol + 3;
-	if (nol < 1 || L > MAX_L) {
-		*err = "sift3d: n_octave_layers must be in [1, " + std::to_string(MAX_L - 3) + "]";
-		return -2;
-	}
-	int dim_min = std::min(nx0, std::min(ny0, nz0));
-	const int n_octave = s3::octave_count(dim_min, (int)cfg[s3::CFG_MIN_DIMENSION]);
-	out.n_octave = n_octave;
+	const int L = plan.L, nol = L - 3;
 	out.n_cand = out.n_kp = 0;
 	out.max_abs.clear();
-	const float kappa = s3::kappa_of(nol);
-	std::vector<float> scale((size_t)n_octave * L), sigma((size_t)n_octave * L, 0.f);
-	scale[0] = 1.f / kappa * cfg[s3::CFG_SIGMA_BASE];
-	sigma[0] = sqrtf(scale[0] * scale[0] - cfg[s3::CFG_SIGMA_SOURCE] * cfg[s3::CFG_SIGMA_SOURCE]);
-	for (int i = 1; i < n_octave * L; i++) {
-		const int o = i / L, lio = i % L;
-		if (lio == 0) {
-			scale[i] = scale[(o - 1) * L + nol];
-		} else {
-			scale[i] = kappa * scale[i - 1];
-			sigma[i] = sqrtf(kappa * kappa - 1.f) * scale[lio - 1];
-		}
-	}
-	const size_t N0 = (size_t)nx0 * ny0 * nz0;
-	if ((size_t)nol * N0 > (size_t)1 << 62) {
-		*err = "sift3d: volume too large";
-		return -2;
-	}
-	S3_CK(s->layers.reserve(N0 * L, 0, st));
-	S3_CK(s->tmp.reserve(N0, 0, st));
-	S3_CK(s->sel.reserve(N0 * nol, 0, st));
-	S3_CK(s->max_bits.reserve(MAX_L, 0, st));
-	S3_CK(s->counters.reserve(2, 0, st));
-	float unit[3] = { unit0[0], unit0[1], unit0[2] };
-	int nx = nx0, ny = ny0, nz = nz0;
-	StageTimer tm{ s, st };
-	auto layer = [&](int l) { return s->layers.p + (size_t)l * N0; };
-	auto blur = [&](const float* src, float* dst, float sg) -> int {
-		int rad[3];
-		std::vector<float> w(3 * (MAX_R + 1));
-		if (!s3::blur_kernels(sg, unit, MAX_R, rad, w.data())) {
-			*err = "sift3d: blur radius exceeds " + std::to_string(MAX_R) + " voxels (physical units too anisotropic)";
-			return -2;
-		}
-		BlurW wx, wy, wz;
-		std::copy(w.begin(), w.begin() + MAX_R + 1, wx.w);
-		std::copy(w.begin() + MAX_R + 1, w.begin() + 2 * (MAX_R + 1), wy.w);
-		std::copy(w.begin() + 2 * (MAX_R + 1), w.end(), wz.w);
-		const dim3 blk(32, 8), grd((nx + 31) / 32, (ny + 7) / 8, std::min(nz, 64));
-		blur_axis_kernel<0><<<grd, blk, 0, st>>>(src, dst, nx, ny, nz, rad[0], wx);
-		blur_axis_kernel<1><<<grd, blk, 0, st>>>(dst, s->tmp.p, nx, ny, nz, rad[1], wy);
-		blur_axis_kernel<2><<<grd, blk, 0, st>>>(s->tmp.p, dst, nx, ny, nz, rad[2], wz);
-		*launches += 3;
-		return 0;
-	};
+	const size_t N0 = (size_t)plan.octave[0].nx * plan.octave[0].ny * plan.octave[0].nz;
+	cudaError_t e;
+	if ((e = grow(s->layers, N0 * L * sizeof(float), st)) != cudaSuccess || (e = grow(s->tmp, N0 * sizeof(float), st)) != cudaSuccess
+		|| (e = grow(s->sel, N0 * nol * sizeof(long long), st)) != cudaSuccess
+		|| (e = grow(s->counters, (SIFT3D_MAX_L + 2) * sizeof(int), st)) != cudaSuccess)
+		return e;
+	float* const tmp = s->tmp.as<float>();
+	long long* const sel = s->sel.as<long long>();
+	int* const counters = s->counters.as<int>();
+	int* const n_found = counters + SIFT3D_MAX_L; // candidates, kept
+	auto layer = [&](int l) { return s->layers.as<float>() + (size_t)l * N0; };
 	const int grid1d = sm_count * 8;
-	for (int o = 0; o < n_octave; o++) {
+	for (int o = 0; o < plan.n_octave; o++) {
+		const Sift3dOctave& oc = plan.octave[o];
+		const Sift3dLayer* lay = &plan.layer[(size_t)o * L];
+		const size_t N = (size_t)oc.nx * oc.ny * oc.nz;
 		// ---- Gaussian layers
-		tm.begin(4 * which + 0);
+		if ((e = tm.begin(4 * which + 0)) != cudaSuccess) return e;
 		if (o == 0) {
-			if (int rc = blur(d_img, layer(0), sigma[0])) return rc;
+			if ((e = blur(d_img, layer(0), tmp, oc, lay[0], st, launches)) != cudaSuccess) return e;
 		} else {
-			const int sx = nx, sy = ny;
-			nx /= 2, ny /= 2, nz /= 2;
-			for (int a = 0; a < 3; a++) unit[a] *= 2;
-			downsample_kernel<<<grid1d, 256, 0, st>>>(layer(nol), s->tmp.p, sx, sy, nx, ny, nz);
-			S3_CK(cudaMemcpyAsync(layer(0), s->tmp.p, (size_t)nx * ny * nz * sizeof(float), cudaMemcpyDeviceToDevice, st));
-			*launches += 1;
+			downsample_kernel<<<grid1d, 256, 0, st>>>(layer(nol), tmp, plan.octave[o - 1].nx, plan.octave[o - 1].ny, oc.nx, oc.ny, oc.nz);
+			if ((e = launched(launches)) != cudaSuccess) return e;
+			if ((e = cudaMemcpyAsync(layer(0), tmp, N * sizeof(float), cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return e;
 		}
 		for (int l = 1; l < L; l++)
-			if (int rc = blur(layer(l - 1), layer(l), sigma[o * L + l])) return rc;
-		const size_t N = (size_t)nx * ny * nz;
-		std::vector<int> init(L - 1, float_bits(-1.f));
-		S3_CK(cudaMemcpyAsync(s->max_bits.p, init.data(), (L - 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-		for (int n = 0; n < L - 1; n++) max_abs_kernel<<<grid1d, 256, 0, st>>>(layer(n), layer(n + 1), N, s->max_bits.p + n);
-		*launches += L - 1;
-		tm.end();
-		std::vector<int> bits(L - 1);
-		S3_CK(cudaMemcpyAsync(bits.data(), s->max_bits.p, (L - 1) * sizeof(int), cudaMemcpyDeviceToHost, st));
-		S3_CK(cudaStreamSynchronize(st));
-		OctaveView v;
+			if ((e = blur(layer(l - 1), layer(l), tmp, oc, lay[l], st, launches)) != cudaSuccess) return e;
+		std::vector<float> init(L - 1, -1.f), ma(L - 1); // the maxima travel as the int bits of the floats
+		if ((e = cudaMemcpyAsync(counters, init.data(), (L - 1) * sizeof(int), cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
+		for (int n = 0; n < L - 1; n++) {
+			max_abs_kernel<<<grid1d, 256, 0, st>>>(layer(n), layer(n + 1), N, counters + n);
+			if ((e = launched(launches)) != cudaSuccess) return e;
+		}
+		if ((e = tm.finish(4 * which + 0, ma.data(), counters, (L - 1) * sizeof(int))) != cudaSuccess) return e;
+		ExtremumPred pred;
+		OctaveView& v = pred.v;
 		for (int l = 0; l < L; l++) {
 			v.g[l] = layer(l);
-			v.scale[l] = scale[o * L + l];
+			v.scale[l] = lay[l].scale;
 		}
-		v.nx = nx, v.ny = ny, v.nz = nz;
-		for (int a = 0; a < 3; a++) v.unit[a] = unit[a];
-		ExtremumPred pred;
-		pred.v = v;
-		for (int n = 0; n < L - 1; n++) {
-			float ma;
-			memcpy(&ma, &bits[n], sizeof(float));
-			out.max_abs.push_back(ma);
-			pred.thr[n] = cfg[s3::CFG_ALPHA] * ma;
-		}
+		v.nx = oc.nx, v.ny = oc.ny, v.nz = oc.nz;
+		for (int a = 0; a < 3; a++) v.unit[a] = oc.unit[a];
+		for (int n = 0; n < L - 1; n++) pred.thr[n] = cfg[s3::CFG_ALPHA] * ma[n];
+		out.max_abs.insert(out.max_abs.end(), ma.begin(), ma.end());
 		// ---- extrema: order-preserving selection over (layer, z, y, x)
-		tm.begin(4 * which + 1);
 		const long long items = (long long)nol * (long long)N;
 		thrust::counting_iterator<long long> it(0);
 		size_t ws = 0;
-		S3_CK(cub::DeviceSelect::If(nullptr, ws, it, s->sel.p, s->counters.p, items, pred, st));
-		S3_CK(s->cub_ws.reserve(ws, 0, st));
-		S3_CK(cub::DeviceSelect::If(s->cub_ws.p, ws, it, s->sel.p, s->counters.p, items, pred, st));
-		*launches += 1;
-		tm.end();
+		if ((e = tm.begin(4 * which + 1)) != cudaSuccess) return e;
+		if ((e = cub::DeviceSelect::If(nullptr, ws, it, sel, n_found, items, pred, st)) != cudaSuccess || (e = grow(s->cub_ws, ws, st)) != cudaSuccess
+			|| (e = cub::DeviceSelect::If(s->cub_ws.p, ws, it, sel, n_found, items, pred, st)) != cudaSuccess)
+			return e;
+		++*launches;
 		int n_cand = 0;
-		S3_CK(cudaMemcpyAsync(&n_cand, s->counters.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-		S3_CK(cudaStreamSynchronize(st));
-		tm.collect();
+		if ((e = tm.finish(4 * which + 1, &n_cand, n_found, sizeof(int))) != cudaSuccess) return e;
 		if (n_cand == 0) continue;
 		// ---- orientation
-		S3_CK(out.cand.reserve(5 * (out.n_cand + n_cand), 5 * out.n_cand, st));
-		S3_CK(s->kp_tmp.reserve((size_t)s3::KP_FLOATS * n_cand, 0, st));
-		S3_CK(s->keep.reserve(n_cand, 0, st));
-		S3_CK(s->kept_idx.reserve(n_cand, 0, st));
-		tm.begin(4 * which + 2);
+		if ((e = grow(out.cand, 5 * (out.n_cand + n_cand) * sizeof(int), st, 5 * out.n_cand * sizeof(int))) != cudaSuccess
+			|| (e = grow(s->kp_tmp, (size_t)s3::KP_FLOATS * n_cand * sizeof(float), st)) != cudaSuccess
+			|| (e = grow(s->keep, n_cand * sizeof(int), st)) != cudaSuccess || (e = grow(s->kept_idx, n_cand * sizeof(int), st)) != cudaSuccess)
+			return e;
+		if ((e = tm.begin(4 * which + 2)) != cudaSuccess) return e;
 		OrientParams prm{ cfg[s3::CFG_BETA], cfg[s3::CFG_GAMMA], cfg[s3::CFG_GRADIENT_THRESHOLD], o };
-		orientation_kernel<<<(n_cand + 127) / 128, 128, 0, st>>>(v, prm, s->sel.p, n_cand, out.cand.p + 5 * out.n_cand, s->kp_tmp.p, s->keep.p);
-		ws = 0;
-		S3_CK(cub::DeviceSelect::Flagged(nullptr, ws, thrust::counting_iterator<int>(0), s->keep.p, s->kept_idx.p, s->counters.p + 1, n_cand, st));
-		S3_CK(s->cub_ws.reserve(ws, 0, st));
-		S3_CK(cub::DeviceSelect::Flagged(s->cub_ws.p, ws, thrust::counting_iterator<int>(0), s->keep.p, s->kept_idx.p, s->counters.p + 1, n_cand, st));
-		*launches += 2;
-		tm.end();
+		float* const kp_tmp = s->kp_tmp.as<float>();
+		int *const keep = s->keep.as<int>(), *const kept_idx = s->kept_idx.as<int>();
+		orientation_kernel<<<(n_cand + 127) / 128, 128, 0, st>>>(v, prm, sel, n_cand, out.cand.as<int>() + 5 * out.n_cand, kp_tmp, keep);
+		if ((e = launched(launches)) != cudaSuccess) return e;
+		const thrust::counting_iterator<int> idx(0);
+		if ((e = cub::DeviceSelect::Flagged(nullptr, ws, idx, keep, kept_idx, n_found + 1, n_cand, st)) != cudaSuccess
+			|| (e = grow(s->cub_ws, ws, st)) != cudaSuccess
+			|| (e = cub::DeviceSelect::Flagged(s->cub_ws.p, ws, idx, keep, kept_idx, n_found + 1, n_cand, st)) != cudaSuccess)
+			return e;
+		++*launches;
 		out.n_cand += n_cand;
 		int n_kept = 0;
-		S3_CK(cudaMemcpyAsync(&n_kept, s->counters.p + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-		S3_CK(cudaStreamSynchronize(st));
-		tm.collect();
+		if ((e = tm.finish(4 * which + 2, &n_kept, n_found + 1, sizeof(int))) != cudaSuccess) return e;
 		if (n_kept == 0) continue;
 		// ---- descriptors
-		S3_CK(out.kp.reserve((size_t)s3::KP_FLOATS * (out.n_kp + n_kept), (size_t)s3::KP_FLOATS * out.n_kp, st));
-		S3_CK(out.desc.reserve((size_t)s3::DESC * (out.n_kp + n_kept), (size_t)s3::DESC * out.n_kp, st));
-		float* kp_o = out.kp.p + (size_t)s3::KP_FLOATS * out.n_kp;
-		tm.begin(4 * which + 3);
-		gather_kp_kernel<<<std::max(1, std::min(grid1d, (n_kept * s3::KP_FLOATS + 255) / 256)), 256, 0, st>>>(s->kp_tmp.p, s->kept_idx.p,
-			s->counters.p + 1, kp_o);
-		descriptor_kernel<<<n_kept, DESC_THREADS, 0, st>>>(v, kp_o, cfg[s3::CFG_TRUNCATE_THRESHOLD], out.desc.p + (size_t)s3::DESC * out.n_kp);
-		*launches += 2;
-		tm.end();
+		const size_t kp_bytes = (size_t)s3::KP_FLOATS * sizeof(float), desc_bytes = (size_t)s3::DESC * sizeof(float);
+		if ((e = grow(out.kp, kp_bytes * (out.n_kp + n_kept), st, kp_bytes * out.n_kp)) != cudaSuccess
+			|| (e = grow(out.desc, desc_bytes * (out.n_kp + n_kept), st, desc_bytes * out.n_kp)) != cudaSuccess)
+			return e;
+		if ((e = tm.begin(4 * which + 3)) != cudaSuccess) return e;
+		float* kp_o = out.kp.as<float>() + (size_t)s3::KP_FLOATS * out.n_kp;
+		gather_kp_kernel<<<std::max(1, std::min(grid1d, (n_kept * s3::KP_FLOATS + 255) / 256)), 256, 0, st>>>(kp_tmp, kept_idx, n_found + 1, kp_o);
+		if ((e = launched(launches)) != cudaSuccess) return e;
+		float* desc_o = out.desc.as<float>() + (size_t)s3::DESC * out.n_kp;
+		descriptor_kernel<<<n_kept, DESC_THREADS, 0, st>>>(v, kp_o, cfg[s3::CFG_TRUNCATE_THRESHOLD], desc_o);
+		if ((e = launched(launches)) != cudaSuccess || (e = tm.end(4 * which + 3)) != cudaSuccess) return e;
 		out.n_kp += n_kept;
 	}
-	S3_CK(cudaGetLastError());
-	S3_CK(cudaStreamSynchronize(st));
-	tm.collect();
-	return 0;
+	if ((e = cudaStreamSynchronize(st)) == cudaSuccess) tm.collect();
+	return e;
 }
 
 // monodirectionalMatch (:1251-1418) after the brute-force scan: ratio test, many-to-one resolution and output, on the host.
@@ -771,42 +655,43 @@ void match_post(const std::vector<float>& top2, size_t n1, float ratio, std::vec
 
 } // namespace
 
-int sift3d_run(Sift3d* s, const float* d_ref, const float* d_tar, int nx, int ny, int nz, const float* cfg, const float* unit, float ratio,
-	int sm_count, cudaStream_t st, long long* launches, std::string* err) {
+cudaError_t sift3d_run(Sift3d* s, const Sift3dPlan& plan, const float* d_ref, const float* d_tar, const float* cfg, float ratio, int sm_count,
+	cudaStream_t st, long long* launches) {
 	for (float& t : s->stage_ms) t = 0.f;
+	cudaError_t e;
+	for (cudaEvent_t& ev : s->ev)
+		if (!ev && (e = cudaEventCreate(&ev)) != cudaSuccess) return e;
+	StageTimer tm{ s, st };
 	const float* imgs[2] = { d_ref, d_tar };
 	for (int w = 0; w < 2; w++)
-		if (int rc = extract(s, w, imgs[w], nx, ny, nz, cfg, unit, sm_count, st, launches, err)) return rc;
+		if ((e = extract(s, plan, w, imgs[w], cfg, sm_count, st, tm, launches)) != cudaSuccess) return e;
 	s->ref_xyz.clear();
 	s->tar_xyz.clear();
 	const size_t n1 = s->img[0].n_kp, n2 = s->img[1].n_kp;
-	if (n1 == 0) return 0;
-	if (n1 > 0x7fffffff || n2 > 0x7fffffff) {
-		*err = "sift3d: too many keypoints";
-		return -2;
-	}
-	StageTimer tm{ s, st };
-	tm.begin(8);
+	if (n1 == 0) return cudaSuccess;
+	if (n1 > 0x7fffffff || n2 > 0x7fffffff) return SIFT3D_TOO_MANY_KEYPOINTS;
 	const int row_blocks = (int)((n1 + MT - 1) / MT), col_tiles = (int)((n2 + MT - 1) / MT);
 	// split the target rows into segments so that the grid covers the GPU even when the reference set is small
 	int segs = std::max(1, std::min(col_tiles, (2 * sm_count + row_blocks - 1) / row_blocks));
 	const int tiles_per_seg = std::max(1, (col_tiles + segs - 1) / segs);
 	segs = std::max(1, (col_tiles + tiles_per_seg - 1) / tiles_per_seg);
-	S3_CK(s->part.reserve((size_t)segs * n1, 0, st));
-	S3_CK(s->top2.reserve(3 * n1, 0, st));
+	if ((e = tm.begin(8)) != cudaSuccess) return e;
+	if ((e = grow(s->part, (size_t)segs * n1 * sizeof(float4), st)) != cudaSuccess || (e = grow(s->top2, 3 * n1 * sizeof(float), st)) != cudaSuccess)
+		return e;
 	if (n2 > 0) {
-		match_kernel<<<dim3(row_blocks, segs), 256, 0, st>>>(s->img[0].desc.p, (int)n1, s->img[1].desc.p, (int)n2, tiles_per_seg, s->part.p);
-		*launches += 1;
+		match_kernel<<<dim3(row_blocks, segs), 256, 0, st>>>(s->img[0].desc.as<float>(), (int)n1, s->img[1].desc.as<float>(), (int)n2, tiles_per_seg,
+			s->part.as<float4>());
+		if ((e = launched(launches)) != cudaSuccess) return e;
 	}
-	match_merge_kernel<<<(int)((n1 + 255) / 256), 256, 0, st>>>(s->part.p, (int)n1, n2 > 0 ? segs : 0, s->top2.p);
-	*launches += 1;
+	match_merge_kernel<<<(int)((n1 + 255) / 256), 256, 0, st>>>(s->part.as<float4>(), (int)n1, n2 > 0 ? segs : 0, s->top2.as<float>());
+	if ((e = launched(launches)) != cudaSuccess) return e;
 	std::vector<float> top2(3 * n1), kp1((size_t)s3::KP_FLOATS * n1), kp2((size_t)s3::KP_FLOATS * n2);
-	S3_CK(cudaMemcpyAsync(top2.data(), s->top2.p, top2.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
-	tm.end();
-	S3_CK(cudaMemcpyAsync(kp1.data(), s->img[0].kp.p, kp1.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
-	if (n2) S3_CK(cudaMemcpyAsync(kp2.data(), s->img[1].kp.p, kp2.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
-	S3_CK(cudaGetLastError());
-	S3_CK(cudaStreamSynchronize(st));
+	if ((e = cudaMemcpyAsync(top2.data(), s->top2.p, top2.size() * sizeof(float), cudaMemcpyDeviceToHost, st)) != cudaSuccess
+		|| (e = tm.end(8)) != cudaSuccess
+		|| (e = cudaMemcpyAsync(kp1.data(), s->img[0].kp.p, kp1.size() * sizeof(float), cudaMemcpyDeviceToHost, st)) != cudaSuccess
+		|| (n2 && (e = cudaMemcpyAsync(kp2.data(), s->img[1].kp.p, kp2.size() * sizeof(float), cudaMemcpyDeviceToHost, st)) != cudaSuccess)
+		|| (e = cudaStreamSynchronize(st)) != cudaSuccess)
+		return e;
 	tm.collect();
 	const auto t0 = std::chrono::steady_clock::now();
 	std::vector<std::pair<int, int>> pairs;
@@ -818,29 +703,7 @@ int sift3d_run(Sift3d* s, const float* d_ref, const float* d_tar, int nx, int ny
 		}
 	}
 	s->stage_ms[9] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-	return 0;
-}
-
-size_t sift3d_n_matched(const Sift3d* s) { return s->ref_xyz.size() / 3; }
-int sift3d_n_octave(const Sift3d* s, int which) { return s->img[which].n_octave; }
-const float* sift3d_stage_ms(const Sift3d* s) { return s->stage_ms; }
-
-void sift3d_get_matches(const Sift3d* s, float* ref_xyz, float* tar_xyz) {
-	if (ref_xyz) std::copy(s->ref_xyz.begin(), s->ref_xyz.end(), ref_xyz);
-	if (tar_xyz) std::copy(s->tar_xyz.begin(), s->tar_xyz.end(), tar_xyz);
-}
-
-int sift3d_inspect(const Sift3d* s, int which, size_t* counts, int* cand, float* max_abs, float* kp, float* desc, cudaStream_t st, std::string* err) {
-	const Sift3dImage& im = s->img[which];
-	counts[0] = im.n_cand;
-	counts[1] = im.max_abs.size();
-	counts[2] = im.n_kp;
-	if (max_abs) std::copy(im.max_abs.begin(), im.max_abs.end(), max_abs);
-	if (cand && im.n_cand) S3_CK(cudaMemcpyAsync(cand, im.cand.p, 5 * im.n_cand * sizeof(int), cudaMemcpyDeviceToHost, st));
-	if (kp && im.n_kp) S3_CK(cudaMemcpyAsync(kp, im.kp.p, (size_t)s3::KP_FLOATS * im.n_kp * sizeof(float), cudaMemcpyDeviceToHost, st));
-	if (desc && im.n_kp) S3_CK(cudaMemcpyAsync(desc, im.desc.p, (size_t)s3::DESC * im.n_kp * sizeof(float), cudaMemcpyDeviceToHost, st));
-	S3_CK(cudaStreamSynchronize(st));
-	return 0;
+	return cudaSuccess;
 }
 
 } // namespace ocb

@@ -573,13 +573,6 @@ struct StrainWs {
 	}
 };
 
-// the kernel just enqueued: its launch error, or cudaSuccess and one more launch counted
-cudaError_t launched(long long* launches) {
-	const cudaError_t e = cudaGetLastError();
-	if (e == cudaSuccess) ++*launches;
-	return e;
-}
-
 // bbox and finite count (the call's one readback), keys, sort, gather, strain.  moved null: the pair call over n records
 // (`only`: Strain::compute(POI*, queue)); else the series over n_frames frames of n records, which sets *moved instead of
 // writing anything when the positions of some frame are not frame 0's.

@@ -5,39 +5,13 @@ import numpy as np
 import pytest
 
 import opencorr_b200 as ob
-from opencorr_b200 import _capi, synth
+from opencorr_b200 import _capi
 from oracle import sift3d as s3
+from sift3d_cases import CASES, cfg as _cfg, crop as _crop, volumes
 
 pytestmark = pytest.mark.gpu
 
 MARGIN = 1e-5
-
-
-def _crop():
-    z = np.load("tests/golden/al_foam4_crop.npz")
-    return z["ref"].astype(np.float32), z["tar"].astype(np.float32)
-
-
-def _synth(dx, dy, dz):
-    ref, tar = synth.speckle_pair_3d(dx, dy, dz)  # target displaced by synth.displacement_3d
-    return ref.astype(np.float32), tar.astype(np.float32)
-
-
-def _cfg(**kw):
-    cfg = ob.SIFT3D_DEFAULT_CONFIG.copy()
-    for k, v in kw.items():
-        cfg[ob.api.SIFT3D_CONFIG_FIELDS.index(k)] = v
-    return cfg
-
-
-CASES = {
-    "al_foam4_crop": (_crop, (1.0, 1.0, 1.0), {}),
-    "synthetic_120": (lambda: _synth(120, 120, 120), (1.0, 1.0, 1.0), {}),
-    "odd_101x77x130": (lambda: _synth(101, 77, 130), (1.0, 1.0, 1.0), {}),
-    "anisotropic_112x104x60": (lambda: _synth(112, 104, 60), (1.0, 1.0, 2.0), {}),
-    "two_octave_layers": (lambda: _synth(96, 90, 84), (1.0, 1.0, 1.0), {"n_octave_layers": 2}),
-    "mirror_clamp_128": (lambda: _synth(128, 128, 128), (1.0, 1.0, 1.0), {}),  # top octave 8^3: blur radius 8 >= side
-}
 
 
 def _same_bits(a, b):
@@ -63,8 +37,8 @@ def _check_image(gpu, ora, label):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_sift3d_matches_oracle(engine, name):
-    make, unit, kw = CASES[name]
-    ref, tar = make()
+    _, unit, kw = CASES[name]
+    ref, tar = volumes(name)
     cfg = _cfg(**kw)
     engine.set_images_3d(ref, tar)
     a, b, n_octave = engine.sift3d(cfg, unit)
@@ -137,6 +111,59 @@ def test_sift3d_rejects_bad_arguments(engine):
         engine.sift3d(unit=(1.0, 0.0, 1.0))
     with pytest.raises(_capi.OpenCorrB200Error):
         engine.sift3d(_cfg(n_octave_layers=0))
+
+
+def _expected_launches(fr, ft, n_octave_layers):
+    """Launches of one call, from the oracle's products: per octave of each image the blurs (three passes each; octave > 0
+    downsamples its bottom layer), the max|DoG| kernels and the extrema selection, then orientation and its selection where the
+    octave has candidates, gather and descriptors where it keeps keypoints; matching where the reference image has keypoints."""
+    L = n_octave_layers + 3
+    n = 0
+    for f in (fr, ft):
+        for o in range(f.n_octave):
+            n += (3 * L if o == 0 else 1 + 3 * (L - 1)) + (L - 1) + 1
+            n += 2 * bool((f.cand[:, 0] == o).any()) + 2 * bool((f.kp[:, 6] == o).any())
+    return n + (1 + bool(len(ft.kp)) if len(fr.kp) else 0)
+
+
+def test_sift3d_launch_count(engine):
+    """Two identical calls each add the same number of launches, the number the oracle's products imply."""
+    ref, tar = _crop()
+    engine.set_images_3d(ref, tar)
+    added = []
+    for _ in range(2):
+        before = engine.launch_count()
+        engine.sift3d()
+        added.append(engine.launch_count() - before)
+    expected = _expected_launches(s3.Features(ref), s3.Features(tar), 3)
+    print("launches per call:", added, "expected", expected)
+    assert added == [expected, expected]
+
+
+def _matches(engine, n):
+    a, b = np.empty((n, 3), np.float32), np.empty((n, 3), np.float32)
+    engine._ck(engine._lib.ocb_sift3d_get_matches(engine._ctx, a.ctypes.data, b.ctypes.data))
+    return a, b
+
+
+def test_sift3d_refusal_keeps_results(engine):
+    """A call refused before any device work (a blur radius above 64 voxels, n_octave_layers = 14) leaves the previous call's
+    matches, image products and stage times readable, bit for bit."""
+    ref, tar = _crop()
+    engine.set_images_3d(ref, tar)
+    a, b, _ = engine.sift3d()
+    products = [engine.sift3d_inspect(i) for i in (0, 1)]
+    times = engine.sift3d_stage_times()
+    for kw in ({"unit": (1.0, 1.0, 8.5)}, {"config": _cfg(n_octave_layers=14)}):
+        with pytest.raises(_capi.OpenCorrB200Error) as err:
+            engine.sift3d(**kw)
+        assert err.value.code == _capi.OCB_ERR_ARG, (kw, str(err.value))
+        ga, gb = _matches(engine, len(a))
+        assert _same_bits(ga, a) and _same_bits(gb, b), kw
+        for i in (0, 1):
+            now = engine.sift3d_inspect(i)
+            assert all(_same_bits(now[k], products[i][k]) for k in products[i]), (kw, i)
+        assert engine.sift3d_stage_times() == times, kw
 
 
 def test_sift3d_shim_program(engine, tmp_path):
