@@ -1154,6 +1154,79 @@ namespace opencorr
 		}
 	};
 
+	// RegionFit2D / RegionFit3D (reference src/oc_region_fit.h:25-85, src/oc_region_fit.cpp): a POI's new initial guess from the
+	// plane fit of its reliable neighbours' displacements (include/opencorr_b200.h ocb_region_fit2d).  setNeighbor keeps a pointer
+	// to the reliable queue, read when compute() runs; prepare() builds kd-trees in the reference and is empty here.
+	class RegionFit2D : public DIC
+	{
+	protected:
+		std::vector<POI2D>* neighbor_reliable = nullptr;
+		float neighbor_search_radius;
+		int neighbor_number_min;
+
+	public:
+		RegionFit2D(float neighbor_search_radius, int neighbor_number_min, int thread_number)
+		{
+			this->neighbor_search_radius = neighbor_search_radius;
+			this->neighbor_number_min = neighbor_number_min;
+			this->thread_number = thread_number;
+		}
+		~RegionFit2D() {}
+		float getSearchRadius() const { return neighbor_search_radius; }
+		int getNeighborMin() const { return neighbor_number_min; }
+		void setSearchRadius(float neighbor_search_radius) { this->neighbor_search_radius = neighbor_search_radius; }
+		void setNeighborMin(int neighbor_number_min) { this->neighbor_number_min = neighbor_number_min; }
+		void setNeighbor(std::vector<POI2D>& reliable_pois) { neighbor_reliable = &reliable_pois; }
+
+		void prepare() {}
+		void compute(POI2D* poi) { run(poi, 1); }
+		void compute(std::vector<POI2D>& poi_queue) { run(poi_queue.data(), poi_queue.size()); }
+
+	private:
+		void run(POI2D* q, size_t n)
+		{
+			if (!neighbor_reliable) throw std::string("opencorr_b200: RegionFit2D::compute needs setNeighbor() first");
+			b200::Engine& e = b200::Engine::get();
+			std::lock_guard<std::mutex> g(e.lock);
+			e.check(ocb_region_fit2d(e.context(), neighbor_reliable->data(), neighbor_reliable->size(), q, n, neighbor_search_radius, neighbor_number_min));
+		}
+	};
+
+	class RegionFit3D : public DVC
+	{
+	protected:
+		std::vector<POI3D>* neighbor_reliable = nullptr;
+		float neighbor_search_radius;
+		int neighbor_number_min;
+
+	public:
+		RegionFit3D(float neighbor_search_radius, int neighbor_number_min, int thread_number)
+		{
+			this->neighbor_search_radius = neighbor_search_radius;
+			this->neighbor_number_min = neighbor_number_min;
+			this->thread_number = thread_number;
+		}
+		~RegionFit3D() {}
+		float getSearchRadius() const { return neighbor_search_radius; }
+		int getNeighborMin() const { return neighbor_number_min; }
+		void setSearchRadius(float neighbor_search_radius) { this->neighbor_search_radius = neighbor_search_radius; }
+		void setNeighborMin(int neighbor_number_min) { this->neighbor_number_min = neighbor_number_min; }
+		void setNeighbor(std::vector<POI3D>& reliable_pois) { neighbor_reliable = &reliable_pois; }
+
+		void prepare() {}
+		void compute(POI3D* poi) { run(poi, 1); }
+		void compute(std::vector<POI3D>& poi_queue) { run(poi_queue.data(), poi_queue.size()); }
+
+	private:
+		void run(POI3D* q, size_t n)
+		{
+			if (!neighbor_reliable) throw std::string("opencorr_b200: RegionFit3D::compute needs setNeighbor() first");
+			b200::Engine& e = b200::Engine::get();
+			std::lock_guard<std::mutex> g(e.lock);
+			e.check(ocb_region_fit3d(e.context(), neighbor_reliable->data(), neighbor_reliable->size(), q, n, neighbor_search_radius, neighbor_number_min));
+		}
+	};
+
 	// NR2D1 (forward-additive Newton-Raphson), reference src/oc_nr.h:46-71, src/oc_nr.cpp:66-334
 	class NR2D1 : public DIC
 	{

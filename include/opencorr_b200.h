@@ -329,6 +329,24 @@ int ocb_strain3d_series_dev(ocb_ctx* ctx, void* d_poi3d, size_t n_frames, size_t
 int ocb_strain2ds_series_dev(ocb_ctx* ctx, void* d_poi2ds, size_t n_frames, size_t n, float radius, int min_neighbors, float zncc_threshold,
 	int approximation);
 
+/* ---- RegionFit2D / RegionFit3D (src/oc_region_fit.cpp): a new initial guess for unreliable POIs from their reliable neighbours.
+ *      setNeighbor(reliable) + prepare + compute(queue), the reliable set read when the call runs.  For every queue POI with a
+ *      finite position: the n_reliable reliable records (POI2D / POI3D, the same kind as the queue) whose float squared distance
+ *      (x, y(, z)) is strictly below radius^2 are its neighbours (a negative radius acts as its magnitude); when fewer than
+ *      min_neighbors are found, the min(min_neighbors, n_reliable) nearest take their place (ties to the lower reliable index).
+ *      Every neighbour counts, whatever its ZNCC.  With at least min_neighbors of them, the least-squares plane
+ *      [1, x_i - x, y_i - y(, z_i - z)] over u, v (, w) -- the basic solution when rank-deficient -- writes u ux uy v vx vy
+ *      (POI3D: u ux uy uz v .. wz) and zncc = 0; every other field (POI2D: the second-order terms too) is left as it was, and a
+ *      POI with too few neighbours is left untouched.  Reliable POIs with a non-finite position are no one's neighbour.
+ *      OCB_ERR_ARG, with nothing written, for NULL records with a count > 0 or either count >= 2^31.  n = 0 does nothing.  The
+ *      host variants copy both sets and the queue back; the _dev variants take BORROWED device records and only enqueue
+ *      (single-device context).  One readback and the same five launches per call whatever the counts; on a group context the
+ *      first member runs the host variants. */
+int ocb_region_fit2d(ocb_ctx* ctx, const void* reliable, size_t n_reliable, void* poi2d, size_t n, float radius, int min_neighbors);
+int ocb_region_fit3d(ocb_ctx* ctx, const void* reliable, size_t n_reliable, void* poi3d, size_t n, float radius, int min_neighbors);
+int ocb_region_fit2d_dev(ocb_ctx* ctx, const void* d_reliable, size_t n_reliable, void* d_poi2d, size_t n, float radius, int min_neighbors);
+int ocb_region_fit3d_dev(ocb_ctx* ctx, const void* d_reliable, size_t n_reliable, void* d_poi3d, size_t n, float radius, int min_neighbors);
+
 /* ---- Stereo reconstruction: Calibration::prepare / undistort (src/oc_calibration.cpp:161-264) and
  *      Stereovision::reconstruct (src/oc_stereovision.cpp:70-133) ----------------------------------------------------------
  * intrinsics: the 13 floats of CameraIntrinsics (src/oc_calibration.h:25-35), fx fy fs cx cy k1 k2 k3 k4 k5 k6 p1 p2.

@@ -6,4 +6,4 @@ include/opencorr_b200.h; this package is the Python mirror of the reference's op
 """
 from ._capi import OpenCorrB200Error, LIB_PATH  # noqa: F401
 from .api import (Calibration, Engine, EpipolarSearch, FFTCC2D, FFTCC3D, ICGN2D1, ICGN2D2, ICGN3D1, ICLM2D1, ICLM2D2, NR2D1, Strain, P2, P3, POI2D_FLOATS,  # noqa: F401
-                  POI3D_FLOATS, SIFT3D, SIFT3D_DEFAULT_CONFIG, Stereovision, default_engine, make_poi2d, make_poi3d)
+                  POI3D_FLOATS, RegionFit2D, RegionFit3D, SIFT3D, SIFT3D_DEFAULT_CONFIG, Stereovision, default_engine, make_poi2d, make_poi3d)

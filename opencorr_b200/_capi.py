@@ -97,6 +97,10 @@ SIGNATURES = {
     "ocb_strain2d_series_dev": (_i, [_vp, _vp, _sz, _sz, _f, _i, _f, _i]),
     "ocb_strain3d_series_dev": (_i, [_vp, _vp, _sz, _sz, _f, _i, _f, _i]),
     "ocb_strain2ds_series_dev": (_i, [_vp, _vp, _sz, _sz, _f, _i, _f, _i]),
+    "ocb_region_fit2d": (_i, [_vp, _vp, _sz, _vp, _sz, _f, _i]),
+    "ocb_region_fit3d": (_i, [_vp, _vp, _sz, _vp, _sz, _f, _i]),
+    "ocb_region_fit2d_dev": (_i, [_vp, _vp, _sz, _vp, _sz, _f, _i]),
+    "ocb_region_fit3d_dev": (_i, [_vp, _vp, _sz, _vp, _sz, _f, _i]),
     "ocb_nr2d_prepare": (_i, [_vp]),
     "ocb_nr2d1": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_nr2d1_dev": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),

@@ -398,6 +398,23 @@ class Engine:
         fn = getattr(self._lib, "ocb_strain%s_series_dev" % kind)
         self._ck(fn(self._ctx, int(d_q), n_frames, n, float(radius), int(min_neighbors), float(zncc_threshold), int(approximation)))
 
+    def region_fit(self, reliable, q, radius, min_neighbors):
+        """RegionFit2D / RegionFit3D (reference src/oc_region_fit.cpp) setNeighbor(reliable) + compute(queue): q and reliable are
+        both POI2D [n,25] or both POI3D [n,31]; every POI of q with enough reliable neighbours takes their plane fit as its
+        first-order deformation, with zncc 0 (include/opencorr_b200.h ocb_region_fit2d)."""
+        floats = POI3D_FLOATS if q.ndim == 2 and q.shape[1] == POI3D_FLOATS else POI2D_FLOATS
+        _check_queue(q, floats)
+        _check_queue(reliable, floats)
+        fn = self._lib.ocb_region_fit3d if floats == POI3D_FLOATS else self._lib.ocb_region_fit2d
+        self._ck(fn(self._ctx, _vp(reliable), reliable.shape[0], _vp(q), q.shape[0], float(radius), int(min_neighbors)))
+
+    def region_fit_dev(self, kind, d_reliable, n_reliable, d_q, n, radius, min_neighbors):
+        """region_fit on device records (pointers as ints); kind "2d" or "3d".  Only enqueues."""
+        if kind not in ("2d", "3d"):
+            raise ValueError("kind must be '2d' or '3d'")
+        fn = getattr(self._lib, "ocb_region_fit%s_dev" % kind)
+        self._ck(fn(self._ctx, int(d_reliable), n_reliable, int(d_q), n, float(radius), int(min_neighbors)))
+
     def nr2d_prepare(self):
         self._ck(self._lib.ocb_nr2d_prepare(self._ctx))
 
@@ -1047,6 +1064,58 @@ class Strain:
     setZnccThreshold = set_zncc_threshold
     setDescription = set_description
     setApproximation = set_approximation
+
+
+class _RegionFit:
+    """RegionFit2D / RegionFit3D(float neighbor_search_radius, int neighbor_number_min, int thread_number), reference
+    src/oc_region_fit.h:25-85.  setNeighbor keeps a reference to the reliable queue, which is read when compute runs."""
+    _floats = None
+
+    def __init__(self, neighbor_search_radius, neighbor_number_min, thread_number=0, engine=None):
+        self.engine = engine if engine is not None else default_engine()
+        self.neighbor_search_radius = float(neighbor_search_radius)
+        self.neighbor_number_min = int(neighbor_number_min)
+        self.thread_number = thread_number
+        self.neighbor_reliable = np.zeros((0, self._floats), np.float32)
+
+    def get_search_radius(self):
+        return self.neighbor_search_radius
+
+    def get_neighbor_min(self):
+        return self.neighbor_number_min
+
+    def set_search_radius(self, r):
+        self.neighbor_search_radius = float(r)
+
+    def set_neighbor_min(self, k):
+        self.neighbor_number_min = int(k)
+
+    def set_neighbor(self, reliable_pois):
+        _check_queue(reliable_pois, self._floats)
+        self.neighbor_reliable = reliable_pois
+
+    def prepare(self):
+        """The reference builds its kd-trees here; the grid over the reliable set is built inside compute()."""
+
+    def compute(self, poi_queue):
+        """compute(std::vector<POI>&) on a queue [n, floats]; a single record [floats] is compute(POI*)."""
+        q = poi_queue if poi_queue.ndim == 2 else poi_queue.reshape(1, -1)
+        self.engine.region_fit(self.neighbor_reliable, q, self.neighbor_search_radius, self.neighbor_number_min)
+        return poi_queue
+
+    getSearchRadius = get_search_radius
+    getNeighborMin = get_neighbor_min
+    setSearchRadius = set_search_radius
+    setNeighborMin = set_neighbor_min
+    setNeighbor = set_neighbor
+
+
+class RegionFit2D(_RegionFit):
+    _floats = POI2D_FLOATS
+
+
+class RegionFit3D(_RegionFit):
+    _floats = POI3D_FLOATS
 
 
 class ICGN3D1(_DVC):

@@ -1642,6 +1642,55 @@ int ocb_strain3d_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, float radius, int mi
 	return strain_dev(ctx, ocb::PoiKind::POI3D, d_poi3d, n, radius, min_neighbors, zncc_threshold, approximation);
 }
 
+// ---- RegionFit2D / RegionFit3D: Strain's neighbour search and plane fit over a second, reliable set ------------------
+// The reliable set is checked like the queue: NULL only with n_reliable 0, and at most 2^31 - 1 records (the kernels index it
+// with int).
+static int region_fit_dev(ocb_ctx* ctx, ocb::PoiKind kind, const void* d_reliable, size_t n_reliable, void* d_q, size_t n, float radius,
+	int min_neighbors) {
+	int rc = pair_checks(ctx, "region_fit", d_q, n, (d_reliable || !n_reliable) && n_reliable <= 0x7fffffffull, nullptr, 0, nullptr, true);
+	if (rc != PAIR_GO) return rc;
+	if ((rc = grow(ctx, ctx->d_strain_ws, ocb::strain_workspace_bytes(n_reliable)))) return rc;
+	const cudaError_t e = ocb::region_fit_launch(kind, (const float*)d_reliable, n_reliable, (float*)d_q, n, radius, min_neighbors, ctx->d_strain_ws.p,
+		ctx->sm_count, ctx->stream, &ctx->launches);
+	if (e != cudaSuccess) return set_error(ctx, OCB_ERR_CUDA, "region_fit launch failed: %s", cudaGetErrorString(e));
+	return OCB_OK;
+}
+
+// Both sets are staged in the context's queue buffer, queue first; only the queue is copied back.
+static int region_fit_host(ocb_ctx* ctx, ocb::PoiKind kind, const void* reliable, size_t n_reliable, void* q, size_t n, float radius,
+	int min_neighbors) {
+	if (is_group(ctx)) // every POI may need any reliable POI: not sharded, the first member runs it (as Strain)
+		return on_exec(ctx, [&](ocb_ctx* x) { return region_fit_host(x, kind, reliable, n_reliable, q, n, radius, min_neighbors); });
+	if (!ctx || (!q && n) || (!reliable && n_reliable) || n > 0x7fffffffull || n_reliable > 0x7fffffffull)
+		return set_error(ctx, OCB_ERR_ARG, "region_fit: bad arguments");
+	if (n == 0) return OCB_OK;
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	const size_t rec = (size_t)ocb::poi_floats(kind) * sizeof(float);
+	int rc;
+	if ((rc = grow(ctx, ctx->d_poi, (n + n_reliable) * rec))) return rc;
+	float* const d_q = ctx->d_poi.as<float>();
+	float* const d_rel = d_q + n * (size_t)ocb::poi_floats(kind);
+	OCB_CUDA(ctx, cudaMemcpyAsync(d_q, q, n * rec, cudaMemcpyHostToDevice, ctx->stream));
+	if (n_reliable) OCB_CUDA(ctx, cudaMemcpyAsync(d_rel, reliable, n_reliable * rec, cudaMemcpyHostToDevice, ctx->stream));
+	if ((rc = region_fit_dev(ctx, kind, d_rel, n_reliable, d_q, n, radius, min_neighbors))) return rc;
+	OCB_CUDA(ctx, cudaMemcpyAsync(q, d_q, n * rec, cudaMemcpyDeviceToHost, ctx->stream));
+	OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return OCB_OK;
+}
+
+int ocb_region_fit2d(ocb_ctx* ctx, const void* reliable, size_t n_reliable, void* poi2d, size_t n, float radius, int min_neighbors) {
+	return region_fit_host(ctx, ocb::PoiKind::POI2D, reliable, n_reliable, poi2d, n, radius, min_neighbors);
+}
+int ocb_region_fit3d(ocb_ctx* ctx, const void* reliable, size_t n_reliable, void* poi3d, size_t n, float radius, int min_neighbors) {
+	return region_fit_host(ctx, ocb::PoiKind::POI3D, reliable, n_reliable, poi3d, n, radius, min_neighbors);
+}
+int ocb_region_fit2d_dev(ocb_ctx* ctx, const void* d_reliable, size_t n_reliable, void* d_poi2d, size_t n, float radius, int min_neighbors) {
+	return region_fit_dev(ctx, ocb::PoiKind::POI2D, d_reliable, n_reliable, d_poi2d, n, radius, min_neighbors);
+}
+int ocb_region_fit3d_dev(ocb_ctx* ctx, const void* d_reliable, size_t n_reliable, void* d_poi3d, size_t n, float radius, int min_neighbors) {
+	return region_fit_dev(ctx, ocb::PoiKind::POI3D, d_reliable, n_reliable, d_poi3d, n, radius, min_neighbors);
+}
+
 // Strain over a series: n_frames frames of n records, frame-major.  Their bytes, n_frames n rec_floats floats, must fit a size_t.
 static bool strain_series_fits(ocb::PoiKind kind, size_t n_frames, size_t n) {
 	const size_t rec = (size_t)ocb::poi_floats(kind) * sizeof(float);

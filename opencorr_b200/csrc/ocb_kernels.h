@@ -393,6 +393,11 @@ cudaError_t strain_launch(PoiKind kind, float* d_pois, size_t n, float radius, i
 // search coordinates differ from frame 0's as bits, *moved is set and nothing is written.
 cudaError_t strain_series_launch(PoiKind kind, float* d_pois, size_t n_frames, size_t n, float radius, int k_min, float zncc_threshold,
 	int approximation, void* workspace, int sm_count, cudaStream_t stream, long long* launches, bool* moved);
+// RegionFit2D / RegionFit3D (kind POI2D or POI3D): every queue POI with a finite position and at least k_min neighbours among the
+// n_reliable reliable records (Strain's search over them, no ZNCC filter) takes the plane fit's intercept and slopes as its
+// first-order deformation, with zncc 0.  Workspace: strain_workspace_bytes(n_reliable); one readback and five launches per call.
+cudaError_t region_fit_launch(PoiKind kind, const float* d_reliable, size_t n_reliable, float* d_queue, size_t n, float radius, int k_min,
+	void* workspace, int sm_count, cudaStream_t stream, long long* launches);
 // FFTCC2D: which of the three kernels a window takes, and what that kernel needs
 constexpr int FFTW32_WARPS = 4;     // fftcc2d_w32.cu: one-POI warps per CTA
 constexpr int FFTREG_THREADS = 128; // fftcc2d_reg.cu: one thread per window row, 128 / N POIs per CTA

@@ -18,6 +18,10 @@
 //
 // Over a series of frames that share their positions (strain_series_kernel), the bbox, grid and sort run once on frame 0 and
 // each POI's neighbours are searched once; only the fits run per frame.
+//
+// RegionFit2D / RegionFit3D (region_fit_kernel) is the same search and fit with the neighbours taken from a second set of POIs
+// (the reliable ones, binned, sorted and gathered by the same kernels) and the fit itself as the output: its intercept and
+// slopes become a queue POI's first-order deformation, an initial guess for IC-GN.
 #include <stdint.h>
 #include <string.h>
 
@@ -628,9 +632,96 @@ cudaError_t strain_run(float* d_pois, size_t n, size_t n_frames, float radius, i
 	return launched(launches);
 }
 
+// RegionFit2D::compute(POI2D*) / RegionFit3D::compute(POI3D*) (src/oc_region_fit.cpp:91-170, :268-355), one warp per queue POI
+// i < n with a finite position (any other is left alone).  Its neighbours are the reliable POIs -- sorted and gathered into pos /
+// disp, n_valid of them -- within the radius, or the k_min nearest when fewer are found, every one of them whatever its ZNCC (the
+// fit flag pos.w is not read).  With at least k_min neighbours, lane 0 writes the plane fit's intercept and slopes to the
+// first-order deformation (u, ux, uy(, uz), v, ...) and sets zncc to 0; every other field stays as it was.
+template <PoiKind K>
+__global__ void __launch_bounds__(256) region_fit_kernel(float* __restrict__ queue, int n, int n_valid, StrainGrid g, const unsigned int* __restrict__ keys,
+	const int* __restrict__ order, const float4* __restrict__ pos, const float4* __restrict__ disp, float radius, int k_min) {
+	typedef SL<K> L;
+	constexpr int D = L::SD;
+	const int lane = threadIdx.x & 31;
+	const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	const int n_warps = (gridDim.x * blockDim.x) >> 5;
+	const float r2 = __fmul_rn(radius, radius);
+	for (int i = warp_global; i < n; i += n_warps) {
+		float* const p = queue + (size_t)i * poi_floats(K);
+		if (!finite_position<K>(p)) continue;
+		const float4 centre = make_float4(p[0], p[1], D == 3 ? p[2] : 0.f, 0.f);
+		int run_lo, run_hi;
+		neighbour_runs<D>(g, centre, keys, n_valid, lane, run_lo, run_hi);
+		FitSums<D> sums;
+		sums.clear();
+		if (radius_visit<D>(centre, run_lo, run_hi, r2, pos, lane, [&](int j, const float4& q) { sums.add(centre, q, __ldg(disp + j)); }) < k_min) {
+			sums.clear(); // oc_region_fit.cpp:116-126: the k nearest replace the radius set
+			knn_visit<D>(centre, k_min, n_valid, order, pos, lane, [&](int j) {
+				if (lane == 0) sums.add(centre, __ldg(pos + j), __ldg(disp + j));
+			});
+		}
+		sums.reduce();
+		if (lane == 0 && sums.a[0] >= (double)k_min) {
+			double x[D][D + 1];
+			solve_normal<D>(sums, x);
+			const int field[3] = { L::U, L::V, L::W };
+#pragma unroll
+			for (int k = 0; k < D; k++)
+#pragma unroll
+				for (int c = 0; c <= D; c++) p[field[k] + c] = (float)x[k][c];
+			p[L::Z0] = 0.f;
+		}
+	}
+}
+
+// bbox of the reliable set and its finite count (the call's one readback), keys, sort, gather, fit: always these five launches
+template <PoiKind K>
+cudaError_t region_fit_run(const float* d_reliable, size_t n_reliable, float* d_queue, size_t n, float radius, int k_min, const StrainWs& w,
+	int sm_count, cudaStream_t stream, long long* launches) {
+	const int threads = 256;
+	int blocks = (int)((n_reliable + threads - 1) / threads);
+	if (blocks > sm_count * 8) blocks = sm_count * 8;
+	if (blocks < 1) blocks = 1;
+	cudaError_t e;
+	unsigned int hb[8] = { 0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u, 0u };
+	if ((e = cudaMemcpyAsync(w.bbox, hb, sizeof(hb), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+	strain_bbox_kernel<K, false><<<blocks, threads, 0, stream>>>(d_reliable, (int)n_reliable, w.bbox, 1);
+	if ((e = launched(launches)) != cudaSuccess || (e = cudaMemcpyAsync(hb, w.bbox, sizeof(hb), cudaMemcpyDeviceToHost, stream)) != cudaSuccess
+		|| (e = cudaStreamSynchronize(stream)) != cudaSuccess)
+		return e;
+	// no reliable POI with a finite position: an empty grid, so that every query finds no neighbour (and, with k_min <= 0,
+	// is fitted over none, as the reference's arithmetic does)
+	const int n_valid = (int)hb[6];
+	float lo[3] = { 0.f, 0.f, 0.f }, hi[3] = { 0.f, 0.f, 0.f };
+	for (int d = 0; d < SL<K>::SD && n_valid; d++) { lo[d] = ordered_to_float(hb[d]); hi[d] = ordered_to_float(hb[3 + d]); }
+	StrainGrid g;
+	strain_grid_plan(SL<K>::SD, lo, hi, radius, &g);
+	strain_keys_kernel<K><<<blocks, threads, 0, stream>>>(d_reliable, (int)n_reliable, g, w.keys_in, w.vals_in);
+	if ((e = launched(launches)) != cudaSuccess) return e;
+	const int end_bit = 32 - __builtin_clz(g.n_cells);
+	size_t cub_bytes = w.cub_bytes;
+	if ((e = cub::DeviceRadixSort::SortPairs(w.cub_temp, cub_bytes, w.keys_in, w.keys_out, w.vals_in, w.vals_out, (int)n_reliable, 0, end_bit,
+		stream)) != cudaSuccess)
+		return e;
+	++*launches;
+	strain_gather_kernel<K><<<blocks, threads, 0, stream>>>(d_reliable, (int)n_reliable, w.vals_out, -INFINITY, w.pos, w.disp, w.fpos);
+	if ((e = launched(launches)) != cudaSuccess) return e;
+	long long grid = ((long long)n * 32 + threads - 1) / threads;
+	if (grid > (long long)sm_count * 8) grid = (long long)sm_count * 8;
+	region_fit_kernel<K><<<(int)grid, threads, 0, stream>>>(d_queue, (int)n, n_valid, g, w.keys_out, w.vals_out, w.pos, w.disp, radius, k_min);
+	return launched(launches);
+}
+
 } // namespace
 
 size_t strain_workspace_bytes(size_t n, size_t n_frames) { return StrainWs(nullptr, n, n_frames).bytes; }
+
+cudaError_t region_fit_launch(PoiKind kind, const float* d_reliable, size_t n_reliable, float* d_queue, size_t n, float radius, int k_min,
+	void* workspace, int sm_count, cudaStream_t stream, long long* launches) {
+	const StrainWs w(workspace, n_reliable, 1);
+	if (kind == PoiKind::POI3D) return region_fit_run<PoiKind::POI3D>(d_reliable, n_reliable, d_queue, n, radius, k_min, w, sm_count, stream, launches);
+	return region_fit_run<PoiKind::POI2D>(d_reliable, n_reliable, d_queue, n, radius, k_min, w, sm_count, stream, launches);
+}
 
 cudaError_t strain_launch(PoiKind kind, float* d_pois, size_t n, float radius, int k_min, float zncc_threshold, int approximation, long long only,
 	void* workspace, int sm_count, cudaStream_t stream, long long* launches) {
