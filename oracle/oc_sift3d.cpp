@@ -11,9 +11,9 @@
 //   - A mirrored blur index that is still out of range (:424-536, when a line is not longer than the blur radius) is clamped
 //     into the line, and only the voxels of the line are written (the reference's border loops can run past its end).
 //   - y_max of the orientation window multiplies by the unit where the other bounds divide (:870): reproduced.
-//   - Matching post-pass (:1306-1390): kp_matches[j + 1] read one past the end (:1335) and a many-to-one run that ends the
-//     list (never pushed to mto_tar_amount, :1349-1356) both mean "the run ends here".  std::sort (not stable) orders runs of
-//     equal tar_idx; here both sorts are stable, so a run keeps the descending ref_idx order of the first sort.  If every
+//   - Matching post-pass (:1306-1390): kp_matches[j + 1] is read one past the resized end (:1335), where the stale element is a
+//     row that failed the ratio test (tar_idx -1), so a many-to-one run that ends the list is closed like the others: here
+//     every maximal run, the last one included.  std::sort (not stable) orders runs of equal tar_idx; here both sorts are stable, so a run keeps the descending ref_idx order of the first sort.  If every
 //     reference keypoint passes the ratio test, matched_amount stays 0 and nothing is returned (:1309-1317): reproduced.
 //
 // Besides the reference's products, the oracle reports float64 margins of the decisions a rounding difference could flip:

@@ -1,5 +1,5 @@
 """CPU: the SIFT3D pyramid plan (ocb::sift3d_plan, opencorr_b200/csrc/ocb_kernels.h) compiled for the host.  On every case of
-sift3d_cases.py the octave count, the octaves' dimensions and units and the layers' scales and sigmas equal a float32 restatement
+sift3d_cases.py (CASES and SWEEP) the octave count, the octaves' dimensions and units and the layers' scales and sigmas equal a float32 restatement
 of createGaussianPyramid (src/oc_sift.cpp:676-739), and every blurred layer's radii and weights are the oracle's blur_kernel at
 that layer's sigma and units, bit for bit.  The refusals sit exactly at their bounds: n_octave_layers 13 / 14, the unit ratio
 whose blur radius first exceeds 64 voxels, and n_octave_layers x voxels = 2^62."""
@@ -92,6 +92,7 @@ def _bits(x):
 def test_sift3d_plan_cases(tmp_path):
     assert np.load(os.path.join(ROOT, sc.CROP))["ref"].shape == sc.CASES["al_foam4_crop"][0][::-1]
     cases = {name: (dims, unit, sc.cfg(**kw)) for name, (dims, unit, kw) in sc.CASES.items()}
+    cases.update({name: (dims, unit, sc.cfg(**kw)) for name, (dims, unit, kw, _, _) in sc.SWEEP.items()})
     got = plans(tmp_path, cases)
     for name, (dims, unit, cfg) in cases.items():
         p = got[name]
