@@ -347,6 +347,32 @@ int ocb_region_fit3d(ocb_ctx* ctx, const void* reliable, size_t n_reliable, void
 int ocb_region_fit2d_dev(ocb_ctx* ctx, const void* d_reliable, size_t n_reliable, void* d_poi2d, size_t n, float radius, int min_neighbors);
 int ocb_region_fit3d_dev(ocb_ctx* ctx, const void* d_reliable, size_t n_reliable, void* d_poi3d, size_t n, float radius, int min_neighbors);
 
+/* ---- Recovery of unreliable POIs: rounds of RegionFit and IC-GN in one call (the loop of the reference's
+ *      examples/test_3d_reconstruction_sift_icgn2_regfit.cpp:215-270).  q: n registered records (POI2D: ICGN2D<order> on the pair of
+ *      ocb_set_images_2d*, prepared; POI3D: ICGN3D1 on the volume pair, prepared).
+ *      1. Once: U = { i : zncc < zncc_low || convergence > conv } and R = { i not in U : zncc >= zncc_high }, both in queue order
+ *         (literal float comparisons: a NaN field fails both).  Every other POI is left alone.
+ *      2. Round k, while k < max_rounds and U is not empty: RegionFit (ocb_region_fit*_dev, radius, min_neighbors) over the
+ *         reliable set in its current order, on U's working records; the pair IC-GN on them (the plan of a _dev pair call over
+ *         |U| POIs); every one with zncc >= zncc_high && convergence <= conv is accepted: written to q and appended to the
+ *         reliable set in queue order, and leaves U.  recovered[k] = how many; the loop stops after a round that accepts none.
+ *      3. A POI never accepted keeps its bytes in q; its failed records only seed its next round's fit, as in the example.
+ *      Unlike the example, whose erase inside its index loop skips the POI after each accepted one for that round, every POI
+ *      that passes is accepted.  recovered (max_rounds entries, zero past the last round run, or NULL) and *remaining (|U| at the
+ *      end, or NULL) are written only on success.  Refused with nothing written, before any device work: the pair call's checks
+ *      and plan, order not 1 or 2, max_rounds < 0, NaN conv / zncc_high / zncc_low, NULL records with n > 0, n >= 2^31.
+ *      The host variants stage the queue once and copy it back once; the _dev variants take device records and synchronise the
+ *      stream (the per-round counts size the next launches), and need a single-device context.  On a group context the first
+ *      member runs the host variants.  Launches: two for the classification, then one move and nine per round, whatever n. */
+int ocb_icgn2d_recover(ocb_ctx* ctx, int order, void* poi2d, size_t n, int rx, int ry, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+int ocb_icgn2d_recover_dev(ocb_ctx* ctx, int order, void* d_poi2d, size_t n, int rx, int ry, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+int ocb_icgn3d_recover(ocb_ctx* ctx, void* poi3d, size_t n, int rx, int ry, int rz, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+int ocb_icgn3d_recover_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int rz, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+
 /* ---- Stereo reconstruction: Calibration::prepare / undistort (src/oc_calibration.cpp:161-264) and
  *      Stereovision::reconstruct (src/oc_stereovision.cpp:70-133) ----------------------------------------------------------
  * intrinsics: the 13 floats of CameraIntrinsics (src/oc_calibration.h:25-35), fx fy fs cx cy k1 k2 k3 k4 k5 k6 p1 p2.

@@ -101,6 +101,10 @@ SIGNATURES = {
     "ocb_region_fit3d": (_i, [_vp, _vp, _sz, _vp, _sz, _f, _i]),
     "ocb_region_fit2d_dev": (_i, [_vp, _vp, _sz, _vp, _sz, _f, _i]),
     "ocb_region_fit3d_dev": (_i, [_vp, _vp, _sz, _vp, _sz, _f, _i]),
+    "ocb_icgn2d_recover": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
+    "ocb_icgn2d_recover_dev": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
+    "ocb_icgn3d_recover": (_i, [_vp, _vp, _sz, _i, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
+    "ocb_icgn3d_recover_dev": (_i, [_vp, _vp, _sz, _i, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
     "ocb_nr2d_prepare": (_i, [_vp]),
     "ocb_nr2d1": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_nr2d1_dev": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),

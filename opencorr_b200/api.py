@@ -415,6 +415,40 @@ class Engine:
         fn = getattr(self._lib, "ocb_region_fit%s_dev" % kind)
         self._ck(fn(self._ctx, int(d_reliable), n_reliable, int(d_q), n, float(radius), int(min_neighbors)))
 
+    def icgn2d_recover(self, order, q, rx, ry, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """Recover the unreliable POIs of a registered POI2D queue q [n,25] in place: rounds of RegionFit2D over the reliable POIs
+        and ICGN2D<order> on the unreliable ones, each POI that passes moved into the reliable set, until a round recovers none
+        or max_rounds have run (include/opencorr_b200.h ocb_icgn2d_recover).  Returns (recovered int64 (max_rounds,): the POIs
+        accepted in each round, remaining: the POIs still unreliable)."""
+        _check_queue(q, POI2D_FLOATS)
+        return self._recover(self._lib.ocb_icgn2d_recover, (int(order), _vp(q), q.shape[0], rx, ry), conv, stop, radius, min_neighbors,
+                             zncc_high, zncc_low, max_rounds)
+
+    def icgn3d_recover(self, q, rx, ry, rz, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """icgn2d_recover for a POI3D queue q [n,31], with RegionFit3D and ICGN3D1.  Returns (recovered, remaining)."""
+        _check_queue(q, POI3D_FLOATS)
+        return self._recover(self._lib.ocb_icgn3d_recover, (_vp(q), q.shape[0], rx, ry, rz), conv, stop, radius, min_neighbors, zncc_high,
+                             zncc_low, max_rounds)
+
+    def icgn2d_recover_dev(self, order, d_q, n, rx, ry, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """icgn2d_recover on device records (a pointer as an int); synchronises the stream.  Returns (recovered, remaining)."""
+        return self._recover(self._lib.ocb_icgn2d_recover_dev, (int(order), int(d_q), n, rx, ry), conv, stop, radius, min_neighbors,
+                             zncc_high, zncc_low, max_rounds)
+
+    def icgn3d_recover_dev(self, d_q, n, rx, ry, rz, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """icgn3d_recover on device records (a pointer as an int); synchronises the stream.  Returns (recovered, remaining)."""
+        return self._recover(self._lib.ocb_icgn3d_recover_dev, (int(d_q), n, rx, ry, rz), conv, stop, radius, min_neighbors, zncc_high,
+                             zncc_low, max_rounds)
+
+    def _recover(self, fn, head, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        if int(max_rounds) < 0:
+            raise ValueError("max_rounds must be >= 0")
+        counts = np.zeros(int(max_rounds), np.uint64)
+        remaining = ctypes.c_size_t(0)
+        self._ck(fn(self._ctx, *head, float(conv), float(stop), float(radius), int(min_neighbors), float(zncc_high), float(zncc_low),
+                    int(max_rounds), _vp(counts) if len(counts) else None, ctypes.byref(remaining)))
+        return counts.astype(np.int64), int(remaining.value)
+
     def nr2d_prepare(self):
         self._ck(self._lib.ocb_nr2d_prepare(self._ctx))
 

@@ -183,6 +183,8 @@ struct ocb_ctx {
 	bool bands_fresh = false;         // nothing has been enqueued on `stream` since the banded upload
 	DevBuf d_cand;      // EpipolarSearch candidate queue
 	DevBuf d_strain_ws; // Strain: sort keys / compact neighbour arrays / cub scratch
+	// the recovery calls: index lists, counts and cub scratch; the reliable set and the two working sets of records
+	DevBuf recover_ws, recover_rec;
 	DevBuf d_stereo;    // stereo reconstruction / undistortion: staged points
 	ocb::Sift3d* sift3d = nullptr; // SIFT3D working buffers and the products of the last ocb_sift3d call
 };
@@ -1796,6 +1798,164 @@ int ocb_icgn3d1_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int r
 int ocb_icgn3d1(ocb_ctx* ctx, void* poi3d, size_t n, int rx, int ry, int rz, float conv, float stop) {
 	return pair_host(ctx, "icgn3d1", nullptr, poi3d, n, OCB_POI3D_FLOATS, OCB_GROUP_MIN_3D, STAGED,
 		[=](ocb_ctx* x, float* d, size_t m) { return ocb_icgn3d1_dev(x, d, m, rx, ry, rz, conv, stop); });
+}
+
+// ---- Recovery: rounds of RegionFit and IC-GN over the unreliable POIs of a registered queue --------------------------
+// The registration a recovery call runs on its working records: ICGN2D1 / ICGN2D2 (np 6 / 12) on the image pair, or ICGN3D1
+// (dim 3) on the volume pair.
+struct RecoverMethod {
+	int dim, np, r[3];
+	float conv, stop;
+};
+
+// The checks of a recovery call, before any device work: those of the method's pair call, then the order, max_rounds, NaN
+// thresholds and the method's plan.  Returns the refusal, OCB_OK when n = 0, or PAIR_GO.
+static int recover_checks(ocb_ctx* ctx, const char* what, const RecoverMethod& m, const void* q, size_t n, float zncc_high, float zncc_low,
+	int max_rounds) {
+	const bool radii = m.r[0] >= 1 && m.r[1] >= 1 && (m.dim == 2 || m.r[2] >= 1);
+	const char* refusal = nullptr;
+	if (m.dim == 2 && m.np != 6 && m.np != 12) refusal = "order must be 1 or 2";
+	else if (max_rounds < 0) refusal = "max_rounds must be >= 0";
+	else if (m.conv != m.conv || zncc_high != zncc_high || zncc_low != zncc_low) refusal = "conv, zncc_high and zncc_low must not be NaN";
+	int rc = pair_checks(ctx, what, q, n, radii, refusal, m.dim, m.dim == 2 ? &ocb_ctx::prepared2 : &ocb_ctx::prepared3, true);
+	if (rc != PAIR_GO) return rc;
+	if (m.dim == 2) {
+		ocb::Icgn2dPlan plan;
+		rc = icgn2d_plan_or_error(ctx, n, n, m.np, m.r[0], m.r[1], false, &plan);
+	} else {
+		ocb::Icgn3dPlan plan;
+		rc = icgn3d1_plan_or_error(ctx, m.r[0], m.r[1], m.r[2], &plan);
+	}
+	return rc ? rc : PAIR_GO;
+}
+
+// The pair launch of the method on the k device records q, with the plan a _dev pair call over k POIs chooses
+static int recover_register(ocb_ctx* ctx, const RecoverMethod& m, float* q, size_t k) {
+	if (m.dim == 2) return icgn2d_run(ctx, m.np, ctx->img2, q, k, k, m.r[0], m.r[1], m.conv, m.stop, nullptr, nullptr);
+	ocb::Icgn3dPlan plan;
+	if (const int rc = icgn3d1_plan_or_error(ctx, m.r[0], m.r[1], m.r[2], &plan)) return rc;
+	return launched(ctx, "icgn3d1",
+		ocb::icgn3d1_launch(plan, ctx->img3, q, k, m.r[0], m.r[1], m.r[2], m.conv, m.stop, ctx->sm_count, ctx->d_counter + 1, ctx->stream));
+}
+
+// The recovery loop on the n device records d_q (1 <= n < 2^31), after recover_checks:
+//   classification: two selections over the queue (reliable R, unreliable U, each in queue order) and one readback of their sizes;
+//   with max_rounds = 0 or U empty, nothing more.  Otherwise one move gathers R into the reliable set and U into working set 0;
+//   round k: RegionFit over the reliable set on the working records (five launches, one readback), the pair registration on them,
+//   two selections (accepted, kept) and one move that appends the accepted records to the reliable set, writes them to d_q and
+//   compacts the kept ones with their queue indices into the other working set; one readback of the accepted count.
+// counts gets one entry per round run, *left the size of U at the end.
+static int recover_run(ocb_ctx* ctx, const RecoverMethod& m, float* d_q, size_t n, float radius, int min_neighbors, float zncc_high, float zncc_low,
+	int max_rounds, std::vector<size_t>* counts, size_t* left) {
+	const ocb::PoiKind kind = m.dim == 2 ? ocb::PoiKind::POI2D : ocb::PoiKind::POI3D;
+	const size_t N = (size_t)ocb::poi_floats(kind);
+	auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+	const size_t list = up(n * sizeof(int)), temp_bytes = ocb::recover_select_bytes(n);
+	int rc;
+	if ((rc = grow(ctx, ctx->recover_ws, 4 * list + 256 + up(temp_bytes))) || (rc = grow(ctx, ctx->recover_rec, 3 * n * N * sizeof(float)))
+		|| (rc = grow(ctx, ctx->d_strain_ws, ocb::strain_workspace_bytes(n))))
+		return rc;
+	char* const b = ctx->recover_ws.as<char>();
+	int* const list1 = (int*)b;                                      // reliable / accepted positions
+	int* const list2 = (int*)(b + list);                             // unreliable / kept positions
+	int* const widx[2] = { (int*)(b + 2 * list), (int*)(b + 3 * list) }; // the working sets' queue indices
+	int* const d_counts = (int*)(b + 4 * list);                      // the sizes of list 1 and list 2
+	void* const temp = b + 4 * list + 256;
+	float* const rel = ctx->recover_rec.as<float>();
+	float* const work[2] = { rel + n * N, rel + 2 * n * N };
+	auto select = [&](const float* rec, size_t k, ocb::RecoverTest test, int* out, int* count) {
+		return launched(ctx, "recover_select",
+			ocb::recover_select_launch(m.dim, rec, k, test, zncc_high, zncc_low, m.conv, out, count, temp, temp_bytes, ctx->stream));
+	};
+	int h[2] = { 0, 0 };
+	auto read_counts = [&](int k) {
+		OCB_CUDA(ctx, cudaMemcpyAsync(h, d_counts, k * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		return (int)OCB_OK;
+	};
+	if ((rc = select(d_q, n, ocb::RecoverTest::RELIABLE, list1, d_counts)) || (rc = select(d_q, n, ocb::RecoverTest::UNRELIABLE, list2, d_counts + 1))
+		|| (rc = read_counts(2)))
+		return rc;
+	size_t n_rel = (size_t)h[0], left_now = (size_t)h[1];
+	*left = left_now;
+	if (max_rounds == 0 || left_now == 0) return OCB_OK;
+	if ((rc = launched(ctx, "recover_move", ocb::recover_move_launch(m.dim, d_q, nullptr, n_rel + left_now, list1, d_counts, rel, nullptr, list2, work[0],
+			 widx[0], ctx->sm_count, ctx->stream))))
+		return rc;
+	for (int round = 0, c = 0; round < max_rounds && left_now; round++, c ^= 1) {
+		const cudaError_t e = ocb::region_fit_launch(kind, rel, n_rel, work[c], left_now, radius, min_neighbors, ctx->d_strain_ws.p, ctx->sm_count,
+			ctx->stream, &ctx->launches);
+		if (e != cudaSuccess) return set_error(ctx, OCB_ERR_CUDA, "region_fit launch failed: %s", cudaGetErrorString(e));
+		if ((rc = recover_register(ctx, m, work[c], left_now)) || (rc = select(work[c], left_now, ocb::RecoverTest::ACCEPTED, list1, d_counts))
+			|| (rc = select(work[c], left_now, ocb::RecoverTest::KEPT, list2, d_counts + 1))
+			|| (rc = launched(ctx, "recover_move", ocb::recover_move_launch(m.dim, work[c], widx[c], left_now, list1, d_counts, rel + n_rel * N, d_q, list2,
+					work[c ^ 1], widx[c ^ 1], ctx->sm_count, ctx->stream)))
+			|| (rc = read_counts(1)))
+			return rc;
+		counts->push_back((size_t)h[0]);
+		n_rel += (size_t)h[0];
+		left_now -= (size_t)h[0];
+		*left = left_now;
+		if (h[0] == 0) break;
+	}
+	return OCB_OK;
+}
+
+// A recovery call: checks, then (host) the queue staged once in the context's queue buffer, the loop, and the queue back once.
+// recovered (max_rounds entries, zero past the last round run) and remaining are written only when the call succeeds.  A
+// device-pointer call (dev) returns after synchronising the stream.  On a group context the host variants run on the first member.
+static int recover_call(ocb_ctx* ctx, const char* what, bool dev, const RecoverMethod& m, void* q, size_t n, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	if (!dev && is_group(ctx)) // every POI may need any reliable POI: not sharded (as RegionFit)
+		return on_exec(ctx, [&](ocb_ctx* x) {
+			return recover_call(x, what, false, m, q, n, radius, min_neighbors, zncc_high, zncc_low, max_rounds, recovered, remaining);
+		});
+	int rc = recover_checks(ctx, what, m, q, n, zncc_high, zncc_low, max_rounds);
+	std::vector<size_t> counts;
+	size_t left = 0;
+	if (rc == PAIR_GO) {
+		const size_t bytes = n * (size_t)(m.dim == 2 ? OCB_POI2D_FLOATS : OCB_POI3D_FLOATS) * sizeof(float);
+		float* d = (float*)q;
+		if (!dev) {
+			if ((rc = grow(ctx, ctx->d_poi, bytes))) return rc;
+			d = ctx->d_poi.as<float>();
+			OCB_CUDA(ctx, cudaMemcpyAsync(d, q, bytes, cudaMemcpyHostToDevice, ctx->stream));
+		}
+		if ((rc = recover_run(ctx, m, d, n, radius, min_neighbors, zncc_high, zncc_low, max_rounds, &counts, &left))) return rc;
+		if (!dev) OCB_CUDA(ctx, cudaMemcpyAsync(q, d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	} else if (rc != OCB_OK) {
+		return rc;
+	}
+	if (recovered) {
+		memset(recovered, 0, (size_t)max_rounds * sizeof(size_t));
+		if (!counts.empty()) memcpy(recovered, counts.data(), counts.size() * sizeof(size_t));
+	}
+	if (remaining) *remaining = left;
+	return OCB_OK;
+}
+
+int ocb_icgn2d_recover(ocb_ctx* ctx, int order, void* poi2d, size_t n, int rx, int ry, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	return recover_call(ctx, "icgn2d_recover", false, { 2, order == 1 ? 6 : (order == 2 ? 12 : 0), { rx, ry, 0 }, conv, stop }, poi2d, n, radius,
+		min_neighbors, zncc_high, zncc_low, max_rounds, recovered, remaining);
+}
+int ocb_icgn2d_recover_dev(ocb_ctx* ctx, int order, void* d_poi2d, size_t n, int rx, int ry, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	OCB_NO_GROUP(ctx, "icgn2d_recover_dev");
+	return recover_call(ctx, "icgn2d_recover", true, { 2, order == 1 ? 6 : (order == 2 ? 12 : 0), { rx, ry, 0 }, conv, stop }, d_poi2d, n, radius,
+		min_neighbors, zncc_high, zncc_low, max_rounds, recovered, remaining);
+}
+int ocb_icgn3d_recover(ocb_ctx* ctx, void* poi3d, size_t n, int rx, int ry, int rz, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	return recover_call(ctx, "icgn3d_recover", false, { 3, 0, { rx, ry, rz }, conv, stop }, poi3d, n, radius, min_neighbors, zncc_high, zncc_low,
+		max_rounds, recovered, remaining);
+}
+int ocb_icgn3d_recover_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry, int rz, float conv, float stop, float radius, int min_neighbors,
+	float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	OCB_NO_GROUP(ctx, "icgn3d_recover_dev");
+	return recover_call(ctx, "icgn3d_recover", true, { 3, 0, { rx, ry, rz }, conv, stop }, d_poi3d, n, radius, min_neighbors, zncc_high, zncc_low,
+		max_rounds, recovered, remaining);
 }
 
 // ---- volume series: one reference volume, n_frames target volumes, each frame seeded by the previous one ------------------

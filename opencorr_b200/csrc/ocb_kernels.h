@@ -292,6 +292,19 @@ cudaError_t reseed_rebuild_launch(int dim, const float* d_seeds, const float* d_
 // scatter: record k of frame g of src (frames x m records, frame-major) -> out[(f0 + g) * n + idx[k]]
 cudaError_t reseed_scatter_launch(int dim, const float* d_src, size_t m, int frames, const int* d_idx, float* d_out, size_t n, int f0, int sm_count,
 	cudaStream_t stream);
+// region_recover.cu: the selections and record moves of the recovery calls (dim: 2 or 3, POI2D or POI3D records).
+// The tests of a record with ZNCC z and convergence c: UNRELIABLE z < zncc_low || c > conv; RELIABLE not UNRELIABLE and
+// z >= zncc_high; ACCEPTED z >= zncc_high && c <= conv; KEPT not ACCEPTED.
+enum class RecoverTest { UNRELIABLE, RELIABLE, ACCEPTED, KEPT };
+// select: idx = the positions i < count whose record d_rec[i] passes `test`, ascending; *d_count = how many
+size_t recover_select_bytes(size_t n); // temporary storage recover_select_launch needs for count <= n
+cudaError_t recover_select_launch(int dim, const float* d_rec, size_t count, RecoverTest test, float zncc_high, float zncc_low, float conv, int* d_idx,
+	int* d_count, void* d_temp, size_t temp_bytes, cudaStream_t stream);
+// move: total = *d_count1 + the length of list 2.  Record k < *d_count1 is src[list1[k]]: it goes to dst1[k] and, with d_q set, to
+// d_q[src_idx[list1[k]]].  Record k2 of list 2 is src[list2[k2]]: it goes to dst2[k2], its queue index (src_idx[list2[k2]], or
+// list2[k2] when src_idx is null) to idx2[k2].
+cudaError_t recover_move_launch(int dim, const float* d_src, const int* d_src_idx, size_t total, const int* d_list1, const int* d_count1, float* d_dst1,
+	float* d_q, const int* d_list2, float* d_dst2, int* d_idx2, int sm_count, cudaStream_t stream);
 // nr2d.cu
 constexpr int NR2D_TILE_MARGIN = 1;
 __host__ __device__ inline int nr2d_tar_w(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * NR2D_TILE_MARGIN + 4 + 3); }
