@@ -230,6 +230,42 @@ int ocb_icgn3d_series_reseed(ocb_ctx* ctx, const void* seeds, void* out, size_t 
 int ocb_icgn3d_series_reseed_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop,
 	int fft_rx, int fft_ry, int fft_rz, float zncc_min, size_t* reseeded);
 
+/* ---- Series that recover unreliable POIs with rounds of RegionFit and IC-GN in the frame where they fail.  Replaces the loop a
+ *      reference user writes to keep a field alive over a load series with the regfit example's recovery in every frame:
+ *        for f: dic.setImages(ref, tar[f]); icgn.prepare(); icgn.compute(queue); the recovery of ocb_icgn2d_recover on queue
+ *      over the series set by ocb_set_series_2d* / ocb_set_series_3d*, frames f = 0 ... n_frames - 1 in order:
+ *        1. every POI is registered from its frame f - 1 record (frame 0: its seed), as ocb_icgn2d_series / ocb_icgn3d_series do;
+ *        2. frame f's n records then go through ocb_icgn2d_recover's rules 1-3 against (ref, tars[f]) with (radius, min_neighbors,
+ *           zncc_high, zncc_low, max_rounds): U and R classified once, each round RegionFit over the reliable set on U's working
+ *           records and IC-GN on them (the plan of a _dev pair call over |U|), accepted POIs written and appended, a POI never
+ *           accepted keeps its bytes;
+ *        3. recovered[f * max_rounds + k] (n_frames x max_rounds counts, zero past the last round run, or NULL) is the number
+ *           accepted in round k of frame f; remaining[f] (n_frames counts, or NULL) is |U| at the end of frame f;
+ *        4. frame f + 1 starts from every POI's final frame-f record: a recovered POI carries its recovered record forward, and a
+ *           POI whose subset was occluded in frame k comes back in frame k + 1 once its neighbours can vouch for it.
+ *      out, recovered and remaining equal, byte for byte, the loop of ocb_set_images_*(ref, tars[f]), the prepare, the pair IC-GN
+ *      (order; 3D ICGN3D1) on all n POIs from frame f - 1's records and ocb_icgn*_recover_dev on them.  3D: always.  2D: when
+ *      OCB_ICGN2D_WPP forces the warps per POI; otherwise the series launches take the warps per POI of a launch over all n POIs
+ *      and the recovery rounds those of |U|, as the loop does.  max_rounds = 0, or thresholds under which no record is
+ *      unreliable, give out byte-identical to the plain series call.
+ * Cost: 2D runs the plain series launch, one scan and one synchronisation; each frame that holds an unreliable record adds the
+ *   recovery rounds (as ocb_icgn2d_recover_dev, plus one launch per round), one series launch of the accepted POIs over the later
+ *   frames, a scatter, a rescan and one more synchronisation.  3D runs the rounds' classification (one synchronisation) in every
+ *   frame.  The workspaces are the context's grow-only buffers.
+ * The _dev variants take BORROWED device seeds and out (recovered, remaining are host pointers), synchronise ctx's stream
+ *   (the counts size the launches) and need a single-device context; on a group context the first member runs the host
+ *   variants.  Pair state (images, prepared tables) is not touched.  Errors are detected before any work and write nothing to
+ *   out, recovered or remaining: OCB_ERR_STATE without a series, OCB_ERR_ARG for bad arguments or sizes, an order not 1 or 2,
+ *   max_rounds < 0 or a NaN conv / zncc_high / zncc_low, OCB_ERR_UNSUPPORTED for a subset the pair calls reject. */
+int ocb_icgn2d_series_recover(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, float radius,
+	int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+int ocb_icgn2d_series_recover_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
+	float radius, int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+int ocb_icgn3d_series_recover(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop, float radius,
+	int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+int ocb_icgn3d_series_recover_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop,
+	float radius, int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining);
+
 /* ---- IC-LM siblings (SURVEY.md section 8(f) N2): ICLM2D1::compute(std::vector<POI2D>&) src/oc_iclm.cpp:360-368
  *      (per POI :150-358) and ICLM2D2 :732-740 (:502-730).  Same prepare() as IC-GN (ocb_icgn2d_prepare).
  *      lambda, alpha, beta = DampingParameter (src/oc_iclm.h:32-37; defaults 100, 0.1, 10; setDamping()). */

@@ -105,6 +105,10 @@ SIGNATURES = {
     "ocb_icgn2d_recover_dev": (_i, [_vp, _i, _vp, _sz, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
     "ocb_icgn3d_recover": (_i, [_vp, _vp, _sz, _i, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
     "ocb_icgn3d_recover_dev": (_i, [_vp, _vp, _sz, _i, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
+    "ocb_icgn2d_series_recover": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
+    "ocb_icgn2d_series_recover_dev": (_i, [_vp, _i, _vp, _vp, _sz, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
+    "ocb_icgn3d_series_recover": (_i, [_vp, _vp, _vp, _sz, _i, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
+    "ocb_icgn3d_series_recover_dev": (_i, [_vp, _vp, _vp, _sz, _i, _i, _i, _f, _f, _f, _i, _f, _f, _i, _vp, _vp]),
     "ocb_nr2d_prepare": (_i, [_vp]),
     "ocb_nr2d1": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),
     "ocb_nr2d1_dev": (_i, [_vp, _vp, _sz, _i, _i, _f, _f]),

@@ -318,6 +318,48 @@ class Engine:
                                                     int(fft_rz), float(zncc_min), _vp(counts)))
         return out, counts.astype(np.int64)
 
+    def icgn2d_series_recover(self, order, seeds, rx, ry, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """icgn2d_series that recovers unreliable POIs in the frame where they fail: each frame's records go through icgn2d_recover's
+        rounds of RegionFit2D and ICGN2D<order> against that frame, and frame f + 1 starts from the recovered records
+        (include/opencorr_b200.h ocb_icgn2d_series_recover).  Returns (records float32 (F, n, 25), recovered int64 (F, max_rounds):
+        the POIs accepted in each round of each frame, remaining int64 (F,): the POIs still unreliable at the end of each frame)."""
+        _check_queue(seeds, POI2D_FLOATS)
+        n_frames = self._series_frames("2d", "icgn2d_series_recover")
+        out = np.empty((n_frames, seeds.shape[0], POI2D_FLOATS), np.float32)
+        return self._series_recover(self._lib.ocb_icgn2d_series_recover, (int(order), _vp(seeds), _vp(out), seeds.shape[0], rx, ry), n_frames, out,
+                                    conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds)
+
+    def icgn3d_series_recover(self, seeds, rx, ry, rz, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """icgn2d_series_recover over the volume series, with RegionFit3D and ICGN3D1.  Returns (records float32 (F, n, 31),
+        recovered int64 (F, max_rounds), remaining int64 (F,))."""
+        _check_queue(seeds, POI3D_FLOATS)
+        n_frames = self._series_frames("3d", "icgn3d_series_recover")
+        out = np.empty((n_frames, seeds.shape[0], POI3D_FLOATS), np.float32)
+        return self._series_recover(self._lib.ocb_icgn3d_series_recover, (_vp(seeds), _vp(out), seeds.shape[0], rx, ry, rz), n_frames, out, conv,
+                                    stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds)
+
+    def icgn2d_series_recover_dev(self, order, d_seeds, d_out, n, rx, ry, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """icgn2d_series_recover on device pointers; synchronises the stream.  Returns (recovered (F, max_rounds), remaining (F,))."""
+        n_frames = self._series_frames("2d", "icgn2d_series_recover")
+        return self._series_recover(self._lib.ocb_icgn2d_series_recover_dev, (int(order), int(d_seeds), int(d_out), n, rx, ry), n_frames, None,
+                                    conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds)
+
+    def icgn3d_series_recover_dev(self, d_seeds, d_out, n, rx, ry, rz, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        """icgn3d_series_recover on device pointers; synchronises the stream.  Returns (recovered (F, max_rounds), remaining (F,))."""
+        n_frames = self._series_frames("3d", "icgn3d_series_recover")
+        return self._series_recover(self._lib.ocb_icgn3d_series_recover_dev, (int(d_seeds), int(d_out), n, rx, ry, rz), n_frames, None, conv,
+                                    stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds)
+
+    def _series_recover(self, fn, head, n_frames, out, conv, stop, radius, min_neighbors, zncc_high, zncc_low, max_rounds):
+        if int(max_rounds) < 0:
+            raise ValueError("max_rounds must be >= 0")
+        recovered = np.zeros((n_frames, int(max_rounds)), np.uint64)
+        remaining = np.zeros(n_frames, np.uint64)
+        self._ck(fn(self._ctx, *head, float(conv), float(stop), float(radius), int(min_neighbors), float(zncc_high), float(zncc_low),
+                    int(max_rounds), _vp(recovered) if recovered.size else None, _vp(remaining)))
+        counts = (recovered.astype(np.int64), remaining.astype(np.int64))
+        return counts if out is None else (out,) + counts
+
     def set_stereo_series(self, ref1, tars1, tars2):
         """A stereo load series for stereo_series: reference view 1 (H, W) and the two views of every frame, tars1 and tars2
         (F, H, W), float32.  Kept apart from set_images_2d's pair and set_series_2d's series."""

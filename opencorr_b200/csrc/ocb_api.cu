@@ -1808,16 +1808,21 @@ struct RecoverMethod {
 	float conv, stop;
 };
 
+// The argument refusal of a recovery call (null: none): the order, max_rounds, NaN thresholds
+static const char* recover_refusal(const RecoverMethod& m, float zncc_high, float zncc_low, int max_rounds) {
+	if (m.dim == 2 && m.np != 6 && m.np != 12) return "order must be 1 or 2";
+	if (max_rounds < 0) return "max_rounds must be >= 0";
+	if (m.conv != m.conv || zncc_high != zncc_high || zncc_low != zncc_low) return "conv, zncc_high and zncc_low must not be NaN";
+	return nullptr;
+}
+
 // The checks of a recovery call, before any device work: those of the method's pair call, then the order, max_rounds, NaN
 // thresholds and the method's plan.  Returns the refusal, OCB_OK when n = 0, or PAIR_GO.
 static int recover_checks(ocb_ctx* ctx, const char* what, const RecoverMethod& m, const void* q, size_t n, float zncc_high, float zncc_low,
 	int max_rounds) {
 	const bool radii = m.r[0] >= 1 && m.r[1] >= 1 && (m.dim == 2 || m.r[2] >= 1);
-	const char* refusal = nullptr;
-	if (m.dim == 2 && m.np != 6 && m.np != 12) refusal = "order must be 1 or 2";
-	else if (max_rounds < 0) refusal = "max_rounds must be >= 0";
-	else if (m.conv != m.conv || zncc_high != zncc_high || zncc_low != zncc_low) refusal = "conv, zncc_high and zncc_low must not be NaN";
-	int rc = pair_checks(ctx, what, q, n, radii, refusal, m.dim, m.dim == 2 ? &ocb_ctx::prepared2 : &ocb_ctx::prepared3, true);
+	int rc = pair_checks(ctx, what, q, n, radii, recover_refusal(m, zncc_high, zncc_low, max_rounds), m.dim,
+		m.dim == 2 ? &ocb_ctx::prepared2 : &ocb_ctx::prepared3, true);
 	if (rc != PAIR_GO) return rc;
 	if (m.dim == 2) {
 		ocb::Icgn2dPlan plan;
@@ -1829,14 +1834,23 @@ static int recover_checks(ocb_ctx* ctx, const char* what, const RecoverMethod& m
 	return rc ? rc : PAIR_GO;
 }
 
-// The pair launch of the method on the k device records q, with the plan a _dev pair call over k POIs chooses
-static int recover_register(ocb_ctx* ctx, const RecoverMethod& m, float* q, size_t k) {
-	if (m.dim == 2) return icgn2d_run(ctx, m.np, ctx->img2, q, k, k, m.r[0], m.r[1], m.conv, m.stop, nullptr, nullptr);
+// The pair launch of the method on the k device records q against img2 (2D) or img3 (3D: its packed gradients and coefficients),
+// with the plan a _dev pair call over k POIs chooses.  The pair calls pass the context's pair, the series calls one frame.
+static int recover_register(ocb_ctx* ctx, const RecoverMethod& m, const ocb::Image2D& img2, const ocb::Image3D& img3, float* q, size_t k) {
+	if (m.dim == 2) return icgn2d_run(ctx, m.np, img2, q, k, k, m.r[0], m.r[1], m.conv, m.stop, nullptr, nullptr);
 	ocb::Icgn3dPlan plan;
 	if (const int rc = icgn3d1_plan_or_error(ctx, m.r[0], m.r[1], m.r[2], &plan)) return rc;
 	return launched(ctx, "icgn3d1",
-		ocb::icgn3d1_launch(plan, ctx->img3, q, k, m.r[0], m.r[1], m.r[2], m.conv, m.stop, ctx->sm_count, ctx->d_counter + 1, ctx->stream));
+		ocb::icgn3d1_launch(plan, img3, q, k, m.r[0], m.r[1], m.r[2], m.conv, m.stop, ctx->sm_count, ctx->d_counter + 1, ctx->stream));
 }
+
+// What a series recovery call needs of recover_run besides the records: the queue indices of the POIs accepted over all rounds
+// (idx, device), in the order the moves appended their records to the reliable set, where those `count` records start at `rec`.
+struct RecoverAccepted {
+	const int* idx = nullptr;
+	const float* rec = nullptr;
+	size_t count = 0;
+};
 
 // The recovery loop on the n device records d_q (1 <= n < 2^31), after recover_checks:
 //   classification: two selections over the queue (reliable R, unreliable U, each in queue order) and one readback of their sizes;
@@ -1844,16 +1858,17 @@ static int recover_register(ocb_ctx* ctx, const RecoverMethod& m, float* q, size
 //   round k: RegionFit over the reliable set on the working records (five launches, one readback), the pair registration on them,
 //   two selections (accepted, kept) and one move that appends the accepted records to the reliable set, writes them to d_q and
 //   compacts the kept ones with their queue indices into the other working set; one readback of the accepted count.
-// counts gets one entry per round run, *left the size of U at the end.
-static int recover_run(ocb_ctx* ctx, const RecoverMethod& m, float* d_q, size_t n, float radius, int min_neighbors, float zncc_high, float zncc_low,
-	int max_rounds, std::vector<size_t>* counts, size_t* left) {
+// counts gets one entry per round run, *left the size of U at the end.  The registration runs against img2 / img3
+// (recover_register).  With acc set, each round adds one launch that collects its accepted queue indices (RecoverAccepted).
+static int recover_run(ocb_ctx* ctx, const RecoverMethod& m, const ocb::Image2D& img2, const ocb::Image3D& img3, float* d_q, size_t n, float radius,
+	int min_neighbors, float zncc_high, float zncc_low, int max_rounds, std::vector<size_t>* counts, size_t* left, RecoverAccepted* acc = nullptr) {
 	const ocb::PoiKind kind = m.dim == 2 ? ocb::PoiKind::POI2D : ocb::PoiKind::POI3D;
 	const size_t N = (size_t)ocb::poi_floats(kind);
 	auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
 	const size_t list = up(n * sizeof(int)), temp_bytes = ocb::recover_select_bytes(n);
 	int rc;
-	if ((rc = grow(ctx, ctx->recover_ws, 4 * list + 256 + up(temp_bytes))) || (rc = grow(ctx, ctx->recover_rec, 3 * n * N * sizeof(float)))
-		|| (rc = grow(ctx, ctx->d_strain_ws, ocb::strain_workspace_bytes(n))))
+	if ((rc = grow(ctx, ctx->recover_ws, 4 * list + 256 + up(temp_bytes) + (acc ? list : 0)))
+		|| (rc = grow(ctx, ctx->recover_rec, 3 * n * N * sizeof(float))) || (rc = grow(ctx, ctx->d_strain_ws, ocb::strain_workspace_bytes(n))))
 		return rc;
 	char* const b = ctx->recover_ws.as<char>();
 	int* const list1 = (int*)b;                                      // reliable / accepted positions
@@ -1861,6 +1876,7 @@ static int recover_run(ocb_ctx* ctx, const RecoverMethod& m, float* d_q, size_t 
 	int* const widx[2] = { (int*)(b + 2 * list), (int*)(b + 3 * list) }; // the working sets' queue indices
 	int* const d_counts = (int*)(b + 4 * list);                      // the sizes of list 1 and list 2
 	void* const temp = b + 4 * list + 256;
+	int* const acc_idx = (int*)(b + 4 * list + 256 + up(temp_bytes)); // with acc: the accepted queue indices
 	float* const rel = ctx->recover_rec.as<float>();
 	float* const work[2] = { rel + n * N, rel + 2 * n * N };
 	auto select = [&](const float* rec, size_t k, ocb::RecoverTest test, int* out, int* count) {
@@ -1878,6 +1894,7 @@ static int recover_run(ocb_ctx* ctx, const RecoverMethod& m, float* d_q, size_t 
 		return rc;
 	size_t n_rel = (size_t)h[0], left_now = (size_t)h[1];
 	*left = left_now;
+	if (acc) *acc = RecoverAccepted{ acc_idx, rel + n_rel * N, 0 };
 	if (max_rounds == 0 || left_now == 0) return OCB_OK;
 	if ((rc = launched(ctx, "recover_move", ocb::recover_move_launch(m.dim, d_q, nullptr, n_rel + left_now, list1, d_counts, rel, nullptr, list2, work[0],
 			 widx[0], ctx->sm_count, ctx->stream))))
@@ -1886,13 +1903,18 @@ static int recover_run(ocb_ctx* ctx, const RecoverMethod& m, float* d_q, size_t 
 		const cudaError_t e = ocb::region_fit_launch(kind, rel, n_rel, work[c], left_now, radius, min_neighbors, ctx->d_strain_ws.p, ctx->sm_count,
 			ctx->stream, &ctx->launches);
 		if (e != cudaSuccess) return set_error(ctx, OCB_ERR_CUDA, "region_fit launch failed: %s", cudaGetErrorString(e));
-		if ((rc = recover_register(ctx, m, work[c], left_now)) || (rc = select(work[c], left_now, ocb::RecoverTest::ACCEPTED, list1, d_counts))
+		if ((rc = recover_register(ctx, m, img2, img3, work[c], left_now))
+			|| (rc = select(work[c], left_now, ocb::RecoverTest::ACCEPTED, list1, d_counts))
 			|| (rc = select(work[c], left_now, ocb::RecoverTest::KEPT, list2, d_counts + 1))
 			|| (rc = launched(ctx, "recover_move", ocb::recover_move_launch(m.dim, work[c], widx[c], left_now, list1, d_counts, rel + n_rel * N, d_q, list2,
 					work[c ^ 1], widx[c ^ 1], ctx->sm_count, ctx->stream)))
+			|| (acc
+				&& (rc = launched(ctx, "recover_collect",
+						ocb::recover_collect_launch(widx[c], left_now, list1, d_counts, acc_idx + acc->count, ctx->sm_count, ctx->stream))))
 			|| (rc = read_counts(1)))
 			return rc;
 		counts->push_back((size_t)h[0]);
+		if (acc) acc->count += (size_t)h[0];
 		n_rel += (size_t)h[0];
 		left_now -= (size_t)h[0];
 		*left = left_now;
@@ -1921,7 +1943,7 @@ static int recover_call(ocb_ctx* ctx, const char* what, bool dev, const RecoverM
 			d = ctx->d_poi.as<float>();
 			OCB_CUDA(ctx, cudaMemcpyAsync(d, q, bytes, cudaMemcpyHostToDevice, ctx->stream));
 		}
-		if ((rc = recover_run(ctx, m, d, n, radius, min_neighbors, zncc_high, zncc_low, max_rounds, &counts, &left))) return rc;
+		if ((rc = recover_run(ctx, m, ctx->img2, ctx->img3, d, n, radius, min_neighbors, zncc_high, zncc_low, max_rounds, &counts, &left))) return rc;
 		if (!dev) OCB_CUDA(ctx, cudaMemcpyAsync(q, d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
 		OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	} else if (rc != OCB_OK) {
@@ -1956,6 +1978,148 @@ int ocb_icgn3d_recover_dev(ocb_ctx* ctx, void* d_poi3d, size_t n, int rx, int ry
 	OCB_NO_GROUP(ctx, "icgn3d_recover_dev");
 	return recover_call(ctx, "icgn3d_recover", true, { 3, 0, { rx, ry, rz }, conv, stop }, d_poi3d, n, radius, min_neighbors, zncc_high, zncc_low,
 		max_rounds, recovered, remaining);
+}
+
+// ---- Series that recover unreliable POIs: the recovery rounds in every frame that holds an unreliable record ---------------
+// What a series recovery call adds to the plain series: the recovery arguments and the host counts, zeroed on entry.
+// recovered[f * max_rounds + k]: the POIs accepted in round k of frame f; remaining[f]: |U| at the end of frame f.
+struct SeriesRecover {
+	float radius;
+	int min_neighbors;
+	float zncc_high, zncc_low;
+	int max_rounds;
+	size_t* recovered;
+	size_t* remaining;
+};
+
+// recover_run on the n records q of frame f against img2 / img3, its counts stored in sr's slots of frame f
+static int series_recover_frame(ocb_ctx* ctx, const RecoverMethod& m, const ocb::Image2D& img2, const ocb::Image3D& img3, float* q, size_t n, int f,
+	const SeriesRecover& sr, RecoverAccepted* acc) {
+	std::vector<size_t> counts;
+	size_t left = 0;
+	if (const int rc = recover_run(ctx, m, img2, img3, q, n, sr.radius, sr.min_neighbors, sr.zncc_high, sr.zncc_low, sr.max_rounds, &counts, &left, acc))
+		return rc;
+	for (size_t k = 0; k < counts.size(); k++) sr.recovered[(size_t)f * sr.max_rounds + k] = counts[k];
+	sr.remaining[f] = left;
+	return OCB_OK;
+}
+
+// The 2D series recovery of reference s.ref against the F frames of s.tar with IC-GN (m) over the n device seeds into d_out:
+//   1. one series launch over all n POIs and frames, as the plain series;
+//   2. one scan of every record for each POI's first UNRELIABLE frame, whose per-frame counts come back in one copy (none: done);
+//   3. for the smallest frame f that holds an unreliable record: the recovery rounds on out[f] against frame f (recover_run, the
+//      rounds' IC-GN with the plan of |U|), collecting the accepted POIs' queue indices; one series launch carries the accepted
+//      records through frames f + 1 ... F - 1 (into ctx->reseed_cont, the plan of n) and they are scattered into out; the POIs
+//      whose first unreliable frame was f, accepted or not, are scanned again from f + 1;
+//   4. step 3 repeats for the next frame that holds an unreliable record.
+// A POI never accepted keeps its frame-f bytes, so its records of the later frames, already in out, stand.
+static int icgn2d_series_recover_run(ocb_ctx* ctx, const RecoverMethod& m, const ocb::Image2D& s, int F, const float* d_seeds, float* d_out, size_t n,
+	const SeriesRecover& sr) {
+	const SubsetMethod2D sm{ false, m.np == 6 ? 1 : 2, nullptr };
+	const size_t frame_px = (size_t)s.w * s.h, rec = OCB_POI2D_FLOATS;
+	const int rx = m.r[0], ry = m.r[1];
+	int rc;
+	if ((rc = subset2d_series_launch(ctx, sm, s, F, d_seeds, d_out, n, n, rx, ry, m.conv, m.stop))) return rc;
+	ReseedWs w;
+	auto scan = [&](int f_begin, const int* idx, size_t count) {
+		const int r = launched(ctx, "recover_scan",
+			ocb::recover_scan_launch(2, d_out, n, f_begin, F, idx, count, sr.zncc_low, m.conv, w.first, w.hist, ctx->sm_count, ctx->stream));
+		return r ? r : reseed_read_hist(ctx, &w);
+	};
+	if ((rc = reseed_workspace(ctx, n, F, 2, &w)) || (rc = scan(0, nullptr, n))) return rc;
+	for (int f = 0; f < F; f++) {
+		const size_t held = (size_t)w.h_hist[f];
+		if (!held) continue;
+		const ocb::Image2D frame{ s.ref, s.tar + (size_t)f * frame_px, s.w, s.h };
+		RecoverAccepted acc;
+		if ((rc = series_recover_frame(ctx, m, frame, ocb::Image3D{}, d_out + (size_t)f * n * rec, n, f, sr, f + 1 < F ? &acc : nullptr))) return rc;
+		if (f + 1 == F) break;
+		if ((rc = launched(ctx, "reseed_select", ocb::reseed_select_launch(w.first, f, n, w.idx, w.count, w.temp, w.temp_bytes, ctx->stream)))) return rc;
+		if (acc.count) {
+			const int rest = F - f - 1;
+			if ((rc = grow(ctx, ctx->reseed_cont, (size_t)rest * acc.count * rec * sizeof(float)))) return rc;
+			float* const cont = ctx->reseed_cont.as<float>();
+			const ocb::Image2D later{ s.ref, s.tar + (size_t)(f + 1) * frame_px, s.w, s.h };
+			if ((rc = subset2d_series_launch(ctx, sm, later, rest, acc.rec, cont, acc.count, n, rx, ry, m.conv, m.stop))
+				|| (rc = launched(ctx, "reseed_scatter",
+						ocb::reseed_scatter_launch(2, cont, acc.count, rest, acc.idx, d_out, n, f + 1, ctx->sm_count, ctx->stream))))
+				return rc;
+		}
+		if ((rc = scan(f + 1, w.idx, held))) return rc;
+	}
+	return OCB_OK;
+}
+
+// Checks and runs the 2D series recovery on a single-device context (device seeds and out): the series call's checks, then
+// recover_refusal and the IC-GN plan, all before any device work.
+static int icgn2d_series_recover_dev(ocb_ctx* ctx, const char* what, const RecoverMethod& m, const void* d_seeds, void* d_out, size_t n,
+	const SeriesRecover& sr) {
+	if (!ctx || ((!d_seeds || !d_out) && n) || m.r[0] < 1 || m.r[1] < 1) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
+	if (m.np != 6 && m.np != 12) return set_error(ctx, OCB_ERR_ARG, "%s: order must be 1 or 2", what);
+	const SeriesStore& s = ctx->series2d;
+	if (!s.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
+	if (const char* refusal = recover_refusal(m, sr.zncc_high, sr.zncc_low, sr.max_rounds)) return set_error(ctx, OCB_ERR_ARG, "%s: %s", what, refusal);
+	if (n == 0) return OCB_OK;
+	int rc;
+	if ((rc = series_size_check(ctx, what, n, s.frames, OCB_POI2D_FLOATS * sizeof(float), false))) return rc;
+	ocb::Icgn2dPlan plan;
+	if ((rc = icgn2d_plan_or_error(ctx, n, n, m.np, m.r[0], m.r[1], false, &plan))) return rc;
+	if (ensure_device(ctx)) return OCB_ERR_CUDA;
+	return icgn2d_series_recover_run(ctx, m, s.view2(0), s.frames, (const float*)d_seeds, (float*)d_out, n, sr);
+}
+
+static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv,
+	float stop, const SeriesReseed* rs, const SeriesRecover* sr);
+
+// A series recovery call (dev: device seeds and out): the counts go to recovered / remaining only when it succeeds, and a
+// device-pointer call returns after synchronising the stream.  On a group context the first member runs the host variants.
+static int series_recover_call(ocb_ctx* ctx, const char* what, bool dev, const RecoverMethod& m, const void* seeds, void* out, size_t n, float radius,
+	int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	SeriesStore ocb_ctx::*const which = m.dim == 2 ? &ocb_ctx::series2d : &ocb_ctx::series3d;
+	const SeriesStore* s = ctx ? &(exec_member(ctx)->*which) : nullptr;
+	const size_t frames = s && s->ref ? (size_t)s->frames : 0, rounds = max_rounds > 0 ? (size_t)max_rounds : 0;
+	std::vector<size_t> rec_counts(frames * rounds, 0), left(frames, 0);
+	const SeriesRecover sr{ radius, min_neighbors, zncc_high, zncc_low, max_rounds, rec_counts.data(), left.data() };
+	auto body = [&](ocb_ctx* x, const void* d_in, void* d_o) {
+		return m.dim == 2 ? icgn2d_series_recover_dev(x, what, m, d_in, d_o, n, sr)
+						  : icgn3d_series_dev(x, what, d_in, d_o, n, m.r[0], m.r[1], m.r[2], m.conv, m.stop, nullptr, &sr);
+	};
+	int rc;
+	if (dev) {
+		rc = body(ctx, seeds, out);
+		if (rc == OCB_OK && n) OCB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	} else {
+		const size_t floats = m.dim == 2 ? OCB_POI2D_FLOATS : OCB_POI3D_FLOATS;
+		rc = series_host(ctx, what, which, n, { seeds }, floats, { { out, floats } },
+			[&](ocb_ctx* x, const float* const* d_in, float* const* d_o) { return body(x, d_in[0], d_o[0]); });
+	}
+	if (rc != OCB_OK) return rc;
+	if (recovered && !rec_counts.empty()) memcpy(recovered, rec_counts.data(), rec_counts.size() * sizeof(size_t));
+	if (remaining && !left.empty()) memcpy(remaining, left.data(), left.size() * sizeof(size_t));
+	return OCB_OK;
+}
+
+int ocb_icgn2d_series_recover(ocb_ctx* ctx, int order, const void* seeds, void* out, size_t n, int rx, int ry, float conv, float stop, float radius,
+	int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	return series_recover_call(ctx, "icgn2d_series_recover", false, { 2, order == 1 ? 6 : (order == 2 ? 12 : 0), { rx, ry, 0 }, conv, stop }, seeds, out,
+		n, radius, min_neighbors, zncc_high, zncc_low, max_rounds, recovered, remaining);
+}
+int ocb_icgn2d_series_recover_dev(ocb_ctx* ctx, int order, const void* d_seeds, void* d_out, size_t n, int rx, int ry, float conv, float stop,
+	float radius, int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	OCB_NO_GROUP(ctx, "icgn2d_series_recover_dev");
+	return series_recover_call(ctx, "icgn2d_series_recover", true, { 2, order == 1 ? 6 : (order == 2 ? 12 : 0), { rx, ry, 0 }, conv, stop }, d_seeds,
+		d_out, n, radius, min_neighbors, zncc_high, zncc_low, max_rounds, recovered, remaining);
+}
+int ocb_icgn3d_series_recover(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop, float radius,
+	int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	return series_recover_call(ctx, "icgn3d_series_recover", false, { 3, 0, { rx, ry, rz }, conv, stop }, seeds, out, n, radius, min_neighbors,
+		zncc_high, zncc_low, max_rounds, recovered, remaining);
+}
+int ocb_icgn3d_series_recover_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop,
+	float radius, int min_neighbors, float zncc_high, float zncc_low, int max_rounds, size_t* recovered, size_t* remaining) {
+	OCB_NO_GROUP(ctx, "icgn3d_series_recover_dev");
+	return series_recover_call(ctx, "icgn3d_series_recover", true, { 3, 0, { rx, ry, rz }, conv, stop }, d_seeds, d_out, n, radius, min_neighbors,
+		zncc_high, zncc_low, max_rounds, recovered, remaining);
 }
 
 // ---- volume series: one reference volume, n_frames target volumes, each frame seeded by the previous one ------------------
@@ -2011,16 +2175,22 @@ int ocb_set_series_3d_u8(ocb_ctx* ctx, const unsigned char* ref, const unsigned 
 	});
 }
 
-// Checks and runs a volume series on a single-device context: device seeds and output; rs null for the plain series.  Per frame:
-// the target's prefilter, a copy of the previous frame's records and one LOAD launch; with rs, then a scan of that frame's
-// records (one synchronisation), and for its m lost POIs a rebuild, FFT-CC against the raw frame, IC-GN (COMPUTE) and a scatter.
+// Checks and runs a volume series on a single-device context: device seeds and output; rs and sr null for the plain series.  Per
+// frame: the target's prefilter, a copy of the previous frame's records and one LOAD launch; with rs, then a scan of that frame's
+// records (one synchronisation), and for its m lost POIs a rebuild, FFT-CC against the raw frame, IC-GN (COMPUTE) and a scatter;
+// with sr (series recovery), then the recovery rounds on that frame's records (recover_run), registered by IC-GN (COMPUTE) with the
+// series' gradient and coefficient volumes.
 static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv,
-	float stop, const SeriesReseed* rs) {
+	float stop, const SeriesReseed* rs, const SeriesRecover* sr) {
 	if (!ctx || ((!d_seeds || !d_out) && n) || rx < 1 || ry < 1 || rz < 1) return set_error(ctx, OCB_ERR_ARG, "%s: bad arguments", what);
 	const SeriesStore& s = ctx->series3d;
 	if (!s.ref) return set_error(ctx, OCB_ERR_STATE, "%s: no series set", what);
 	int rc;
 	if (rs && (rc = reseed_check(ctx, what, 3, *rs))) return rc;
+	const RecoverMethod method{ 3, 0, { rx, ry, rz }, conv, stop };
+	if (sr)
+		if (const char* refusal = recover_refusal(method, sr->zncc_high, sr->zncc_low, sr->max_rounds))
+			return set_error(ctx, OCB_ERR_ARG, "%s: %s", what, refusal);
 	if (n == 0) return OCB_OK;
 	const size_t rec = OCB_POI3D_FLOATS * sizeof(float);
 	if ((rc = series_size_check(ctx, what, n, s.frames, rec, false))) return rc;
@@ -2035,8 +2205,10 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 		|| (rc = grow(ctx, ctx->series3_tmp, elems * sizeof(float))) || (rc = grow(ctx, ctx->series3_cache, n * ocb::ICGN3D_SETUP_FLOATS * sizeof(float))))
 		return rc;
 	ReseedWs w;
-	if (rs && ((rc = reseed_workspace(ctx, n, F, 3, &w)) || (rc = grow(ctx, ctx->reseed_sub, n * rec)))) return rc;
-	float* const sub = rs ? ctx->reseed_sub.as<float>() : nullptr;
+	if (rs && (rc = reseed_workspace(ctx, n, F, 3, &w))) return rc;
+	const bool neutral = rs || sr; // the setup pass runs on neutral copies of the seeds (below)
+	if (neutral && (rc = grow(ctx, ctx->reseed_sub, n * rec))) return rc;
+	float* const sub = neutral ? ctx->reseed_sub.as<float>() : nullptr;
 	float4* const rg = ctx->series3_rg.as<float4>();
 	float* const coef = ctx->series3_coef.as<float>();
 	float* const tmp = ctx->series3_tmp.as<float>();
@@ -2056,14 +2228,16 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 	// subvolume lies inside the volume gets an entry, a seed the guard rejects included: re-seeded in frame f, such a POI
 	// reaches frame f + 1's LOAD with a good record.  The setup state depends only on the reference, the coordinates and the
 	// radii, so the entries of the POIs the plain series stores are the same; a POI without one (coordinates outside the
-	// volume or NaN) is still rejected by every guard.
+	// volume or NaN) is still rejected by every guard.  A recovering call stores them the same way: a POI accepted in frame f
+	// reaches frame f + 1's LOAD with a good record, whatever its seed.
 	if ((rc = launched(ctx, "gradient3d", ocb::gradient3d_launch(s.ref, rg, dx, dy, dz, ctx->sm_count, ctx->stream)))) return rc;
-	if (rs
-		&& ((rc = launched(ctx, "reseed_rebuild",
-				 ocb::reseed_rebuild_launch(3, (const float*)d_seeds, nullptr, nullptr, n, 0.f, nullptr, sub, ctx->sm_count, ctx->stream)))
-			|| (rc = launched(ctx, "reseed_anchor_init", ocb::reseed_anchor_init_launch(3, (const float*)d_seeds, n, w.anchor, ctx->sm_count, ctx->stream)))))
+	if (neutral
+		&& (rc = launched(ctx, "reseed_rebuild",
+				ocb::reseed_rebuild_launch(3, (const float*)d_seeds, nullptr, nullptr, n, 0.f, nullptr, sub, ctx->sm_count, ctx->stream))))
 		return rc;
-	if ((rc = icgn(rs ? sub : const_cast<float*>((const float*)d_seeds), n, ocb::ICGN3D_SETUP_STORE))) return rc;
+	if (rs && (rc = launched(ctx, "reseed_anchor_init", ocb::reseed_anchor_init_launch(3, (const float*)d_seeds, n, w.anchor, ctx->sm_count, ctx->stream))))
+		return rc;
+	if ((rc = icgn(neutral ? sub : const_cast<float*>((const float*)d_seeds), n, ocb::ICGN3D_SETUP_STORE))) return rc;
 	for (int f = 0; f < F; f++) {
 		if (u8) widen(f);
 		const float* const tar = u8 ? tmp : (const float*)frame(f);
@@ -2072,6 +2246,7 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 		const float* prev = f == 0 ? (const float*)d_seeds : q - n * OCB_POI3D_FLOATS;
 		OCB_CUDA(ctx, cudaMemcpyAsync(q, prev, n * rec, cudaMemcpyDeviceToDevice, ctx->stream));
 		if ((rc = icgn(q, n, ocb::ICGN3D_SETUP_LOAD))) return rc;
+		if (sr && (rc = series_recover_frame(ctx, method, ocb::Image2D{}, img, q, n, f, *sr, nullptr))) return rc;
 		if (!rs) continue;
 		if ((rc = launched(ctx, "reseed_scan",
 				 ocb::reseed_scan_launch(3, (const float*)d_out, n, f, f + 1, nullptr, n, rs->zncc_min, w.first, w.hist, ctx->sm_count, ctx->stream)))
@@ -2094,12 +2269,12 @@ static int icgn3d_series_dev(ocb_ctx* ctx, const char* what, const void* d_seeds
 static int icgn3d_series_host(ocb_ctx* ctx, const char* what, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop,
 	const SeriesReseed* rs) {
 	return series_host(ctx, what, &ocb_ctx::series3d, n, { seeds }, OCB_POI3D_FLOATS, { { out, OCB_POI3D_FLOATS } },
-		[&](ocb_ctx* x, const float* const* d_in, float* const* d_out) { return icgn3d_series_dev(x, what, d_in[0], d_out[0], n, rx, ry, rz, conv, stop, rs); });
+		[&](ocb_ctx* x, const float* const* d_in, float* const* d_out) { return icgn3d_series_dev(x, what, d_in[0], d_out[0], n, rx, ry, rz, conv, stop, rs, nullptr); });
 }
 
 int ocb_icgn3d_series_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out, size_t n, int rx, int ry, int rz, float conv, float stop) {
 	OCB_NO_GROUP(ctx, "icgn3d_series_dev");
-	return icgn3d_series_dev(ctx, "icgn3d_series", d_seeds, d_out, n, rx, ry, rz, conv, stop, nullptr);
+	return icgn3d_series_dev(ctx, "icgn3d_series", d_seeds, d_out, n, rx, ry, rz, conv, stop, nullptr, nullptr);
 }
 
 int ocb_icgn3d_series(ocb_ctx* ctx, const void* seeds, void* out, size_t n, int rx, int ry, int rz, float conv, float stop) {
@@ -2111,7 +2286,7 @@ int ocb_icgn3d_series_reseed_dev(ocb_ctx* ctx, const void* d_seeds, void* d_out,
 	OCB_NO_GROUP(ctx, "icgn3d_series_reseed_dev");
 	return series_reseed(ctx, &ocb_ctx::series3d, true, n, reseeded, [&](size_t* counts) {
 		const SeriesReseed rs{ { fft_rx, fft_ry, fft_rz }, zncc_min, counts };
-		return icgn3d_series_dev(ctx, "icgn3d_series_reseed", d_seeds, d_out, n, rx, ry, rz, conv, stop, &rs);
+		return icgn3d_series_dev(ctx, "icgn3d_series_reseed", d_seeds, d_out, n, rx, ry, rz, conv, stop, &rs, nullptr);
 	});
 }
 

@@ -305,6 +305,15 @@ cudaError_t recover_select_launch(int dim, const float* d_rec, size_t count, Rec
 // list2[k2] when src_idx is null) to idx2[k2].
 cudaError_t recover_move_launch(int dim, const float* d_src, const int* d_src_idx, size_t total, const int* d_list1, const int* d_count1, float* d_dst1,
 	float* d_q, const int* d_list2, float* d_dst2, int* d_idx2, int sm_count, cudaStream_t stream);
+// collect (the series recovery calls): d_out[k] = d_src_idx[d_list1[k]] for k < *d_count1 (<= total), the queue indices of a round's
+// accepted POIs in the order the move appends their records to the reliable set
+cudaError_t recover_collect_launch(const int* d_src_idx, size_t total, const int* d_list1, const int* d_count1, int* d_out, int sm_count,
+	cudaStream_t stream);
+// scan (the series recovery calls): as reseed_scan_launch, with the UNRELIABLE test (zncc_low, conv) in place of the lost test:
+// first[i] = the first frame in [f_begin, f_end) whose record of POI i is UNRELIABLE, or -1; hist[f] += the POIs whose first such
+// frame is f.  reseed_select_launch compacts its result.
+cudaError_t recover_scan_launch(int dim, const float* d_out, size_t n, int f_begin, int f_end, const int* d_idx, size_t m, float zncc_low, float conv,
+	int* d_first, int* d_hist, int sm_count, cudaStream_t stream);
 // nr2d.cu
 constexpr int NR2D_TILE_MARGIN = 1;
 __host__ __device__ inline int nr2d_tar_w(int rx) { return round_up4(2 * rx + 1 + 3 + 2 * NR2D_TILE_MARGIN + 4 + 3); }

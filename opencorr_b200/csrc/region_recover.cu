@@ -1,6 +1,8 @@
 // region_recover.cu -- the round bookkeeping of the recovery calls (ocb_icgn2d_recover, ocb_icgn3d_recover): split a registered
 // queue into its reliable and unreliable POIs, and after each round of RegionFit and IC-GN move the POIs that now pass into the
 // reliable set.  The fit and the registration run on the RegionFit and pair IC-GN kernels; these only select and move records.
+// The series recovery calls (ocb_icgn2d_series_recover, ocb_icgn3d_series_recover) add a scan for the frames that hold an
+// unreliable record and the collection of each round's accepted queue indices.
 //
 // Every selection is a stable cub::DeviceSelect::Flagged over the positions 0 .. count-1, its flag read straight from the records
 // (RecordTest), so the index lists come out in ascending order.  The comparisons are the literal float ones: a NaN ZNCC is neither
@@ -58,7 +60,36 @@ __global__ void recover_move_kernel(const float* __restrict__ src, const int* __
 	}
 }
 
+// One thread per position k of a round's working set: the queue index of its k-th accepted record, for k < *count1.
+__global__ void recover_collect_kernel(const int* __restrict__ src_idx, int total, const int* __restrict__ list1, const int* __restrict__ count1,
+	int* __restrict__ out) {
+	const int c1 = *count1;
+	for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < total && k < c1; k += gridDim.x * blockDim.x) out[k] = src_idx[list1[k]];
+}
+
+// One thread per POI of the range (idx[k], or k itself when idx is null) of a frame-major series of records (N floats each): first[i]
+// = its first frame in [f_begin, f_end) whose record is UNRELIABLE (RecordTest's literal comparisons), or -1; hist[f] counts the POIs
+// whose first such frame is f.
+template <int N, int ZNCC, int CONV>
+__global__ void recover_scan_kernel(const float* __restrict__ out, size_t n, int f_begin, int f_end, const int* __restrict__ idx, int m,
+	float zncc_low, float conv_max, int* __restrict__ first, int* __restrict__ hist) {
+	for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < m; k += gridDim.x * blockDim.x) {
+		const int i = idx ? idx[k] : k;
+		int hit = -1;
+		for (int f = f_begin; f < f_end; f++) {
+			const float* const r = out + ((size_t)f * n + i) * N;
+			if (r[ZNCC] < zncc_low || r[CONV] > conv_max) { hit = f; break; }
+		}
+		first[i] = hit;
+		if (hit >= 0) atomicAdd(hist + hit, 1);
+	}
+}
+
 constexpr int RECOVER_THREADS = 256;
+inline int recover_grid(long long work, int sm_count) {
+	const long long b = (work + RECOVER_THREADS - 1) / RECOVER_THREADS, cap = (long long)sm_count * 8;
+	return (int)(b < 1 ? 1 : (b > cap ? cap : b));
+}
 
 } // namespace
 
@@ -89,6 +120,24 @@ cudaError_t recover_move_launch(int dim, const float* d_src, const int* d_src_id
 	else
 		recover_move_kernel<P3_N><<<(int)grid, RECOVER_THREADS, 0, stream>>>(d_src, d_src_idx, (long long)total, d_list1, d_count1, d_dst1, d_q, d_list2,
 			d_dst2, d_idx2);
+	return cudaGetLastError();
+}
+
+cudaError_t recover_collect_launch(const int* d_src_idx, size_t total, const int* d_list1, const int* d_count1, int* d_out, int sm_count,
+	cudaStream_t stream) {
+	recover_collect_kernel<<<recover_grid((long long)total, sm_count), RECOVER_THREADS, 0, stream>>>(d_src_idx, (int)total, d_list1, d_count1, d_out);
+	return cudaGetLastError();
+}
+
+cudaError_t recover_scan_launch(int dim, const float* d_out, size_t n, int f_begin, int f_end, const int* d_idx, size_t m, float zncc_low, float conv,
+	int* d_first, int* d_hist, int sm_count, cudaStream_t stream) {
+	const int grid = recover_grid((long long)m, sm_count);
+	if (dim == 2)
+		recover_scan_kernel<P2_N, P2_ZNCC, P2_CONV><<<grid, RECOVER_THREADS, 0, stream>>>(d_out, n, f_begin, f_end, d_idx, (int)m, zncc_low, conv, d_first,
+			d_hist);
+	else
+		recover_scan_kernel<P3_N, P3_ZNCC, P3_CONV><<<grid, RECOVER_THREADS, 0, stream>>>(d_out, n, f_begin, f_end, d_idx, (int)m, zncc_low, conv, d_first,
+			d_hist);
 	return cudaGetLastError();
 }
 
